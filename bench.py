@@ -48,7 +48,7 @@ MASK_SIDE = 28
 METRIC = "Mask R-CNN R50-FPN training hot-path images/sec (custom-op path fwd+bwd, 2 images/GPU)"
 WORKLOAD = ("configs[2]: Mask R-CNN R50-FPN training hot path, 2 synthetic 3x800x1333 images per GPU: 2 x RPN batched_nms "
             "(8819 boxes), box ROIPooler fwd+bwd (1024 RoIs, 7x7), mask ROIPooler fwd+bwd (256 RoIs, 14x14), 13 DeformConv "
-            "layers of the R50 dconv c3-c5 variant fwd+bwd; fp32 tensors, deform-conv contraction in bf16x3 on tcgen05")
+            "layers of the R50 dconv c3-c5 variant fwd+bwd; fp32 tensors, deform-conv contraction in bf16x3 on wgmma")
 
 
 # ----------------------------------------------------------------------------------------- synthetic inputs
@@ -119,12 +119,6 @@ def tensors_of(d):
                 else:
                     yield from t
 
-
-# constants read off the committed ncu --set full capture of this step (profiles/r2_ncu_full.txt); sm__pipe_tensor_cycles_active
-# per kernel, res3 (C=128) / res4 (C=256) / res5 (C=512) layers
-R2_NCU = {"bwd_pair_dram_bytes": 57178624 + 99328 + 172992256 + 4922624,
-          "tensor_pipe_active_pct": {"dcn_fwd_tc_kernel": [16.0, 32.4, 40.0], "dcn_bwd_data_tc_kernel": [8.8, 17.5, 31.8],
-                                     "dcn_bwd_weight_cols_kernel": [44.6, 47.8, 51.2]}}
 
 E2E_HALF_KEYS = ("feats", "go_box", "go_mask", "dc_x", "dc_off", "dc_go")  # activations / gradients: bf16 under autocast
 
@@ -200,8 +194,8 @@ class TrainRunner:
 
     # -- stages (explicit ops: graph-capturable, no autograd bookkeeping)
     def rpn_nms(self, d):
-        # one call per image like the reference's loop (the two images' NMS in ONE call, `batched_nms_images_fixed`, measured
-        # slower on this step: 281 vs 254 us -- the kernels are latency chains per category, not throughput-bound)
+        # one call per image like the reference's loop (`batched_nms_images_fixed` runs the two images' NMS in ONE call; the
+        # kernels are latency chains per category, not throughput-bound)
         return [self.L.batched_nms_fixed(b, s, d["rpn_levels"], 0.7) for b, s in zip(d["rpn_boxes"], d["rpn_scores"])]
 
     def pool_fwd(self, d, which, feats=None):
@@ -514,6 +508,46 @@ class ClockSampler(threading.Thread):
                 "reasons": sorted(self.reasons)}
 
 
+DUMP_MAX_ELEMS = 1 << 17  # per array (512 KB as float32); a larger output is written as a fixed, seeded sample
+
+
+def dump_outputs(outs, out_dir):
+    """What one step of the timed path returned, as DIR/<name>.npy (float32; integer outputs as float64, exact below 2**53).
+    Arrays above DUMP_MAX_ELEMS elements are sampled at positions drawn from a generator seeded by the array's name, so two
+    builds run with the same arguments write the same elements."""
+    import zlib
+
+    import numpy as np
+
+    arrays = {}
+    for i, (keep, num) in enumerate(outs["keep"]):
+        arrays["rpn_keep_img%d" % i], arrays["rpn_num_kept_img%d" % i] = keep, num
+    arrays["box_pool"], arrays["mask_pool"] = outs["box"], outs["mask"]  # [K, C, P, P]: every RoI, sampled below
+    for l, g in enumerate(outs["gfeat"]):
+        arrays["feat_grad_p%d" % (l + 2)] = g
+    k = 0
+    for si, (c, _, _, layers) in enumerate(DCONV_STAGES):
+        for li in range(layers):
+            y, grads = outs["dc"][k]
+            k += 1
+            arrays["dconv_c%d_l%d_y" % (c, li)] = y
+            for name, g in zip(("grad_x", "grad_offset", "grad_mask", "grad_weight", "grad_bias"), grads):
+                if g is not None and g.numel():
+                    arrays["dconv_c%d_l%d_%s" % (c, li, name)] = g
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        a = t.detach().reshape(-1).cpu()
+        a = a.double() if not a.is_floating_point() else a.float()
+        if a.numel() > DUMP_MAX_ELEMS:
+            rng = np.random.default_rng(zlib.crc32(name.encode()))
+            a = a[torch.from_numpy(np.sort(rng.choice(a.numel(), DUMP_MAX_ELEMS, replace=False)))]
+        arr = a.numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
+        total += arr.nbytes
+    return total
+
+
 def graph_of(fn, stream):
     g = torch.cuda.CUDAGraph()
     with torch.cuda.stream(stream):
@@ -543,6 +577,8 @@ def main():
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -581,7 +617,7 @@ def main():
     sampler = ClockSampler(local_rank)
     sampler.start()  # started before warm-up so that NVML is initialised when the timed region begins
     runner = TrainRunner(dev)
-    NBUF = 2  # two input sets: 2 x 183 MB of features + 183 MB of gradients written per step, far beyond the 126 MB L2
+    NBUF = 2  # two input sets: 2 x 183 MB of features + 183 MB of gradients written per step, far beyond the 50 MB L2
     host = [make_train_inputs(sd) for sd in image_seeds(rank, NBUF)]
     devin = [runner.to_device(h) for h in host]
     torch.cuda.synchronize()
@@ -620,6 +656,8 @@ def main():
     barrier()
     sampler.active = False
     elapsed_ms = t_start.elapsed_time(t_end)
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(graph_outs[(args.steps - 1) % NBUF], args.dump_outputs)
     del graphs, graph_outs
 
     # ---------------- per-stage device time: each stage captured alone in its own graphs, rotating inputs
@@ -776,9 +814,9 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
-    tf_peak = peaks.get("bf16_tflops_sustained", 1400.0)  # the kernel is timed inside a long step
-    src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+    hbm = peaks.get("hbm_gbs", 3350.0)
+    tf_peak = peaks.get("bf16_tflops_sustained", 989.0)  # the kernel is timed inside a long step
+    src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet (700 W), not reached"
     # dominant kernels of the step: the deform-conv backward of the res3 stage (4 layers of 2 x 128 x 100 x 168)
     c, h, w, layers = DCONV_STAGES[0]
     bwd_ms = stage_ms["dconv_c128_bwd_x4"] / layers
@@ -808,22 +846,16 @@ def main():
         "clocks": sampler.summary(),
         "stages_ms": {k: round(v, 4) for k, v in stage_ms.items()},
         "validation": validation,
-        "l2": "two input sets rotate (2 x 183 MB of feature maps) and every step writes 183 MB of gradients: > 126 MB L2",
+        "l2": "two input sets rotate (2 x 183 MB of feature maps) and every step writes 183 MB of gradients: > 50 MB L2",
         "roofline": {"kernel": "deform-conv backward, R50 res3 layer (2 x 128 x 100 x 168): dcn_bwd_data_tc_kernel + "
                                "dcn_bwd_weight_cols_kernel (+ their operand pre-tiling / zero-fill / re-layout launches)",
                      "bound": "tensor", "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s", "frac": ach / tf_peak,
                      "peak_source": src + ", sustained bf16", "algorithmic_flops": flops_bwd, "avg_launch_ms": bwd_ms,
                      "note": "bf16x3 issues 3 MMAs per algorithmic product (fp32-class accuracy); the data-gradient kernel is bound "
                              "by the L2 vector reductions of its scatter (4 corners x 16 B per 4 channels and kernel point: %.0f MB "
-                             "per launch against the 5.9 TB/s red.v4 ceiling of profiles/r2_microbench.txt), see DESIGN.md section 4"
-                             % (IMGS_PER_GPU * h * w * 9 * c * 16 / 1e6),
+                             "per launch), see DESIGN.md section 4" % (IMGS_PER_GPU * h * w * 9 * c * 16 / 1e6),
                      "algorithmic_bytes": dconv_bwd_algorithmic_bytes(c, h, w, IMGS_PER_GPU),
-                     "achieved_hbm_gbs": gbs(dconv_bwd_algorithmic_bytes(c, h, w, IMGS_PER_GPU), bwd_ms),
-                     # DRAM bytes of the two kernels from the committed capture (profiles/r2_ncu_full.txt, launches 11 + 12:
-                     # dcn_bwd_data_tc_kernel 57.2 + 0.1 MB, dcn_bwd_weight_cols_kernel 173.0 + 4.9 MB -- the latter streams the
-                     # forward's saved columns back, 155 MB by design, instead of sampling x a second time)
-                     "traffic": R2_NCU["bwd_pair_dram_bytes"],
-                     "tensor_pipe_active_pct_ncu": R2_NCU["tensor_pipe_active_pct"]},
+                     "achieved_hbm_gbs": gbs(dconv_bwd_algorithmic_bytes(c, h, w, IMGS_PER_GPU), bwd_ms)},
         "roofline_other": {
             "roi_align_fwd_box_pooler": {"bound": "hbm", "algorithmic_bytes": box_alg_f, "avg_launch_ms": stage_ms["box_pool_fwd"],
                                          "achieved": gbs(box_alg_f, stage_ms["box_pool_fwd"]), "peak": hbm, "unit": "GB/s",

@@ -156,7 +156,7 @@ def has_cuda():
 
 
 def get_compiler_version():
-    return "nvcc (sm_100a)"
+    return "nvcc (sm_90a)"
 
 
 # --- the five pybind deform-conv entry points of detectron2._C (csrc/vision.cpp:90-102, deform_conv.h:116-375) -----------
@@ -165,7 +165,7 @@ def get_compiler_version():
 # im2col design that a fused implementation has no use for.  With this module bound as `detectron2._C`, the reference's own
 # `_DeformConv` / `_ModulatedDeformConv` autograd Functions run unchanged on our kernels (INTEGRATION.md).
 # Note the reference's argument order for DCNv1: kW, kH, dW, dH, padW, padH, dilW, dilH (width first, deform_conv.py:69-76).
-DCN_PRECISION = -1  # -1 auto (bf16x3 tcgen05 when the shape is taken, else fp32 FFMA); see include/d2b200.h
+DCN_PRECISION = -1  # -1 auto (bf16x3 wgmma when the shape is taken, else fp32 FFMA); see include/d2b200.h
 
 
 def _into(dst, src):

@@ -3,7 +3,7 @@
 
 D2B_API int d2b_abi_version(void) { return D2B_ABI_VERSION; }
 D2B_API int d2b_cuda_version(void) { return CUDART_VERSION; }
-D2B_API const char* d2b_arch(void) { return "sm_100a"; }
+D2B_API const char* d2b_arch(void) { return "sm_90a"; }
 
 // ---- several buffers zero-filled by ONE launch (gradient outputs of a backward call): a cudaMemsetAsync per buffer costs a
 // graph node / launch each, and most of these buffers are a few KB.  16-byte stores where alignment allows.
@@ -31,6 +31,18 @@ __global__ void __launch_bounds__(256) zero_buffers_kernel(const ZeroList z) {
   }
 }
 }  // namespace
+
+int d2b_num_sms() {
+  static std::atomic<int> cached[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;  // the launch that follows reports the error
+  int n = cached[dev].load(std::memory_order_relaxed);
+  if (n <= 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+    cached[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
 
 int d2b_zero_buffers(void* const* ptrs, const size_t* bytes, int n, cudaStream_t stream) {
   ZeroList z = {};

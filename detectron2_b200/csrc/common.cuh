@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels behind include/d2b200.h.
+// Shared helpers for the sm_90a kernels behind include/d2b200.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,7 +23,9 @@
 
 __host__ __device__ static inline int d2b_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-constexpr int kNumSMs = 148;  // B200
+// SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe): grid sizing in waves.  Queried once per device
+// ordinal and cached, so it costs no CUDA call inside a graph capture after the first eager call (abi.cu).
+int d2b_num_sms();
 
 // up to D2B_MAX_ZERO device buffers zero-filled by one launch (abi.cu); null / empty entries are skipped
 #define D2B_MAX_ZERO 8

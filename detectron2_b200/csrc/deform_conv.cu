@@ -1,4 +1,4 @@
-// Deformable convolution v1/v2 (DeformConv / ModulatedDeformConv) for sm_100a -- fp32 parity path.
+// Deformable convolution v1/v2 (DeformConv / ModulatedDeformConv) for sm_90a -- fp32 parity path.
 //
 // Replaces detectron2/layers/csrc/deformable/{deform_conv_cuda.cu, deform_conv_cuda_kernel.cu}.  The reference
 // materialises `columns[Cin*kh*kw, N*Ho*Wo]` in HBM (offset-im2col), then runs per-group addmm_ on it, and its backward
@@ -15,7 +15,7 @@
 // pixel): they are computed once per CTA tile into shared memory and reused by every channel, where the reference
 // recomputes them per channel (deform_conv_cuda_kernel.cu:238-287).
 //
-// The tcgen05 (bf16 / bf16x3) forward and backward live in deform_conv_tc.cu; this file is the fp32 FFMA path used for
+// The wgmma (bf16 / bf16x3) forward and backward live in deform_conv_tc.cu; this file is the fp32 FFMA path used for
 // parity (<= 1e-4 rel) and for shapes the tensor-core kernels do not take, plus the public entry points that pick one.
 #include "common.cuh"
 
@@ -386,7 +386,7 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
                                 float* grad_offset, float* grad_mask, float* grad_weight, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
-// precision: 0 = fp32 FFMA, 1 = bf16x3 on tcgen05, 2 = bf16 on tcgen05, -1 = auto (1 when the tensor-core kernels take
+// precision: 0 = fp32 FFMA, 1 = bf16x3 on wgmma, 2 = bf16 on wgmma, -1 = auto (1 when the tensor-core kernels take
 // the shape, else 0 -- both are fp32-class, so "auto" never lowers accuracy)
 D2B_API int d2b_deform_conv_tc_shape_supported(const d2b_dcn_params* p, int backward) {
   return backward ? d2b_deform_conv_tc_bwd_supported(p) : d2b_deform_conv_tc_supported(p);
@@ -467,10 +467,10 @@ D2B_API int d2b_deform_conv_backward(const float* x, const float* offset, const 
   if (grad_weight) D2B_CUDA(cudaMemsetAsync(grad_weight, 0, nw * 4, stream));
   if (d.N == 0) return D2B_OK;
   if (grad_x || grad_offset || grad_mask) {
-    // few pixel tiles (small maps) -> split the channel chunks over blockIdx.y so that the grid still fills 148 SMs;
+    // few pixel tiles (small maps) -> split the channel chunks over blockIdx.y so that the grid still fills the SMs;
     // grad_offset / grad_mask partial sums meet through the atomics the kernel already uses
     const int base_ctas = d2b_cdiv(d.HoWo, BN) * d.N * d.G;
-    int csplit = d2b_cdiv(3LL * kNumSMs, base_ctas);
+    int csplit = d2b_cdiv(3LL * d2b_num_sms(), base_ctas);
     const int nchunks = d2b_cdiv(d.cpg, BK);
     if (csplit > nchunks) csplit = nchunks;
     if (csplit < 1) csplit = 1;
@@ -482,9 +482,9 @@ D2B_API int d2b_deform_conv_backward(const float* x, const float* offset, const 
   if (grad_weight) {
     const int ptiles = d2b_cdiv(d.HoWo, BN), total = d.N * ptiles;
     const int n_ctile = d2b_cdiv(d.cpg, BK), n_mtile = d2b_cdiv(d.opg, BM);
-    // split the pixel reduction so that the grid is a few waves of 148 SMs
+    // split the pixel reduction so that the grid is a few waves of the SMs
     int per_tile_ctas = n_ctile * n_mtile * d.G;
-    int splits = d2b_cdiv(4LL * kNumSMs, per_tile_ctas);
+    int splits = d2b_cdiv(4LL * d2b_num_sms(), per_tile_ctas);
     if (splits > total) splits = total;
     if (splits < 1) splits = 1;
     const int tiles_per_cta = d2b_cdiv(total, splits);
@@ -500,7 +500,7 @@ D2B_API int d2b_deform_conv_backward(const float* x, const float* offset, const 
 // ---- conv2 of a DeformBottleneckBlock in one pass (SURVEY.md 8f-3; detectron2/modeling/backbone/resnet.py:305-318):
 //   offset_mask [N, 3*DG*kh*kw, Ho, Wo] is the raw output of conv2_offset -- the chunk / cat / sigmoid of :307-311 happen
 //   while the sampling taps are built;  y = relu(conv * scale + shift) -- FrozenBatchNorm folded to scale / shift, or
-//   scale = NULL and shift = bias -- happens in the TMEM epilogue.  Tensor-core precisions only.
+//   scale = NULL and shift = bias -- happens in the accumulator epilogue.  Tensor-core precisions only.
 D2B_API int d2b_deform_conv_fused_forward(const float* x, const float* offset_mask, const float* weight, const float* scale,
                                           const float* shift, int relu, const d2b_dcn_params* p, int precision, int flags,
                                           float* out, void* cols, void* workspace, size_t workspace_bytes, void* stream) {

@@ -1,12 +1,12 @@
-// Deformable convolution v1/v2 on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a: forward, backward-data
+// Deformable convolution v1/v2 on the Hopper tensor cores (wgmma), sm_90a: forward, backward-data
 // and backward-weight.  Replaces detectron2/layers/csrc/deformable/deform_conv_cuda.cu:272-444 (forward),
 // :446-642 / :985-1221 (backward input + offset + mask) and :644-824 (backward filter).
 //
 // The reference materialises columns[Cin*kh*kw, Ho*Wo] in HBM with a gather kernel and calls cuBLAS per group; its
 // backward materialises grad_columns, runs col2im / col2im_coord over them and re-runs im2col for the filter gradient.
-// Here no column buffer exists: every kernel is an implicit GEMM on tcgen05 whose gathered operand is produced (or whose
-// result is consumed) on the SM, with the operands that are plain matrices pre-tiled once into the UMMA shared-memory
-// image so that ONE linear TMA copy (cp.async.bulk) brings a whole operand tile.
+// Here no column buffer exists: every kernel is an implicit GEMM on wgmma whose gathered operand is produced (or whose
+// result is consumed) on the SM, with the operands that are plain matrices pre-tiled once into the wgmma shared-memory
+// image (128-byte swizzle) so that ONE linear TMA copy (cp.async.bulk) brings a whole operand tile.
 //
 //   K1 forward      D[128 px, oc]   = col[128 px, k'] . W[oc, k']^T        A = gather (K-major), B = weight tiles (TMA)
 //   K2 bwd data     gcol[128 px,k'] = gout[128 px, oc] . W[oc, k']          A = gout tiles (TMA), B = W^T tiles (TMA);
@@ -24,8 +24,10 @@
 //   * precision 1 ("bf16x3"): operands are split x = hi + lo (two bf16) and hi*hi + hi*lo + lo*hi is accumulated in fp32 --
 //     fp32-class accuracy (<= 1e-4 rel) at a third of the bf16 tensor peak.  precision 2: plain bf16 operands.
 //
-// Warp roles (576 threads, one CTA per SM): warps 0-15 gather / scatter / epilogue, warp 16 TMA producer (one lane),
-// warp 17 MMA issuer (one lane) and TMEM owner.
+// Warp roles (640 threads, one CTA per SM): warps 0-15 = four warpgroups that gather / scatter, issue the wgmma of their
+// quarter of the 128-row tile (rows 64 * (g & 1), columns (g >> 1) * BN / 2 of warpgroup g; fp32 accumulators in registers)
+// and run the epilogue; warp 16 TMA producer (one lane), warp 17 the forward's column saver.  The fifth warpgroup drops to
+// kSideRegs registers so that the workers get kWorkerRegs (setmaxnreg).
 #include <algorithm>
 #include <cstdlib>
 
@@ -36,11 +38,18 @@ using namespace d2b_tc;
 
 namespace {
 
-// 16 worker warps (112 registers each) measured faster than 8 warps with twice the loads in flight per lane (K1 res3 79 vs
-// 94 us, K2 132 vs 141 us): the gather / scatter loops are bound by instruction issue and need the warps, not deeper queues.
+// 16 worker warps: the gather / scatter loops are bound by instruction issue and need the warps, not deeper queues; four
+// warpgroups also give every quarter of the 128-row accumulator tile its own wgmma issuer.
 constexpr int kWorkerWarps = 16;
 constexpr int kWorkers = kWorkerWarps * 32;  // 512
-constexpr int kThreads = kWorkers + 64;      // + producer warp + MMA warp
+constexpr int kThreads = kWorkers + 128;     // + producer / saver warpgroup
+// setmaxnreg only moves registers inside the CTA's launch allocation: 640 threads launch with 96 registers each
+// (64 K / 640 rounded down to a multiple of 8), so the workers' raise must fit in what the side warpgroup gives back.
+constexpr int kLaunchRegs = (65536 / kThreads) & ~7;
+constexpr int kWorkerRegs = 112, kSideRegs = 24;
+static_assert(kWorkers * kWorkerRegs + (kThreads - kWorkers) * kSideRegs <= kThreads * kLaunchRegs,
+              "register budget exceeds the launch allocation");
+constexpr int kMaxBN = 128;                  // widest output-channel tile: 64 accumulator columns (32 registers) per warpgroup
 constexpr int kRowsPerHalf = 128 / (2 * kWorkerWarps);  // pixel rows of a 128-row tile owned by one half-warp: 4
 constexpr int kTile = 16384;                 // [128 rows][128 B]
 constexpr int kMaxSmem = 227 * 1024;
@@ -67,7 +76,7 @@ struct Epi {
   int relu;
 };
 
-struct K1P { int BN, noct, gspan, nkp, ksplit, S, tap_bytes, stage_bytes, red; };  // red: k-split partial sums meet through red.add
+struct K1P { int BN, noct, nkp, ksplit, S, tap_bytes, stage_bytes, red; };  // red: k-split partial sums meet through red.add
 struct K2P { int mper, msplit, tap_bytes; };
 struct K3P { int BN, noct, sper, nsplit, S, stage_bytes; };
 
@@ -119,14 +128,14 @@ const float* use_fused_offset_mask(TC& d, const float* offset_mask) {
   return offset_mask + (size_t)d.DG * 2 * d.KK * d.HoWo;
 }
 
-int largest_tile(int n) {  // largest of {256,...,16} dividing n
-  for (int t = 256; t >= 16; t >>= 1)
+int largest_tile(int n) {  // largest of {kMaxBN,...,16} dividing n
+  for (int t = kMaxBN; t >= 16; t >>= 1)
     if (n % t == 0) return t;
   return 0;
 }
 
 // Split `work` units of a CTA `base` times replicated over up to `max_split` parts: the number of parts that minimises
-// (waves over the 148 SMs) x (units per CTA + the CTA's fixed prologue / epilogue cost in units).  One CTA per SM is
+// (waves over the device's SMs) x (units per CTA + the CTA's fixed prologue / epilogue cost in units).  One CTA per SM is
 // resident, so 153 CTAs cost two full waves.
 int best_split(long long base, int work, int max_split, int overhead) {
   int best = 1;
@@ -134,7 +143,7 @@ int best_split(long long base, int work, int max_split, int overhead) {
   for (int s = 1; s <= max_split; ++s) {
     const int per = d2b_cdiv(work, s);
     const int parts = d2b_cdiv(work, per);
-    const long long cost = (long long)d2b_cdiv(base * parts, kNumSMs) * (per + overhead);
+    const long long cost = (long long)d2b_cdiv(base * parts, d2b_num_sms()) * (per + overhead);
     if (best_cost < 0 || cost < best_cost) {
       best_cost = cost;
       best = parts;
@@ -143,31 +152,20 @@ int best_split(long long base, int work, int max_split, int overhead) {
   return best;
 }
 
-int pow2_cols(int n) {
-  int c = 32;
-  while (c < n) c <<= 1;
-  return c;
-}
-
 bool plan_k1(const TC& d, K1P& k) {
-  if (d.ops <= 256) {
-    k.BN = d.ops; k.noct = 1;
-    k.gspan = std::max(1, std::min(d.SG, 256 / d.ops));
-    while (d.SG % k.gspan) --k.gspan;
-  } else {
-    k.BN = largest_tile(d.ops); k.noct = d.ops / k.BN; k.gspan = 1;
-  }
+  k.BN = largest_tile(d.ops);
   if (k.BN < 16) return false;
-  const int base = d.N * d.tiles_img * (d.SG / k.gspan) * k.noct;
+  k.noct = d.ops / k.BN;
+  const int base = d.N * d.tiles_img * d.SG * k.noct;
   k.ksplit = best_split(base, d.KK, d.KK, 1);
   k.nkp = d2b_cdiv(d.KK, k.ksplit);
   k.ksplit = d2b_cdiv(d.KK, k.nkp);
   k.red = k.ksplit > 1;
-  const int ndg = d.DG == 1 ? 1 : std::min(d.DG, d2b_cdiv(k.gspan * d.cps, d.cpdg) + 1);
+  const int ndg = d.DG == 1 ? 1 : std::min(d.DG, d2b_cdiv(d.cps, d.cpdg) + 1);
   k.tap_bytes = ndg * k.nkp * 128 * 16;
   k.stage_bytes = 2 * kTile + 2 * k.BN * 128;
   k.S = 3;
-  while (k.S > 1 && k.S * k.stage_bytes + k.tap_bytes + 1024 + 256 > kMaxSmem) --k.S;
+  while (k.S > 1 && k.S * k.stage_bytes + k.tap_bytes + 1024 + 128 > kMaxSmem) --k.S;
   return k.S >= 2;
 }
 
@@ -180,21 +178,21 @@ bool plan_k2(const TC& d, K2P& k) {
   const int nkp = std::min(d.KK, (2 * k.mper + d.cbs - 1) / d.cbs + 1);
   const int ndg = d.DG == 1 ? 1 : std::min(d.DG, d2b_cdiv(d.cps, d.cpdg) + 1);
   k.tap_bytes = ndg * nkp * 128 * 16;
-  return 2 * 4 * kTile + 128 * kGcolPitch * 4 + k.tap_bytes + 1024 + 256 <= kMaxSmem;
+  return 2 * 4 * kTile + 128 * kGcolPitch * 4 + k.tap_bytes + 1024 + 128 <= kMaxSmem;
 }
 
 bool plan_k3(const TC& d, K3P& k) {
+  if (d.ops % 64) return false;  // as K2: the backward takes whole 64-channel stages, so BN is 64 or 128
   k.BN = largest_tile(d.ops);
-  if (k.BN < 16) return false;
   k.noct = d.ops / k.BN;
   const int units = d.MC * d.SG * k.noct;
   const int total = d.N * d.stages_img;
-  k.nsplit = best_split(units, total, std::min(total, 4 * kNumSMs), 3);
+  k.nsplit = best_split(units, total, std::min(total, 4 * d2b_num_sms()), 3);
   k.sper = d2b_cdiv(total, k.nsplit);
   k.nsplit = d2b_cdiv(total, k.sper);
   k.stage_bytes = 2 * kTile + 2 * k.BN * 128;
   k.S = 3;
-  while (k.S > 1 && k.S * k.stage_bytes + 4096 + 1024 + 256 > kMaxSmem) --k.S;
+  while (k.S > 1 && k.S * k.stage_bytes + 4096 + 1024 + 128 > kMaxSmem) --k.S;
   return k.S >= 2;
 }
 
@@ -289,14 +287,57 @@ __device__ __forceinline__ void gather_store(const Taps4& t, int4 tap, uint8_t* 
   if (split) *reinterpret_cast<uint2*>(a_lo + off) = lo;
 }
 
+// ================================================================================================ wgmma helpers
+// Stage of a 128-row x BN tile: warpgroup g multiplies rows [64 (g & 1), +64) of A by columns [(g >> 1) BN / 2, +BN / 2)
+// of B over the stage's 64 k (four k16 steps); bf16x3 adds hi*lo and lo*hi.  A K-major: 16 k = 32 bytes along the swizzled
+// row; A MN-major (kTransA): 16 k = two 8-row atoms, 2048 bytes.
+template <int BN, int kTransA, int kSplit>
+__device__ __forceinline__ void mma_stage_(float (&acc)[BN / 4], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+  const int g = (threadIdx.x >> 7);
+  const uint32_t ao = kTransA ? (uint32_t)(g & 1) * 8192u : (uint32_t)(g & 1) * 64u * 128u;
+  const uint32_t bo = (uint32_t)(g >> 1) * (uint32_t)(BN / 2) * 128u;
+  const uint32_t lbo = kTransA ? 8192u : 0u;
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const uint32_t ak = ao + (kTransA ? (uint32_t)kk * 2048u : (uint32_t)kk * 32u), bk = bo + (uint32_t)kk * 32u;
+    Wgmma<BN / 2, kTransA>::mma(acc, wgmma_desc(a_hi + ak, lbo, 1024), wgmma_desc(b_hi + bk, 0, 1024), 1);
+    if (kSplit) {
+      Wgmma<BN / 2, kTransA>::mma(acc, wgmma_desc(a_hi + ak, lbo, 1024), wgmma_desc(b_lo + bk, 0, 1024), 1);
+      Wgmma<BN / 2, kTransA>::mma(acc, wgmma_desc(a_lo + ak, lbo, 1024), wgmma_desc(b_hi + bk, 0, 1024), 1);
+    }
+  }
+  wgmma_commit();
+}
+// The precision is chosen outside the wgmma sequence: a branch between the MMAs of one accumulator makes ptxas insert
+// warpgroup fences around each of them.
+template <int BN, int kTransA>
+__device__ __forceinline__ void mma_stage(float (&acc)[BN / 4], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                          int split) {
+  if (split) mma_stage_<BN, kTransA, 1>(acc, a_hi, a_lo, b_hi, b_lo);
+  else mma_stage_<BN, kTransA, 0>(acc, a_hi, a_lo, b_hi, b_lo);
+}
+
+// tile row / column of accumulator element i of this thread (see Wgmma in tc_common.cuh)
+template <int BN>
+__device__ __forceinline__ int acc_row(int i) {
+  const int t = threadIdx.x & 127;
+  return (threadIdx.x >> 7 & 1) * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + ((i >> 1) & 1) * 8;
+}
+template <int BN>
+__device__ __forceinline__ int acc_col(int i) {
+  return (threadIdx.x >> 8) * (BN / 2) + (i >> 2) * 8 + (threadIdx.x & 3) * 2 + (i & 1);
+}
+
 // ================================================================================================ K1: forward
-// grid (N * tiles_img, spans * oc tiles, k splits).  One more warp than K2 / K3: the SAVER, which (when the caller keeps the
+// grid (N * tiles_img, SG * oc tiles, k splits).  Warp 17 is the SAVER, which (when the caller keeps the
 // sampled columns for the weight gradient) copies every finished A stage -- already bf16 hi | lo in the tensor core's
 // swizzled tile layout -- to global memory with one bulk store, so that the backward streams the tiles back instead of
 // sampling x a second time (dcn_bwd_weight_cols_kernel).  Column tile of (image tile, super-group, unit): 16 KB hi [+ 16 KB lo].
-constexpr int kThreadsK1 = kThreads + 32;
-template <int kTmemCols>
-__global__ void __launch_bounds__(kThreadsK1, 1) dcn_fwd_tc_kernel(const float* __restrict__ xh,
+// The workers issue the MMAs of stage t right after gathering it and release stage t - 1 once its MMAs are done, so the
+// gather of a stage overlaps the MMAs of the previous one.
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __restrict__ xh,
                                                                    const float* __restrict__ offset,
                                                                    const float* __restrict__ mask,
                                                                    const uint8_t* __restrict__ wt, const Epi ep, const TC d,
@@ -308,50 +349,48 @@ __global__ void __launch_bounds__(kThreadsK1, 1) dcn_fwd_tc_kernel(const float* 
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(taps) + k.tap_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + k.S;
-  uint64_t* accum_bar = bars + 2 * k.S;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * k.S + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.x / d.tiles_img, p0 = (blockIdx.x - b * d.tiles_img) * 128;
-  const int span = blockIdx.y / k.noct, oct = blockIdx.y - span * k.noct;
-  const int sg0 = span * k.gspan;
+  const int sg = blockIdx.y / k.noct, oct = blockIdx.y - sg * k.noct;
   const int kp0 = blockIdx.z * k.nkp, nkp = min(d.KK, kp0 + k.nkp) - kp0;
-  const int nt = k.gspan * nkp * d.cbs;
-  const int dg0 = (sg0 * d.cps) / d.cpdg;
+  const int nt = nkp * d.cbs;
+  const int dg0 = (sg * d.cps) / d.cpdg;
   const bool saving = cols != nullptr && oct == 0;  // CTAs of the other output-channel tiles build the same columns
 
   if (tid == 0) {
     for (int s = 0; s < k.S; ++s) {
       mbar_init(&full_bar[s], kWorkerWarps + 1);
-      mbar_init(&empty_bar[s], saving ? 2 : 1);  // the tensor core is done with the stage [+ the saver has copied it out]
+      mbar_init(&empty_bar[s], kWorkerWarps + (saving ? 1 : 0));  // every worker warp's MMAs [+ the saver's copy] are done
     }
-    mbar_init(accum_bar, 1);
     mbar_init_fence();
   }
-  if (warp == kWorkerWarps + 1) tmem_alloc<kTmemCols>(tmem_slot);
   if (tid < kWorkers) {
-    const int ndg = ((sg0 + k.gspan) * d.cps - 1) / d.cpdg - dg0 + 1;
+    const int ndg = ((sg + 1) * d.cps - 1) / d.cpdg - dg0 + 1;
     for (int i = tid; i < ndg * nkp * 128; i += kWorkers) {
       const int row = i & 127, r = i >> 7;
       const int dgl = r / nkp, kpl = r - dgl * nkp;
       taps[i] = make_tap(d, offset, mask, b, dg0 + dgl, kp0 + kpl, p0 + row);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (warp < kWorkerWarps) reg_alloc<kWorkerRegs>();
+  else reg_dealloc<kSideRegs>();
 
   if (warp < kWorkerWarps) {
-    // =============================================================== GATHER: A tile [128 px][64 k'] K-major, hi + lo
+    // =============================================================== GATHER: A tile [128 px][64 k'] K-major, hi + lo; MMA
     const int half = lane >> 4, q = lane & 15;
     const float* __restrict__ ximg = xh + (size_t)b * d.H * d.W * d.Cin - (size_t)(d.W + 1) * d.Cin;  // biased: load_corners
     const uint32_t ucin = (uint32_t)d.Cin, urs = (uint32_t)(d.W * d.Cin);
-    int sgl = 0, kpl = 0, cb = 0;
-    for (int t = 0; t < nt; ++t) {
+    float acc[BN / 4];
+#pragma unroll
+    for (int i = 0; i < BN / 4; ++i) acc[i] = 0.f;
+    int kpl = 0, cb = 0;
+    // gather stage t, then issue its MMAs (one wgmma group)
+    auto stage = [&](int t) {
       const int s = t % k.S;
       const uint32_t par = (uint32_t)((t / k.S) & 1);
-      const int cbase = (sg0 + sgl) * d.cps + cb * 64;
+      const int cbase = sg * d.cps + cb * 64;
       const int4* __restrict__ tp = taps + ((cbase / d.cpdg - dg0) * nkp + kpl) * 128;
       const float* __restrict__ xc = ximg + cbase + q * 4;
       uint8_t* a_hi = smem + s * k.stage_bytes;
@@ -373,121 +412,76 @@ __global__ void __launch_bounds__(kThreadsK1, 1) dcn_fwd_tc_kernel(const float* 
       fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
       __syncwarp();
       if (lane == 0) mbar_arrive(&full_bar[s]);
-      if (++cb == d.cbs) {
-        cb = 0;
-        if (++kpl == nkp) { kpl = 0; ++sgl; }
-      }
+      mbar_wait(&full_bar[s], par);  // every warp's rows and the weight tile are in
+      const uint32_t sa = smem_u32(a_hi), sb = sa + 2 * kTile;
+      mma_stage<BN, 0>(acc, sa, sa + kTile, sb, sb + (uint32_t)BN * 128u, split);
+      if (++cb == d.cbs) { cb = 0; ++kpl; }
+    };
+    // The first stage is issued before the loop so that every pass through the loop head has exactly one wgmma group in
+    // flight; otherwise ptxas waits for it there and the gather of stage t no longer overlaps the MMAs of stage t - 1.
+    stage(0);
+    for (int t = 1; t < nt; ++t) {
+      stage(t);
+      wgmma_wait<1>();  // stage t - 1's MMAs are done: release it
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[(t - 1) % k.S]);
     }
-    // =============================================================== EPILOGUE: TMEM -> registers -> NCHW global
-    mbar_wait(accum_bar, 0u);
-    tc_fence_after();
-    const int quad = warp & 3, cgrp = warp >> 2;
-    const int row = quad * 32 + lane, p = p0 + row;
-    const bool pix_ok = p < d.HoWo;
-    const int ntot = k.gspan * k.BN;
-    const int oc0 = sg0 * d.ops + oct * k.BN;
+    wgmma_wait<0>();
+    // =============================================================== EPILOGUE: registers -> NCHW global
+    const int oc0 = sg * d.ops + oct * k.BN;
     const bool add_shift = ep.shift != nullptr && blockIdx.z == 0;
-    for (int c16 = cgrp; c16 * 16 < ntot; c16 += kWorkerWarps / 4) {
-      uint32_t r[16];
-      tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(c16 * 16), r);
-      tmem_ld_wait();
-      if (pix_ok) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int oc = oc0 + c16 * 16 + i;
-          float* dst = out + ((size_t)b * d.Cout + oc) * d.HoWo + p;
-          float v = __uint_as_float(r[i]);
-          if (k.red) {  // k-split partial sums: scale / relu run in dcn_epilogue_kernel once all partials are in
-            red_add(dst, v + ((add_shift && !ep.scale && !ep.relu) ? __ldg(ep.shift + oc) : 0.f));
-          } else {
-            if (ep.scale) v *= __ldg(ep.scale + oc);
-            if (ep.shift) v += __ldg(ep.shift + oc);
-            if (ep.relu) v = fmaxf(v, 0.f);
-            *dst = v;
-          }
-        }
+    for (int i = 0; i < BN / 4; ++i) {
+      const int p = p0 + acc_row<BN>(i);
+      if (p >= d.HoWo) continue;
+      const int oc = oc0 + acc_col<BN>(i);
+      float* dst = out + ((size_t)b * d.Cout + oc) * d.HoWo + p;
+      float v = acc[i];
+      if (k.red) {  // k-split partial sums: scale / relu run in dcn_epilogue_kernel once all partials are in
+        red_add(dst, v + ((add_shift && !ep.scale && !ep.relu) ? __ldg(ep.shift + oc) : 0.f));
+      } else {
+        if (ep.scale) v *= __ldg(ep.scale + oc);
+        if (ep.shift) v += __ldg(ep.shift + oc);
+        if (ep.relu) v = fmaxf(v, 0.f);
+        *dst = v;
       }
     }
   } else if (warp == kWorkerWarps) {
     // =============================================================== TMA producer: weight tile of every chunk
     if (lane == 0) {
       const uint32_t bytes = (uint32_t)(split ? 2 : 1) * (uint32_t)k.BN * 128u;
-      int sgl = 0, kpl = 0, cb = 0;
       for (int t = 0; t < nt; ++t) {
         const int s = t % k.S;
         const uint32_t par = (uint32_t)((t / k.S) & 1);
         mbar_wait(&empty_bar[s], par ^ 1u);
-        const size_t tile = ((size_t)((sg0 + sgl) * k.noct + oct) * d.U + (size_t)(kp0 + kpl) * d.cbs + cb);
+        const size_t tile = ((size_t)(sg * k.noct + oct) * d.U + (size_t)kp0 * d.cbs + t);
         mbar_arrive_expect_tx(&full_bar[s], bytes);
         bulk_g2s(smem + s * k.stage_bytes + 2 * kTile, wt + tile * (size_t)(2 * k.BN * 128), bytes, &full_bar[s]);
-        if (++cb == d.cbs) {
-          cb = 0;
-          if (++kpl == nkp) { kpl = 0; ++sgl; }
-        }
       }
     }
-  } else if (warp == kWorkerWarps + 2) {
+  } else if (warp == kWorkerWarps + 1) {
     // =============================================================== SAVER: finished A stages -> column tiles in global memory
     if (saving && lane == 0) {
       const uint32_t tile_bytes = (uint32_t)(split ? 2 : 1) * (uint32_t)kTile;
-      int sgl = 0, kpl = 0, cb = 0;
       for (int t = 0; t < nt; ++t) {
         const int s = t % k.S;
         const uint32_t par = (uint32_t)((t / k.S) & 1);
         mbar_wait(&full_bar[s], par);  // the workers' writes are fenced to the async proxy before they arrive
-        const size_t tile = ((size_t)blockIdx.x * d.SG + (sg0 + sgl)) * d.U + (size_t)(kp0 + kpl) * d.cbs + cb;
+        const size_t tile = ((size_t)blockIdx.x * d.SG + sg) * d.U + (size_t)kp0 * d.cbs + t;
         bulk_s2g(cols + tile * tile_bytes, smem + s * k.stage_bytes, tile_bytes);
         bulk_commit();
         bulk_wait_read0();
         mbar_arrive(&empty_bar[s]);
-        if (++cb == d.cbs) {
-          cb = 0;
-          if (++kpl == nkp) { kpl = 0; ++sgl; }
-        }
       }
       bulk_wait0();
     }
-  } else {
-    // =============================================================== MMA issuer
-    const uint32_t idesc = umma_idesc(k.BN, false, false);
-    const int per_sg = nkp * d.cbs;
-    for (int t = 0; t < nt; ++t) {
-      const int s = t % k.S;
-      const uint32_t par = (uint32_t)((t / k.S) & 1);
-      mbar_wait(&full_bar[s], par);
-      tc_fence_after();
-      if (lane == 0) {
-        const int sgl = t / per_sg;
-        const bool first = (t - sgl * per_sg) == 0;
-        const uint32_t a_hi = smem_u32(smem + s * k.stage_bytes), a_lo = a_hi + kTile;
-        const uint32_t b_hi = a_hi + 2 * kTile, b_lo = b_hi + (uint32_t)k.BN * 128u;
-        const uint32_t dcol = tmem_base + (uint32_t)(sgl * k.BN);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint32_t ko = (uint32_t)kk * 32u;  // 16 bf16 along K inside the swizzled row
-          umma_bf16(dcol, umma_desc(a_hi + ko, 0, 1024), umma_desc(b_hi + ko, 0, 1024), idesc, (!first || kk > 0) ? 1u : 0u);
-          if (split) {
-            umma_bf16(dcol, umma_desc(a_hi + ko, 0, 1024), umma_desc(b_lo + ko, 0, 1024), idesc, 1u);
-            umma_bf16(dcol, umma_desc(a_lo + ko, 0, 1024), umma_desc(b_hi + ko, 0, 1024), idesc, 1u);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (t == nt - 1) umma_commit(accum_bar);
-      }
-      __syncwarp();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWorkerWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
   }
 }
 
 // ================================================================================================ K2: backward data
 // grid (N * tiles_img, SG, macro-chunk splits).  Per macro-chunk (2 units = 128 k'): gcol[128 px][128] = gout . W over the
-// super-group's output channels (TMEM, double buffered), drained to shared memory, then scattered:
+// super-group's output channels (register accumulators of the four worker warpgroups, operand stages double buffered by
+// TMA), drained to shared memory, then scattered:
 //   grad_x   += gcol * mask * bilinear weight      (deform_conv_cuda_kernel.cu:313-362, :923-975) red.global.add.v4 (NHWC)
 //   grad_off += gcol * mask * d(sample)/d(h,w)     (:390-451, :977-1064)                           red.global.add
 //   grad_msk += gcol * sample                      (:1053-1064)
@@ -507,9 +501,6 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(taps) + k.tap_bytes);
   uint64_t* full_bar = bars;         // [2]
   uint64_t* empty_bar = bars + 2;    // [2]
-  uint64_t* acc_full = bars + 4;     // [2]
-  uint64_t* acc_empty = bars + 6;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.x / d.tiles_img, pt = blockIdx.x - b * d.tiles_img, p0 = pt * 128;
@@ -522,13 +513,10 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], kWorkerWarps);
+      mbar_init(&empty_bar[s], kWorkerWarps);
     }
     mbar_init_fence();
   }
-  if (warp == kWorkerWarps + 1) tmem_alloc<256>(tmem_slot);
   if (tid < kWorkers) {
     const int ndg = ((sg + 1) * d.cps - 1) / d.cpdg - dg0 + 1;
     for (int i = tid; i < ndg * nkp * 128; i += kWorkers) {
@@ -537,14 +525,12 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
       taps[i] = make_tap(d, offset, mask, b, dg0 + dgl, kp0 + kpl, p0 + row);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (warp < kWorkerWarps) reg_alloc<kWorkerRegs>();
+  else reg_dealloc<kSideRegs>();
 
   if (warp < kWorkerWarps) {
     const int half = lane >> 4, q = lane & 15;
-    const int quad = warp & 3, cq = warp >> 2;
     // both image pointers are biased by -(W + 1) pixels (see load_corners)
     const size_t img_off = (size_t)b * d.H * d.W * d.Cin - (size_t)(d.W + 1) * d.Cin;
     const float* __restrict__ ximg = xh + img_off;
@@ -611,27 +597,23 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
       const int buf = ml & 1;
       const int m = m0 + ml;
       const int nu = (2 * m + 1 < d.U) ? 2 : 1;
-      mbar_wait(&acc_full[buf], (uint32_t)((ml >> 1) & 1));
-      tc_fence_after();
-      // ---- drain: this warp's 32 TMEM lanes (pixels) x its share of the 128 columns -> gcol[px][col]
-      constexpr int kDrainCols = 128 / (kWorkerWarps / 4);
-      if (cq * kDrainCols < nu * 64) {
-        float* dst = gcol + (quad * 32 + lane) * kGcolPitch + cq * kDrainCols;
+      {  // ---- gcol tile on the tensor cores: 128 columns (the second unit's are zero when nu == 1), then drained to gcol[px][col]
+        float acc[32];
 #pragma unroll
-        for (int h4 = 0; h4 < kDrainCols / 16; ++h4) {
-          uint32_t r[16];
-          tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * 128 + cq * kDrainCols + h4 * 16), r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            *reinterpret_cast<float4*>(dst + h4 * 16 + i * 4) =
-                make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
-                            __uint_as_float(r[4 * i + 3]));
+        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+        for (int ks = 0; ks < d.nks; ++ks) {
+          const int c = ml * d.nks + ks, s = c & 1;
+          mbar_wait(&full_bar[s], (uint32_t)((c >> 1) & 1));
+          const uint32_t sa = smem_u32(smem + s * kStage);
+          mma_stage<128, 0>(acc, sa, sa + kTile, sa + 2 * kTile, sa + 3 * kTile, split);
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[s]);
         }
+#pragma unroll
+        for (int i = 0; i < 32; i += 2)
+          *reinterpret_cast<float2*>(gcol + acc_row<128>(i) * kGcolPitch + acc_col<128>(i)) = make_float2(acc[i], acc[i + 1]);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
       named_bar_sync(1, kWorkers);
       // ---- scatter
       for (int ul = 0; ul < nu; ++ul) {
@@ -668,7 +650,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
             const F2 LH = f2_pack(lh, lh), LW = f2_pack(lw, lw), HH = f2_pack(hh, hh), HW = f2_pack(hw, hw);
             const F2 W0 = f2_pack(w0, w0), W1 = f2_pack(w1, w1), W2 = f2_pack(w2, w2), W3 = f2_pack(w3, w3);
             const F2 MK = f2_pack(mk, mk);
-            // two channels per instruction (packed fp32): pair 0 = channels 0,1; pair 1 = channels 2,3
+            // channel pairs: pair 0 = channels 0,1; pair 1 = channels 2,3
             const F2 G[2] = {f2_pack(g4.x, g4.y), f2_pack(g4.z, g4.w)};
             const F2 A0[2] = {f2_pack(c[e].v0.x, c[e].v0.y), f2_pack(c[e].v0.z, c[e].v0.w)};
             const F2 A1[2] = {f2_pack(c[e].v1.x, c[e].v1.y), f2_pack(c[e].v1.z, c[e].v1.w)};
@@ -728,65 +710,19 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
         }
       }
     }
-  } else {
-    // =============================================================== MMA issuer
-    int c = 0;
-    for (int ml = 0; ml < nm; ++ml) {
-      const int buf = ml & 1;
-      const int m = m0 + ml;
-      const int ncols = (2 * m + 1 < d.U) ? 128 : 64;
-      const uint32_t idesc = umma_idesc(ncols, false, false);
-      mbar_wait(&acc_empty[buf], (uint32_t)(((ml >> 1) & 1) ^ 1));
-      tc_fence_after();
-      for (int ks = 0; ks < d.nks; ++ks, ++c) {
-        const int s = c & 1;
-        const uint32_t par = (uint32_t)((c >> 1) & 1);
-        mbar_wait(&full_bar[s], par);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t a_hi = smem_u32(smem + s * kStage), a_lo = a_hi + kTile, b_hi = a_hi + 2 * kTile, b_lo = b_hi + kTile;
-          const uint32_t dcol = tmem_base + (uint32_t)(buf * 128);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            const uint32_t ko = (uint32_t)kk * 32u;
-            umma_bf16(dcol, umma_desc(a_hi + ko, 0, 1024), umma_desc(b_hi + ko, 0, 1024), idesc, (ks > 0 || kk > 0) ? 1u : 0u);
-            if (split) {
-              umma_bf16(dcol, umma_desc(a_hi + ko, 0, 1024), umma_desc(b_lo + ko, 0, 1024), idesc, 1u);
-              umma_bf16(dcol, umma_desc(a_lo + ko, 0, 1024), umma_desc(b_hi + ko, 0, 1024), idesc, 1u);
-            }
-          }
-          umma_commit(&empty_bar[s]);
-          if (ks == d.nks - 1) umma_commit(&acc_full[buf]);
-        }
-        __syncwarp();
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWorkerWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
   }
 }
 
 // ================================================================================================ weight-gradient epilogue
 // The accumulator tile of a K3 CTA is [128 k' rows][BN oc]; in the weight tensor [Cout][Cin/G][KK] one unit's 64 rows are
 // 36 bytes apart (one kernel point of 64 channels), so writing it directly costs one 32-byte sector atomic per ELEMENT and
-// per pixel split.  Instead every CTA adds its tile with 16-byte vector reductions (64-byte row segments) into the zero-filled
-// staging matrix `part` [SG][MC*128][ops], and a small second kernel moves it into the weight tensor's layout.
-__device__ __forceinline__ void gw_tile_store(uint32_t tmem_base, int quad, int cgrp, int lane, int BN,
-                                              float* __restrict__ tile, int pitch) {
-  float* __restrict__ prow = tile + (size_t)(quad * 32 + lane) * pitch;
-  for (int c16 = cgrp; c16 * 16 < BN; c16 += kWorkerWarps / 4) {
-    uint32_t r[16];
-    tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(c16 * 16), r);
-    tmem_ld_wait();
+// per pixel split.  Instead every CTA adds its tile with 8-byte vector reductions (a thread's accumulator holds column pairs)
+// into the zero-filled staging matrix `part` [SG][MC*128][ops], and a small second kernel moves it into the weight tensor's
+// layout.
+template <int BN>
+__device__ __forceinline__ void gw_tile_store(const float (&acc)[BN / 4], float* __restrict__ tile, int pitch) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
-      red_add_v4(prow + c16 * 16 + i * 4, __uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]),
-                 __uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3]));
-  }
+  for (int i = 0; i < BN / 4; i += 2) red_add_v2(tile + (size_t)acc_row<BN>(i) * pitch + acc_col<BN>(i), acc[i], acc[i + 1]);
 }
 
 // one thread per (super-group, unit row, oc of the super-group); oc fastest: the reads of `part` are coalesced
@@ -837,8 +773,9 @@ __global__ void __launch_bounds__(256) dcn_gw_reduce_tile_kernel(const float* __
 
 // ================================================================================================ K3: backward weight
 // grid (M blocks = pairs of units, pixel splits, SG * oc tiles).  D[128 k'][BN oc] += col^T[128 k'][64 px] . gout[64 px][BN oc]
-// per 64-pixel stage; the gathered tile is written [unit half][pixel][64 ch] = MN-major for the tensor core.
-template <int kTmemCols>
+// per 64-pixel stage; the gathered tile is written [unit half][pixel][64 ch] = MN-major for the tensor core.  As in K1 the
+// workers issue the MMAs of a stage after gathering it and release the previous stage once its MMAs are done.
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const float* __restrict__ xh,
                                                                         const float* __restrict__ offset,
                                                                         const float* __restrict__ mask,
@@ -851,8 +788,6 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const fl
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(tap_s) + 4096);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + k.S;
-  uint64_t* accum_bar = bars + 2 * k.S;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * k.S + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mb = blockIdx.x;
@@ -863,16 +798,13 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const fl
   if (tid == 0) {
     for (int s = 0; s < k.S; ++s) {
       mbar_init(&full_bar[s], kWorkerWarps + 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kWorkerWarps);
     }
-    mbar_init(accum_bar, 1);
     mbar_init_fence();
   }
-  if (warp == kWorkerWarps + 1) tmem_alloc<kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (warp < kWorkerWarps) reg_alloc<kWorkerRegs>();
+  else reg_dealloc<kSideRegs>();
 
   if (warp < kWorkerWarps) {
     // =============================================================== GATHER: A tile [2 units][64 px][64 ch], hi + lo
@@ -902,7 +834,10 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const fl
       if (lane < 2 * PX) my_taps[lane] = tl_ok ? make_tap(d, offset, mask, b0, tl_dg, tl_kp, pb0 + warp * PX + tl_j) : make_int4(0, 0, 0, 0);
     }
     __syncwarp();
-    for (int i = 0; i < ns; ++i) {
+    float acc[BN / 4];
+#pragma unroll
+    for (int i = 0; i < BN / 4; ++i) acc[i] = 0.f;
+    auto stage = [&](int i) {  // gather stage i, then issue its MMAs
       const int s = i % k.S;
       const uint32_t par = (uint32_t)((i / k.S) & 1);
       int b, pbase, bn = 0, pbn = 0;
@@ -938,14 +873,20 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const fl
       fence_proxy_async();
       __syncwarp();
       if (lane == 0) mbar_arrive(&full_bar[s]);
+      mbar_wait(&full_bar[s], par);
+      const uint32_t sa = smem_u32(smem + s * k.stage_bytes), sb = sa + 2 * kTile;
+      mma_stage<BN, 1>(acc, sa, sa + kTile, sb, sb + (uint32_t)BN * 128u, split);
+    };
+    stage(0);  // as in K1: one wgmma group in flight at every pass through the loop head (ns >= 1 by construction)
+    for (int i = 1; i < ns; ++i) {
+      stage(i);
+      wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % k.S]);
     }
-    // =============================================================== EPILOGUE: TMEM [k' row][oc col] -> this split's partial tile
-    mbar_wait(accum_bar, 0u);
-    tc_fence_after();
-    const int quad = warp & 3, cgrp = warp >> 2;
-    gw_tile_store(tmem_base, quad, cgrp, lane, k.BN,
-                  gw + ((size_t)sg * d.MC * 128 + (size_t)mb * 128) * d.ops + (size_t)oct * k.BN,
-                  d.ops);
+    wgmma_wait<0>();
+    // =============================================================== EPILOGUE: registers [k' row][oc col] -> this split's partial tile
+    gw_tile_store<BN>(acc, gw + ((size_t)sg * d.MC * 128 + (size_t)mb * 128) * d.ops + (size_t)oct * k.BN, d.ops);
   } else if (warp == kWorkerWarps) {
     if (lane == 0) {
       const uint32_t bytes = (uint32_t)(split ? 2 : 1) * (uint32_t)k.BN * 128u;
@@ -958,48 +899,14 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const fl
         bulk_g2s(smem + s * k.stage_bytes + 2 * kTile, gt + tile * (size_t)(2 * k.BN * 128), bytes, &full_bar[s]);
       }
     }
-  } else {
-    const uint32_t idesc = umma_idesc(k.BN, true, false);
-    for (int i = 0; i < ns; ++i) {
-      const int s = i % k.S;
-      const uint32_t par = (uint32_t)((i / k.S) & 1);
-      mbar_wait(&full_bar[s], par);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_hi = smem_u32(smem + s * k.stage_bytes), a_lo = a_hi + kTile;
-        const uint32_t b_hi = a_hi + 2 * kTile, b_lo = b_hi + (uint32_t)k.BN * 128u;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          // A: 16 pixels (K) = two 8-row atoms 1024 B apart; the two 64-channel M blocks are 8192 B apart
-          const uint32_t ao = (uint32_t)kk * 2048u, bo = (uint32_t)kk * 32u;
-          umma_bf16(tmem_base, umma_desc(a_hi + ao, 8192, 1024), umma_desc(b_hi + bo, 0, 1024), idesc, (i > 0 || kk > 0) ? 1u : 0u);
-          if (split) {
-            umma_bf16(tmem_base, umma_desc(a_hi + ao, 8192, 1024), umma_desc(b_lo + bo, 0, 1024), idesc, 1u);
-            umma_bf16(tmem_base, umma_desc(a_lo + ao, 8192, 1024), umma_desc(b_hi + bo, 0, 1024), idesc, 1u);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (i == ns - 1) umma_commit(accum_bar);
-      }
-      __syncwarp();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWorkerWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
   }
 }
 
 // ================================================================================================ K3c: backward weight from saved columns
 // Same grid, tiles and epilogue as K3, but the A operand is streamed back from the column tiles the forward saved
-// (dcn_fwd_tc_kernel's saver warp) instead of being sampled from x again: a pure TMA -> tcgen05 pipeline.  A 64-pixel stage of
+// (dcn_fwd_tc_kernel's saver warp) instead of being sampled from x again: a pure TMA -> wgmma pipeline.  A 64-pixel stage of
 // a unit is one contiguous 8 KB half of its [128 px][64 ch] tile (the 128-byte swizzle repeats every 8 rows).
-// (Measured: multicasting the shared grad_out tile over clusters of 2 along the macro-chunk axis changes nothing -- the kernel
-// is bound by the three tcgen05 passes of the bf16x3 split and the column stream, not by L2 reads -- and clusters of 3 / 6 do
-// not fit the one-wave grid, 135 / 132 resident CTAs; the kernel therefore runs without clusters.)
-template <int kTmemCols>
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const uint8_t* __restrict__ cols,
                                                                           const uint8_t* __restrict__ gt, const TC d,
                                                                           const K3P k, const int S, const int split,
@@ -1009,8 +916,6 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * k.stage_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + S;
-  uint64_t* accum_bar = bars + 2 * S;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mb = blockIdx.x;
@@ -1022,12 +927,10 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const 
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kWorkerWarps);
     }
-    mbar_init(accum_bar, 1);
     mbar_init_fence();
   }
-  if (warp == kWorkerWarps + 1) tmem_alloc<kTmemCols>(tmem_slot);
   if (nu == 1 && tid < kWorkers) {  // odd unit count: the second 64 rows of A are never loaded; keep them finite
     for (int s = 0; s < S; ++s)
       for (int i = tid; i < 2 * 512; i += kWorkers) {
@@ -1036,19 +939,30 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const 
       }
     fence_proxy_async();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (warp < kWorkerWarps) reg_alloc<kWorkerRegs>();
+  else reg_dealloc<kSideRegs>();
 
   if (warp < kWorkerWarps) {
-    // =============================================================== EPILOGUE: TMEM [k' row][oc col] -> this split's partial tile
-    mbar_wait(accum_bar, 0u);
-    tc_fence_after();
-    const int quad = warp & 3, cgrp = warp >> 2;
-    gw_tile_store(tmem_base, quad, cgrp, lane, k.BN,
-                  gw + ((size_t)sg * d.MC * 128 + (size_t)mb * 128) * d.ops + (size_t)oct * k.BN,
-                  d.ops);
+    // =============================================================== MMA (as K3), then registers -> this split's partial tile
+    float acc[BN / 4];
+#pragma unroll
+    for (int i = 0; i < BN / 4; ++i) acc[i] = 0.f;
+    auto issue = [&](int i) {
+      const int s = i % S;
+      mbar_wait(&full_bar[s], (uint32_t)((i / S) & 1));
+      const uint32_t sa = smem_u32(smem + s * k.stage_bytes), sb = sa + 2 * kTile;
+      mma_stage<BN, 1>(acc, sa, sa + kTile, sb, sb + (uint32_t)BN * 128u, split);
+    };
+    issue(0);  // as in K1: one wgmma group in flight at every pass through the loop head
+    for (int i = 1; i < ns; ++i) {
+      issue(i);
+      wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+    }
+    wgmma_wait<0>();
+    gw_tile_store<BN>(acc, gw + ((size_t)sg * d.MC * 128 + (size_t)mb * 128) * d.ops + (size_t)oct * k.BN, d.ops);
   } else if (warp == kWorkerWarps) {
     // =============================================================== TMA producer: column halves + grad_out tile per stage
     if (lane == 0) {
@@ -1072,37 +986,6 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const 
         bulk_g2s(stage + 2 * kTile, gt + tile * (size_t)(2 * k.BN * 128), gbytes, &full_bar[s]);
       }
     }
-  } else {
-    // =============================================================== MMA issuer (as K3)
-    const uint32_t idesc = umma_idesc(k.BN, true, false);
-    for (int i = 0; i < ns; ++i) {
-      const int s = i % S;
-      const uint32_t par = (uint32_t)((i / S) & 1);
-      mbar_wait(&full_bar[s], par);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_hi = smem_u32(smem + s * k.stage_bytes), a_lo = a_hi + kTile;
-        const uint32_t b_hi = a_hi + 2 * kTile, b_lo = b_hi + (uint32_t)k.BN * 128u;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint32_t ao = (uint32_t)kk * 2048u, bo = (uint32_t)kk * 32u;
-          umma_bf16(tmem_base, umma_desc(a_hi + ao, 8192, 1024), umma_desc(b_hi + bo, 0, 1024), idesc, (i > 0 || kk > 0) ? 1u : 0u);
-          if (split) {
-            umma_bf16(tmem_base, umma_desc(a_hi + ao, 8192, 1024), umma_desc(b_lo + bo, 0, 1024), idesc, 1u);
-            umma_bf16(tmem_base, umma_desc(a_lo + ao, 8192, 1024), umma_desc(b_hi + bo, 0, 1024), idesc, 1u);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (i == ns - 1) umma_commit(accum_bar);
-      }
-      __syncwarp();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWorkerWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
   }
 }
 
@@ -1189,7 +1072,7 @@ __global__ void __launch_bounds__(256) dcn_gout_px_tiles_kernel(const float* __r
                                                                 uint8_t* __restrict__ dst, uint8_t* __restrict__ dst_oc,
                                                                 int BN, int noct) {
   // grid (tiles, 4): a CTA converts 32 of the tile's 128 pixel rows -- 4x the CTAs of a tile-per-CTA layout, which matters for
-  // the small maps (res5: 144 tiles on 148 SMs)
+  // the small maps (res5: 144 tiles on an H100 SXM's 132 SMs)
   __shared__ float t[64][33];
   const long long tile = blockIdx.x;
   const int ks = (int)(tile % d.nks);
@@ -1377,21 +1260,20 @@ int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float*
     D2B_CHECK_LAUNCH();
   }
   if (k.red) D2B_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)d.N * d.Cout * d.HoWo, stream));
-  const int smem_bytes = k.S * k.stage_bytes + k.tap_bytes + 1024 + 256;
-  const int tcols = pow2_cols(k.gspan * k.BN);
+  const int smem_bytes = k.S * k.stage_bytes + k.tap_bytes + 1024 + 128;
   const int split = precision == 1 ? 1 : 0;
   const Epi ep = {scale, shift, relu};
-  dim3 grid(d.N * d.tiles_img, (d.SG / k.gspan) * k.noct, k.ksplit);
-#define D2B_LAUNCH_K1(COLS)                                                                                            \
+  dim3 grid(d.N * d.tiles_img, d.SG * k.noct, k.ksplit);
+#define D2B_LAUNCH_K1(BN)                                                                                              \
   {                                                                                                                    \
-    D2B_ALLOW_BIG_SMEM(dcn_fwd_tc_kernel<COLS>);                                                                       \
-    dcn_fwd_tc_kernel<COLS><<<grid, kThreadsK1, smem_bytes, stream>>>(xh, offset, mask, wt, ep, d, k, split, out,      \
-                                                                      reinterpret_cast<uint8_t*>(cols));               \
+    D2B_ALLOW_BIG_SMEM(dcn_fwd_tc_kernel<BN>);                                                                         \
+    dcn_fwd_tc_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(xh, offset, mask, wt, ep, d, k, split, out,        \
+                                                                    reinterpret_cast<uint8_t*>(cols));                 \
   }
-  if (tcols <= 32) D2B_LAUNCH_K1(32)
-  else if (tcols == 64) D2B_LAUNCH_K1(64)
-  else if (tcols == 128) D2B_LAUNCH_K1(128)
-  else D2B_LAUNCH_K1(256)
+  if (k.BN == 16) D2B_LAUNCH_K1(16)
+  else if (k.BN == 32) D2B_LAUNCH_K1(32)
+  else if (k.BN == 64) D2B_LAUNCH_K1(64)
+  else D2B_LAUNCH_K1(128)
 #undef D2B_LAUNCH_K1
   D2B_CHECK_LAUNCH();
   if (k.red && (scale || relu)) {
@@ -1501,7 +1383,7 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
       dcn_wtile_bwd_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(weight, d, wt);
       D2B_CHECK_LAUNCH();
     }
-    const int smem_bytes = 2 * 4 * kTile + 128 * kGcolPitch * 4 + k2.tap_bytes + 1024 + 256;
+    const int smem_bytes = 2 * 4 * kTile + 128 * kGcolPitch * 4 + k2.tap_bytes + 1024 + 128;
     D2B_ALLOW_BIG_SMEM(dcn_bwd_data_tc_kernel);
     dim3 grid(d.N * d.tiles_img, d.SG, k2.msplit);
     dcn_bwd_data_tc_kernel<<<grid, kThreads, smem_bytes, stream>>>(xh, offset, mask, gt_px, wt, d, k2, split, gxh, grad_offset,
@@ -1519,33 +1401,28 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
       dcn_gout_oc_tiles_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(grad_out, y_saved, ep, d, k3.BN, k3.noct, gt_oc);
       D2B_CHECK_LAUNCH();
     }
-    const int tcols = pow2_cols(k3.BN);
     dim3 grid(d.MC, k3.nsplit, d.SG * k3.noct);
     if (cols) {  // the forward kept its sampled columns: stream them back (no second pass over x)
       const int S = std::min(6, (kMaxSmem - 2048) / k3.stage_bytes);
-      const int smem_bytes = S * k3.stage_bytes + 1024 + 256;
+      const int smem_bytes = S * k3.stage_bytes + 1024 + 128;
       const uint8_t* cl = reinterpret_cast<const uint8_t*>(cols);
-#define D2B_LAUNCH_K3C(COLS)                                                                                             \
+#define D2B_LAUNCH_K3C(BN)                                                                                             \
   {                                                                                                                      \
-    D2B_ALLOW_BIG_SMEM(dcn_bwd_weight_cols_kernel<COLS>);                                                                \
-    dcn_bwd_weight_cols_kernel<COLS><<<grid, kThreads, smem_bytes, stream>>>(cl, gt_oc, d, k3, S, split, gw_part);       \
+    D2B_ALLOW_BIG_SMEM(dcn_bwd_weight_cols_kernel<BN>);                                                                \
+    dcn_bwd_weight_cols_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(cl, gt_oc, d, k3, S, split, gw_part);       \
   }
-      if (tcols <= 32) D2B_LAUNCH_K3C(32)
-      else if (tcols == 64) D2B_LAUNCH_K3C(64)
-      else if (tcols == 128) D2B_LAUNCH_K3C(128)
-      else D2B_LAUNCH_K3C(256)
+      if (k3.BN == 64) D2B_LAUNCH_K3C(64)
+      else D2B_LAUNCH_K3C(128)
 #undef D2B_LAUNCH_K3C
     } else {
-      const int smem_bytes = k3.S * k3.stage_bytes + 4096 + 1024 + 256;
-#define D2B_LAUNCH_K3(COLS)                                                                                              \
+      const int smem_bytes = k3.S * k3.stage_bytes + 4096 + 1024 + 128;
+#define D2B_LAUNCH_K3(BN)                                                                                              \
   {                                                                                                                      \
-    D2B_ALLOW_BIG_SMEM(dcn_bwd_weight_tc_kernel<COLS>);                                                                  \
-    dcn_bwd_weight_tc_kernel<COLS><<<grid, kThreads, smem_bytes, stream>>>(xh, offset, mask, gt_oc, d, k3, split, gw_part); \
+    D2B_ALLOW_BIG_SMEM(dcn_bwd_weight_tc_kernel<BN>);                                                                  \
+    dcn_bwd_weight_tc_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(xh, offset, mask, gt_oc, d, k3, split, gw_part); \
   }
-      if (tcols <= 32) D2B_LAUNCH_K3(32)
-      else if (tcols == 64) D2B_LAUNCH_K3(64)
-      else if (tcols == 128) D2B_LAUNCH_K3(128)
-      else D2B_LAUNCH_K3(256)
+      if (k3.BN == 64) D2B_LAUNCH_K3(64)
+      else D2B_LAUNCH_K3(128)
 #undef D2B_LAUNCH_K3
     }
     D2B_CHECK_LAUNCH();

@@ -1,4 +1,4 @@
-// NMS (axis-aligned + rotated) and pairwise rotated-box IoU for sm_100a.
+// NMS (axis-aligned + rotated) and pairwise rotated-box IoU for sm_90a.
 //
 // Replaces torchvision::nms as reached from detectron2/layers/nms.py:5-22, and
 // detectron2/layers/csrc/{nms_rotated/nms_rotated_cuda.cu, box_iou_rotated/box_iou_rotated_cuda.cu}.
@@ -740,7 +740,7 @@ D2B_API int d2b_nms(const float* boxes, const float* scores, const int64_t* idxs
   D2B_CHECK_LAUNCH();
   // 3. per-segment greedy scans in parallel + compaction in global score order by the last CTA
   D2B_ALLOW_BIG_SMEM(nms_scan_kernel);
-  const int scan_grid = idxs ? (m < 2 * kNumSMs ? m : 2 * kNumSMs) : 1;
+  const int scan_grid = idxs ? (m < 2 * d2b_num_sms() ? m : 2 * d2b_num_sms()) : 1;
   nms_scan_kernel<<<scan_grid, kScanThreads, smem, stream>>>(w.maskT, w.grank_of_pos, w.orig_of_grank, w.seg_start, w.seg_end,
                                                              w.ctrl, m, w.wcap, w.keepflag, (long long*)keep, (long long*)num_keep);
   D2B_CHECK_LAUNCH();

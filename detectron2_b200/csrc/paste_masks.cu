@@ -1,4 +1,4 @@
-// paste_masks_in_image for sm_100a -- one fused kernel instead of the reference's
+// paste_masks_in_image for sm_90a -- one fused kernel instead of the reference's
 // meshgrid + grid_sample + compare + copy chain (detectron2/layers/mask_ops.py:17-69,74-147).
 //
 // HBM-bound byte kernel: the output (N*H*W bytes) dominates.  Most of every plane cannot see its mask and is written
@@ -323,7 +323,7 @@ D2B_API int d2b_paste_masks_packed(const float* masks, const float* boxes, int N
   const int Ww = d2b_cdiv(W, 32);
   const long long words = (long long)H * Ww;
   if ((long long)H * W >= (1LL << 30)) return D2B_EUNSUPPORTED;
-  int gx = (int)std::min<long long>(d2b_cdiv(words, kThreads), std::max<long long>(1, d2b_cdiv(16LL * kNumSMs, N)));
+  int gx = (int)std::min<long long>(d2b_cdiv(words, kThreads), std::max<long long>(1, d2b_cdiv(16LL * d2b_num_sms(), N)));
   paste_masks_packed_kernel<<<dim3(gx, N), kThreads, 0, (cudaStream_t)stream>>>(masks, boxes, M, H, W, Ww, threshold, out);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
@@ -339,13 +339,13 @@ D2B_API int d2b_paste_masks(const float* masks, const float* boxes, int N, int M
   int chunks = (int)((plane + kPix - 1) / kPix);  // upper bound; chunks past the plane are skipped in-kernel
   const size_t tab_bytes = sizeof(float) * ((size_t)W + (size_t)H + 2);
   const bool tab = W >= 2 * kPix && tab_bytes <= 30 * 1024;  // 16 KB static mask + tables inside the default 48 KB; one-wrap rows
-  const int total = 8 * kNumSMs;
+  const int total = 8 * d2b_num_sms();
   if (2 * N <= total) {  // balanced: CTAs handed to the masks in proportion to their work (decided in-kernel from the boxes)
     if (tab) paste_masks_kernel<true><<<total, kThreads, tab_bytes, (cudaStream_t)stream>>>(masks, boxes, M, H, W, threshold, out, N, 1);
     else paste_masks_kernel<false><<<total, kThreads, 0, (cudaStream_t)stream>>>(masks, boxes, M, H, W, threshold, out, N, 1);
   } else {  // many masks: a fixed, small number of CTAs each
     int gx = d2b_cdiv(chunks + 1, kThreads);
-    int want = d2b_cdiv(8LL * kNumSMs, N);
+    int want = d2b_cdiv(8LL * d2b_num_sms(), N);
     if (gx > want) gx = want < 1 ? 1 : want;
     dim3 grid(gx, N);
     if (tab) paste_masks_kernel<true><<<grid, kThreads, tab_bytes, (cudaStream_t)stream>>>(masks, boxes, M, H, W, threshold, out, N, 0);

@@ -1,4 +1,4 @@
-// RoIAlign / ROIAlignRotated forward + backward for sm_100a.
+// RoIAlign / ROIAlignRotated forward + backward for sm_90a.
 //
 // Semantics follow torchvision roi_align (detectron2/layers/roi_align.py:58-65; arithmetic as in
 // torchvision/ops/roi_align.py::_roi_align) and detectron2/layers/csrc/ROIAlignRotated/ROIAlignRotated_cuda.cu:143-323.
@@ -738,7 +738,7 @@ static int launch_fwd(const Pyr& P, const float* rois, int K, int C, int PH, int
   else D2B_ALLOW_BIG_SMEM(roi_align_v3_kernel<false>);
   const int ngroup = d2b_cdiv(C, kChW);
   int groups_per_cta = ngroup;  // split the channel groups until the grid is several waves deep
-  while (groups_per_cta > kV3Warps && (long long)K * d2b_cdiv(ngroup, groups_per_cta) < 24LL * kNumSMs)
+  while (groups_per_cta > kV3Warps && (long long)K * d2b_cdiv(ngroup, groups_per_cta) < 24LL * d2b_num_sms())
     groups_per_cta = (groups_per_cta + 1) / 2;
   dim3 grid(K, d2b_cdiv(ngroup, groups_per_cta));
   if (gout) roi_align_v3_kernel<true><<<grid, kV3Threads, smem, stream>>>(P, rois, C, PH, PW, sr, aligned, groups_per_cta, gout, nullptr);
@@ -747,10 +747,10 @@ static int launch_fwd(const Pyr& P, const float* rois, int K, int C, int PH, int
   return D2B_OK;
 }
 
-// channels per CTA: enough CTAs to fill 148 SMs a few times over without shrinking the per-CTA tap reuse.
+// channels per CTA: enough CTAs to fill the SMs a few times over without shrinking the per-CTA tap reuse.
 int pick_c_per_cta(int K, int C) {
   int cpc = C;
-  while (cpc > 16 && (long long)K * d2b_cdiv(C, cpc) < 4LL * kNumSMs) cpc = (cpc + 1) / 2;
+  while (cpc > 16 && (long long)K * d2b_cdiv(C, cpc) < 4LL * d2b_num_sms()) cpc = (cpc + 1) / 2;
   return cpc;
 }
 
@@ -764,21 +764,16 @@ constexpr int kNhwcCh = 128;    // channels per CTA
 constexpr int kNhwcChunk = 64;  // bins per output chunk (shared-memory transpose tile: 128 ch x chunk)
 constexpr int kNhwcThreads = 224;  // 7 warps: the 49 bins of a 7x7 output (and 7-multiples of a 14x14 chunk) split evenly
 
-// Packed fp32 FMA (sm_100 FFMA2): d.xy = w * v.xy + c.xy in ONE issue slot.  The tap loop is issue-bound, not FMA-pipe-bound.
+// Pairs of fp32 lanes: d.xy = w * v.xy + c.xy (two fused multiply-adds, each rounded once)
 struct F2 {
-  unsigned long long v;
+  float x, y;
 };
-__device__ __forceinline__ F2 f2_pack(float a, float b) {
-  F2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(a), "f"(b));
-  return r;
+__device__ __forceinline__ F2 f2_pack(float a, float b) { return F2{a, b}; }
+__device__ __forceinline__ void f2_unpack(F2 p, float& a, float& b) {
+  a = p.x;
+  b = p.y;
 }
-__device__ __forceinline__ void f2_unpack(F2 p, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(p.v)); }
-__device__ __forceinline__ F2 f2_fma(F2 w, F2 v, F2 c) {
-  F2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d.v) : "l"(w.v), "l"(v.v), "l"(c.v));
-  return d;
-}
+__device__ __forceinline__ F2 f2_fma(F2 w, F2 v, F2 c) { return F2{__fmaf_rn(w.x, v.x, c.x), __fmaf_rn(w.y, v.y, c.y)}; }
 
 // One bin: XC x-taps (byte offsets / weights held in registers) times RY rows per step = XC * RY independent 512-byte loads in
 // flight per warp.  Table entries hold BYTE offsets premultiplied for the NHWC layout (row: y*W*C*4, column: x*C*4) and the
@@ -1129,7 +1124,7 @@ static int launch_fwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C,
   const int slabs = d2b_cdiv(C, kNhwcCh);
   // bins of a RoI are split into chunks (grid.z): at least enough for the transpose tile, more when K x slabs alone
   // would leave SMs idle (a mask-head call has 100 RoIs x 196 bins)
-  const long long want = d2b_cdiv(8LL * kNumSMs, (long long)K * slabs);
+  const long long want = d2b_cdiv(8LL * d2b_num_sms(), (long long)K * slabs);
   int nchunks = (int)std::max<long long>(d2b_cdiv(bins, kNhwcChunk), std::min<long long>(want, d2b_cdiv(bins, 8)));
   int chunk = d2b_cdiv(bins, nchunks);
   if (nchunks > 1) chunk = std::min(kNhwcChunk - 1, d2b_cdiv(chunk, 7) * 7);  // whole rounds of the CTA's 7 warps
@@ -1408,7 +1403,7 @@ static int launch_bwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C,
   const int slabs = d2b_cdiv(C, kNhwcCh);
   int rows = PH;
   auto smem_of = [&](int r) { return sizeof(float) * kNhwcCh * ((size_t)r * PW + (size_t)(kBwdThreads / 32) * PW); };
-  while (rows > 4 && (smem_of(rows) > 100 * 1024 || (long long)K * slabs * d2b_cdiv(PH, rows) < 4LL * kNumSMs) &&
+  while (rows > 4 && (smem_of(rows) > 100 * 1024 || (long long)K * slabs * d2b_cdiv(PH, rows) < 4LL * d2b_num_sms()) &&
          smem_of(rows) > 56 * 1024)
     rows = (rows + 1) / 2;
   // gradient tile [rows * PW][128] + per-warp row-collapsed tile [8 warps][PW][128]

@@ -1,9 +1,9 @@
-// PTX wrappers shared by the tcgen05 / TMEM / bulk-copy kernels (sm_100a only).
+// PTX wrappers shared by the wgmma / bulk-copy kernels (sm_90a).
 //
-//   mbarrier            producer/consumer rings (generic, async-proxy and tensor-core arrivals)
+//   mbarrier            producer/consumer rings (generic and async-proxy arrivals)
 //   cp.async.bulk       TMA engine, linear form: one instruction moves a whole pre-tiled operand block
 //                       global -> shared and completes on an mbarrier (SASS: UBLKCP)
-//   tcgen05.*           TMEM allocation, UMMA issue (SASS: UTCHMMA), commit (UTCBAR), TMEM loads (LDTM)
+//   wgmma.*             warpgroup MMA from shared-memory descriptors into register accumulators (SASS: HGMMA)
 //   red.global.v4.f32   128-bit vector reduction to global memory (SASS: REDG.E.ADD.F32x4)
 #pragma once
 #include <cuda_bf16.h>
@@ -54,8 +54,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 
 // ------------------------------------------------------------------------------------------------ proxies / fences
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -77,64 +75,93 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ------------------------------------------------------------------------------------------------ TMEM
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t base) {  // the warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "n"(kCols) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (thread i <-> TMEM lane base_lane + i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------ UMMA
-// Shared-memory matrix descriptor (sm_100 version 1), 128-byte swizzle.
+// ------------------------------------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor (sm_90), 128-byte swizzle.
 //   K-major  tile [rows][64 bf16]: rows 128 B apart, 8-row atoms `sbo` bytes apart (1024 when rows are dense)
 //   MN-major tile [k rows][64 bf16 of M/N]: 8-k-row atoms `sbo` bytes apart, 64-element M/N blocks `lbo` bytes apart
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor, kind::f16: D = f32, A = B = bf16, M = 128.
-__device__ __forceinline__ uint32_t umma_idesc(int n, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by one thread for the CTA
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrive once every previously issued MMA of this thread has completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+
+// One warpgroup: D[64 x N] (+)= A[64 x 16] . B[16 x N], bf16 operands from shared memory, fp32 accumulator in registers
+// (N / 2 per thread: element (16 w + l / 4 + 8 h, 8 j + 2 (l % 4) + e) of warp w, lane l is acc[4 j + 2 h + e]).
+// kTransA: A is MN-major (M contiguous); B is always K-major.
+template <int N, int kTransA>
+struct Wgmma;
+
+template <int kTransA>
+struct Wgmma<8, kTransA> {
+  __device__ __forceinline__ static void mma(float (&d)[4], uint64_t a, uint64_t b, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, %5, %6, p, 1, 1, %7, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(accumulate), "l"(a), "l"(b), "n"(kTransA));
+  }
+};
+template <int kTransA>
+struct Wgmma<16, kTransA> {
+  __device__ __forceinline__ static void mma(float (&d)[8], uint64_t a, uint64_t b, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %8, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %9, %10, p, 1, 1, %11, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(accumulate), "l"(a), "l"(b), "n"(kTransA));
+  }
+};
+template <int kTransA>
+struct Wgmma<32, kTransA> {
+  __device__ __forceinline__ static void mma(float (&d)[16], uint64_t a, uint64_t b, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %16, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %17, %18, p, 1, 1, %19, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(accumulate), "l"(a), "l"(b), "n"(kTransA));
+  }
+};
+template <int kTransA>
+struct Wgmma<64, kTransA> {
+  __device__ __forceinline__ static void mma(float (&d)[32], uint64_t a, uint64_t b, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %32, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %33, %34, p, 1, 1, %35, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(accumulate), "l"(a), "l"(b), "n"(kTransA));
+  }
+};
+template <int kTransA>
+struct Wgmma<128, kTransA> {
+  __device__ __forceinline__ static void mma(float (&d)[64], uint64_t a, uint64_t b, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %64, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %65, %66, p, 1, 1, %67, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(accumulate), "l"(a), "l"(b), "n"(kTransA));
+  }
+};
+
+// Register budget of the calling warpgroup (every warp of it executes the instruction): the TMA / saver warpgroup gives
+// registers back so that the four worker warpgroups can hold accumulators and gather state without spilling.
+template <int kRegs>
+__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs>
+__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 
 // ------------------------------------------------------------------------------------------------ misc
 __device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+__device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void red_add(float* p, float a) {
   asm volatile("red.global.add.f32 [%0], %1;" ::"l"(p), "f"(a) : "memory");
@@ -153,36 +180,19 @@ __device__ __forceinline__ void split4(const float (&v)[4], uint2& hi, uint2& lo
   split2(v[0], v[1], hi.x, lo.x);
   split2(v[2], v[3], hi.y, lo.y);
 }
-// Packed fp32 FMA (sm_100 FFMA2): two lanes of fp32 FMA in ONE issue slot -- the gather loops are issue-bound
+// Pairs of fp32 lanes: the gather / scatter loops are written over channel pairs (one FFMA per lane on sm_90)
 struct F2 {
-  unsigned long long v;
+  float x, y;
 };
-__device__ __forceinline__ F2 f2_pack(float a, float b) {
-  F2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(a), "f"(b));
-  return r;
+__device__ __forceinline__ F2 f2_pack(float a, float b) { return F2{a, b}; }
+__device__ __forceinline__ void f2_unpack(F2 p, float& a, float& b) {
+  a = p.x;
+  b = p.y;
 }
-__device__ __forceinline__ void f2_unpack(F2 p, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(p.v)); }
-__device__ __forceinline__ F2 f2_fma(F2 w, F2 v, F2 c) {
-  F2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d.v) : "l"(w.v), "l"(v.v), "l"(c.v));
-  return d;
-}
-__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) {
-  F2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d.v) : "l"(a.v), "l"(b.v));
-  return d;
-}
-__device__ __forceinline__ F2 f2_add(F2 a, F2 b) {
-  F2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d.v) : "l"(a.v), "l"(b.v));
-  return d;
-}
-__device__ __forceinline__ F2 f2_sub(F2 a, F2 b) {
-  F2 d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d.v) : "l"(a.v), "l"(b.v));
-  return d;
-}
+__device__ __forceinline__ F2 f2_fma(F2 w, F2 v, F2 c) { return F2{__fmaf_rn(w.x, v.x, c.x), __fmaf_rn(w.y, v.y, c.y)}; }
+__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) { return F2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ F2 f2_add(F2 a, F2 b) { return F2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+__device__ __forceinline__ F2 f2_sub(F2 a, F2 b) { return F2{__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)}; }
 __device__ __forceinline__ void red_add_v4(float* p, F2 ab, F2 cd) {
   float a, b, c, d;
   f2_unpack(ab, a, b);

@@ -1,4 +1,4 @@
-"""Hot-path subset of `detectron2.layers` (detectron2/layers/__init__.py:2-24), B200-native.
+"""Hot-path subset of `detectron2.layers` (detectron2/layers/__init__.py:2-24), H100-native.
 
 Only the operators that sit on custom kernels are provided; plain-PyTorch helpers of the reference package
 (norm layers, wrappers, losses, ...) are out of scope (SURVEY.md section 8).

@@ -11,8 +11,8 @@ from torch.nn.modules.utils import _pair
 
 from .. import ops
 
-# -1 = auto: bf16x3 operand split on tcgen05/TMEM when the tensor-core kernel takes the shape, else fp32 FFMA (both are
-# fp32-class, <= 1e-4 rel);  0 = fp32 FFMA;  1 = bf16x3 tcgen05;  2 = plain bf16 tcgen05 (autocast-style operands).
+# -1 = auto: bf16x3 operand split on wgmma when the tensor-core kernel takes the shape, else fp32 FFMA (both are
+# fp32-class, <= 1e-4 rel);  0 = fp32 FFMA;  1 = bf16x3 wgmma;  2 = plain bf16 wgmma (autocast-style operands).
 DEFAULT_PRECISION = -1
 
 

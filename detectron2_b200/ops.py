@@ -32,11 +32,13 @@ def _f32c(t: Optional[Tensor]) -> Optional[Tensor]:
 # Feature-map layout policy of the axis-aligned forward (D2B_POOLER_LAYOUT = auto | nchw | nhwc):
 #   * channels_last inputs are consumed in place by the NHWC kernel (torchvision would .contiguous() them first);
 #   * NCHW inputs go to the NCHW kernel, unless the call is large enough that "one layout-change launch + NHWC
-#     pooling" is cheaper (cost model below, fitted to the B200 measurements in profiles/r1_ops.md).
+#     pooling" is cheaper.  Cost model fitted to tools/bench_pooler_layouts.py on an H100 80GB HBM3 SXM at 700 W
+#     (bench.py's 800x1333 pyramid, 256 channels; 1 000 / 512 / 2 000 RoIs at 7x7 and 100 at 14x14); it picks the faster
+#     path on all four.
 POOLER_LAYOUT = os.environ.get("D2B_POOLER_LAYOUT", "auto")
-_NCHW_PS_PER_OUT = 13.0      # NCHW kernel: picoseconds per output element (12.4 mask head .. 17.8 box head)
-_NHWC_PS_PER_OUT = 7.5       # NHWC kernel (7.4 .. 7.6)
-_XPOSE_PS_PER_BYTE = 0.32    # layout change: 91.7 MB of fp32 features in 29 us (reads + writes each byte once)
+_NCHW_PS_PER_OUT = 21.0      # NCHW kernel: picoseconds per output element (13.9 mask head .. 27.5 box head, 512 RoIs)
+_NHWC_PS_PER_OUT = 9.0       # NHWC kernel (7.8 .. 16.8)
+_XPOSE_PS_PER_BYTE = 0.72    # layout change: 91.4 MB of fp32 features in 65-68 us (reads + writes each byte once)
 
 
 def _is_channels_last(t: Tensor) -> bool:
@@ -140,7 +142,9 @@ def _(input, rois, spatial_scale, pooled_h, pooled_w, sampling_ratio, aligned):
     return input.new_empty((rois.shape[0], input.shape[1], pooled_h, pooled_w))
 
 
-_NCHW_BWD_PS_PER_OUT = 40.0  # NCHW backward kernel: picoseconds per grad_out element (33 .. 44 measured)
+# Backward and rotated per-element costs are carried over from the kernels' first tuning and have not been re-measured on an
+# H100 (the layout-change cost per byte above has); the choice only changes speed, every path computes the same result.
+_NCHW_BWD_PS_PER_OUT = 40.0  # NCHW backward kernel: picoseconds per grad_out element
 _NHWC_BWD_PS_PER_OUT = 8.0   # channels-last backward (one red.v4 per footprint pixel)
 
 
@@ -356,7 +360,7 @@ def _pooler_bwd(ctx, grad):
 roi_pooler_op.register_autograd(_pooler_bwd, setup_context=_pooler_setup)
 
 
-_ROT_NCHW_PS = (30.0, 64.0)  # rotated NCHW kernels: picoseconds per output element (forward, backward)
+_ROT_NCHW_PS = (30.0, 64.0)  # rotated NCHW kernels: picoseconds per output element (forward, backward); not re-measured, above
 _ROT_NHWC_PS = (10.0, 16.0)  # rotated channels-last kernels
 
 
@@ -750,7 +754,7 @@ def deform_conv_fused_op(x: Tensor, offset_mask: Tensor, weight: Tensor, scale: 
                          deformable_groups: int, precision: int) -> Tensor:
     """y = relu(modulated_deform_conv(x, offset, sigmoid(mask), weight) * scale + shift) with offset / mask taken straight
     from the raw conv2_offset output `offset_mask` [N, 3*dg*kh*kw, Ho, Wo] (detectron2/modeling/backbone/resnet.py:305-318):
-    the chunk / cat / sigmoid happen while the sampling taps are built, scale / shift / relu in the TMEM epilogue."""
+    the chunk / cat / sigmoid happen while the sampling taps are built, scale / shift / relu in the accumulator epilogue."""
     _C.require_cuda(x, offset_mask, weight, scale, shift)
     kh, kw = weight.shape[2:]
     n, cout, ho, wo = dcn_output_shape(x, weight, stride, padding, dilation)

@@ -1,5 +1,5 @@
 /*
- * d2b200.h -- C ABI of the B200-native detection hot path (libd2b200.so).
+ * d2b200.h -- C ABI of the H100-native detection hot path (libd2b200.so).
  *
  * This is the drop-in boundary: plain pointers, sizes and a CUDA stream, no torch types.
  * Every entry point cites the reference interface it replaces (paths relative to the
@@ -35,7 +35,7 @@ extern "C" {
 int d2b_abi_version(void);
 /* compile-time facts, replaces detectron2._C.get_cuda_version / has_cuda (csrc/vision.cpp:23-49,86-88) */
 int d2b_cuda_version(void);
-const char* d2b_arch(void); /* "sm_100a" */
+const char* d2b_arch(void); /* "sm_90a" */
 
 /* ---- RoIAlign, axis-aligned -------------------------------------------------------------
  * Replaces torchvision::roi_align / torchvision::_roi_align_backward as reached from
@@ -262,8 +262,8 @@ typedef struct {
       deformable_groups;
 } d2b_dcn_params;
 
-/* precision: 0 = fp32 FFMA (parity path), 1 = bf16x3 split on tcgen05 (fp32-class accuracy, <= 1e-4 rel), 2 = plain bf16
- * operands on tcgen05 (autocast path), -1 = auto (1 when the tensor-core kernels take the shape, else 0).
+/* precision: 0 = fp32 FFMA (parity path), 1 = bf16x3 split on wgmma (fp32-class accuracy, <= 1e-4 rel), 2 = plain bf16
+ * operands on wgmma (autocast path), -1 = auto (1 when the tensor-core kernels take the shape, else 0).
  * flags: D2B_DCN_X_NHWC -- x (and grad_x) are channels-last storage [N,H,W,Cin] (the storage of a torch.channels_last
  *        tensor), 16-byte aligned; tensor-core precisions only.  Without it the tensor-core path re-lays x out once per call.
  * The tensor-core path needs scratch (NHWC copy of x, pre-tiled bf16 operands): query the size first; 256-byte aligned.
@@ -294,7 +294,7 @@ int d2b_deform_conv_backward(const float* x, const float* offset, const float* m
 /* conv2 of a DeformBottleneckBlock fused (detectron2/modeling/backbone/resnet.py:305-318): `offset_mask`
  * [N, 3*DG*kh*kw, Ho, Wo] is the raw conv2_offset output (chunk / cat / sigmoid of :307-311 applied while the sampling taps
  * are built), y = relu(conv * scale[oc] + shift[oc]) (FrozenBatchNorm folded, or scale NULL and shift = bias; relu 0/1) is
- * applied in the TMEM epilogue.  Tensor-core precisions only (1, 2 or -1); workspace sizes are those of
+ * applied in the accumulator epilogue.  Tensor-core precisions only (1, 2 or -1); workspace sizes are those of
  * d2b_deform_conv_forward / backward_workspace_bytes.  The backward takes y (to gate the ReLU) and returns the gradient of
  * the fused offset_mask tensor (mask part through the sigmoid). */
 int d2b_deform_conv_fused_forward(const float* x, const float* offset_mask, const float* weight, const float* scale,

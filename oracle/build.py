@@ -2,8 +2,8 @@
 
 build_oracle()  gcc -> oracle/_build/libd2oracle.so   (the C restatement, oracle/d2_oracle.c)
 build_ref()     g++ -> oracle/_ref/d2_ref_cpu.so      (the reference's own CPU csrc, compiled from
-                where it lies under /root/reference; only possible in the authoring container.
-                The built .so travels to the GPU box with the snapshot; sources are never copied.)
+                where the reference source tree lies (REF_SRC); sources are never copied.  The
+                tests compare against reference outputs stored under tests/golden/, not against this .so.)
 
 Reference build recipe follows SURVEY.md Appendix B.1: vision.cpp + */*_cpu.cpp + cocoeval.cpp,
 loaded with torch.ops.load_library (TORCH_LIBRARY ops only; never imported as a python module).
@@ -41,7 +41,7 @@ def build_oracle(force=False):
 
 def build_ref(force=False):
     """Compile the reference CPU csrc in place. Returns the .so path, or None when the reference
-    tree is absent (GPU box) and no prebuilt .so travelled with the snapshot."""
+    tree is absent and no .so was built before."""
     if os.path.exists(REF_SO) and not force:
         return REF_SO
     if not os.path.isdir(REF_SRC):
@@ -63,7 +63,7 @@ def build_ref(force=False):
 
 
 def build_ref_cuda(force=False):
-    """The reference's full csrc (CPU + CUDA kernels) compiled for sm_100a: the GPU kernel-to-beat of the rotated ops and
+    """The reference's full csrc (CPU + CUDA kernels) compiled for sm_90a: the GPU kernel-to-beat of the rotated ops and
     of deformable convolution (SURVEY.md Appendix B.2, flags of the reference's setup.py:74-80).  A python extension
     module (`import d2_ref_cuda` after putting oracle/_ref on sys.path) because the five deform-conv functions are
     pybind-only (csrc/vision.cpp:86-102).  Compiles here without a GPU; only tools/ and tests/ ever load it."""
@@ -75,7 +75,7 @@ def build_ref_cuda(force=False):
 
     bdir = os.path.join(REF_DIR, "_cuda_build")
     os.makedirs(bdir, exist_ok=True)
-    os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0a"
+    os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"
     sources = ([os.path.join(REF_SRC, "vision.cpp")] + sorted(glob.glob(os.path.join(REF_SRC, "**", "*.cpp")))
                + sorted(glob.glob(os.path.join(REF_SRC, "**", "*.cu"))) + sorted(glob.glob(os.path.join(REF_SRC, "*.cu"))))
     load(name="d2_ref_cuda", sources=sources, extra_include_paths=[REF_SRC], build_directory=bdir, with_cuda=True,

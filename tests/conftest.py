@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: run with -m gpu)")
     # The compiled reference (oracle/_ref) DEFines the detectron2:: op schemas; load it before detectron2_b200.ops
     # so that our library only adds CUDA kernels next to the reference's CPU ones (see ops.register_detectron2_namespace).
     try:

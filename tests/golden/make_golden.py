@@ -425,6 +425,151 @@ def gen_postprocessing():
     save("postprocessing", **out)
 
 
+def gen_reference_cross_checks():
+    """Inputs and reference outputs of the oracle cross-checks in tests/test_oracle_pins.py (live comparisons with the
+    compiled reference CPU csrc and the reference's paste_masks_in_image), so that they run without the reference."""
+    out = {}
+    g = torch.Generator().manual_seed(11)
+    n = 150
+    b = torch.stack([torch.rand(n, generator=g) * 80, torch.rand(n, generator=g) * 80, 1 + torch.rand(n, generator=g) * 40,
+                     1 + torch.rand(n, generator=g) * 40, (torch.rand(n, generator=g) - 0.5) * 400], 1)
+    s = torch.rand(n, generator=g)
+    out.update(rot_boxes=b, rot_scores=s, rot_iou=D2.box_iou_rotated(b, b.flip(0)))
+    for thr in (0.2, 0.5):
+        out["rot_keep_%g" % thr] = D2.nms_rotated(b, s, thr)
+    for seed in range(3):
+        g = torch.Generator().manual_seed(3000 + seed)
+        n_, c, h, w = 2, 3 + seed, 17 + 5 * seed, 23
+        ph, pw, sr = [(7, 7, 0), (3, 5, 2), (2, 2, 3)][seed]
+        k = 19
+        rois = torch.cat([torch.randint(0, n_, (k, 1), generator=g).float(),
+                          torch.rand(k, 2, generator=g) * torch.tensor([w * 4.0, h * 4.0]),
+                          2 + torch.rand(k, 2, generator=g) * 50, (torch.rand(k, 1, generator=g) - 0.5) * 360], 1)
+        x = torch.randn(n_, c, h, w, generator=g)
+        y = D2.roi_align_rotated_forward(x, rois, 0.25, ph, pw, sr)
+        go = torch.randn(y.shape, generator=g)
+        gx = D2.roi_align_rotated_backward(go, rois, 0.25, ph, pw, n_, c, h, w, sr)
+        out.update({"rra%d_%s" % (seed, k_): v for k_, v in dict(x=x, rois=rois, y=y, go=go, gx=gx).items()})
+    spec = importlib.util.spec_from_file_location("ref_mask_ops", "/root/reference/detectron2/layers/mask_ops.py")
+    mo = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mo)
+    g = torch.Generator().manual_seed(8)
+    masks = torch.rand(6, 28, 28, generator=g)
+    ctr = torch.rand(6, 2, generator=g) * torch.tensor([200.0, 150.0])
+    wh = 10 + torch.rand(6, 2, generator=g) * 90
+    boxes = torch.cat([ctr - wh / 2, ctr + wh / 2], 1)
+    out.update(paste_masks=masks, paste_boxes=boxes, paste_out=mo.paste_masks_in_image(masks, boxes, (150, 200), 0.5))
+    save("reference_cross_checks", **out)
+
+
+class _FakeCuda(torch.Tensor):
+    """CPU tensor that claims to live on a GPU (the reference's deform-conv wrappers only test the flag)."""
+
+    @property
+    def is_cuda(self):
+        return True
+
+
+def _import_reference_deform_conv(shim):
+    """detectron2/layers/deform_conv.py of the reference, with `shim` bound as detectron2._C (fvcore stubbed)."""
+    import types
+
+    def stub(name, **attrs):
+        m = types.ModuleType(name)
+        m.__dict__.update(attrs)
+        sys.modules[name] = m
+        return m
+
+    fv = stub("fvcore", __version__="0.1.5")
+    fv.nn = stub("fvcore.nn")
+    stub("fvcore.nn.distributed", differentiable_all_reduce=lambda x: x)
+    fv.nn.weight_init = stub("fvcore.nn.weight_init")
+    sys.path.insert(0, "/root/reference")
+    try:
+        import detectron2  # noqa: F401  (the real package __init__)
+
+        sys.modules["detectron2._C"] = shim
+        detectron2._C = shim
+        return importlib.import_module("detectron2.layers.deform_conv")
+    finally:
+        sys.path.remove("/root/reference")
+
+
+def gen_shim_protocol():
+    """Every call the reference's _DeformConv / _ModulatedDeformConv make into detectron2._C, recorded on stand-ins with our
+    shim's parameter lists (tests/test_reference_shim.py replays it), plus the Functions' results."""
+    import json
+    import math
+    import types
+
+    spec = importlib.util.spec_from_file_location("shim_test", os.path.join(ROOT, "tests", "test_reference_shim.py"))
+    st = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(st)
+    g = torch.Generator().manual_seed(0)
+    n, c, h, w, co = 2, 4, 7, 9, 6
+    t = {"x": torch.randn(n, c, h, w, generator=g), "offset": torch.randn(n, 18, h, w, generator=g),
+         "mask": torch.sigmoid(torch.randn(n, 9, h, w, generator=g)),
+         "weight": torch.randn(co, c, 3, 3, generator=g) * (1 / math.sqrt(c * 9)), "bias": torch.randn(co, generator=g),
+         "grad_output": torch.randn(n, co, h, w, generator=g)}
+    fns, _ = st.oracle_shim(t["weight"])
+    fc = {k: torch.Tensor._make_subclass(_FakeCuda, v.clone(), k != "grad_output") for k, v in t.items()}
+    log, keep = [], []
+
+    def describe(v):
+        if not isinstance(v, torch.Tensor):
+            return {"scalar": v}
+        for k, kt in fc.items():
+            if v.numel() and v.data_ptr() == kt.data_ptr() and v.shape == kt.shape:
+                return {"input": k}
+        keep.append(v)  # keeps id() unique while recording
+        ids = [id(b) for b in keep]
+        return {"buffer": "b%d" % ids.index(id(v)), "shape": list(v.shape),
+                "zeroed": bool(v.numel() == 0 or (v == 0).all())}
+
+    def recording(name):
+        def call(*args):
+            log.append({"fn": name, "args": [describe(v) for v in args]})
+            return fns[name](*args)
+        return call
+
+    shim = types.ModuleType("detectron2._C")
+    for name in st.SHIM_FUNCTIONS:
+        setattr(shim, name, recording(name))
+    saved = {k: v for k, v in sys.modules.items() if k.startswith(("detectron2", "fvcore"))}
+    for k in saved:
+        del sys.modules[k]
+    try:
+        mod = _import_reference_deform_conv(shim)
+        protocol, out = [], {}
+        for phase, inputs in (("v1", ("x", "offset", "weight")), ("v2", ("x", "offset", "mask", "weight", "bias"))):
+            log.clear()
+            keep.clear()
+            for k in inputs:
+                fc[k].grad = None
+            if phase == "v1":
+                y = mod.deform_conv(fc["x"], fc["offset"], fc["weight"], 1, 1, 1, 1, 1, 64)
+            else:
+                y = mod.modulated_deform_conv(fc["x"], fc["offset"], fc["mask"], fc["weight"], fc["bias"], 1, 1, 1, 1, 1)
+            y.backward(fc["grad_output"])
+            results = {"y": y}
+            results.update({"grad_" + k: fc[k].grad for k in inputs})
+            names = {}
+            for rn, rt in results.items():
+                # autograd may hand a leaf a copy of the returned gradient: identify the buffer by its exact contents
+                rp = rt.detach().as_subclass(torch.Tensor)
+                buf = [i for i, b in enumerate(keep)
+                       if b.shape == rp.shape and torch.equal(b.detach().as_subclass(torch.Tensor), rp)]
+                assert buf, (phase, rn)
+                names[rn] = "b%d" % buf[0]
+                out["%s_%s" % (phase, rn)] = rt.detach().as_subclass(torch.Tensor).clone()
+            protocol.append({"name": phase, "calls": list(log), "results": names})
+    finally:
+        for k in [k for k in sys.modules if k.startswith(("detectron2", "fvcore"))]:
+            del sys.modules[k]
+        sys.modules.update(saved)
+    save("shim_protocol", protocol=json.dumps(protocol), **t, **out)
+
+
 if __name__ == "__main__":
     torch.set_num_threads(1)
     gen_roi_align()
@@ -437,3 +582,5 @@ if __name__ == "__main__":
     gen_fast_rcnn_inference()
     gen_retinanet_inference()
     gen_postprocessing()
+    gen_reference_cross_checks()
+    gen_shim_protocol()

@@ -20,7 +20,7 @@ def test_header_symbols_exported():
         assert hasattr(lib, name), name
     assert set(_C.EXPORTED) == declared
     assert lib.d2b_abi_version() == _C.ABI_VERSION == 4
-    assert lib.d2b_arch() == b"sm_100a"
+    assert lib.d2b_arch() == b"sm_90a"
     assert _C.get_cuda_version().startswith("CUDA 12")
 
 

@@ -1,5 +1,5 @@
 """GPU parity tests proper: the CUDA path (through the detectron2.layers-shaped surface -> ctypes -> C ABI)
-against the CPU oracle and the committed reference fixtures.  Run on the B200 box: pytest -m gpu.
+against the CPU oracle and the committed reference fixtures.  Run on an H100: pytest -m gpu.
 
 Tolerances (BASELINE.json north_star): bit-exact NMS keep indices and box_iou_rotated; <= 1e-4 relative for
 RoIAlign and deform-conv (fp32).
@@ -824,10 +824,11 @@ def test_roi_align_backward_wide_footprint(L, sr, monkeypatch):
     assert ok, err
 
 
-# ------------------------------------------------------------------------------- deformable conv on tcgen05 / TMEM
+# ------------------------------------------------------------------------------- deformable conv on the tensor cores (wgmma)
 @pytest.mark.parametrize("cin,cout,h,w,grp,dg,mod,stride,prec", [
     (64, 64, 12, 20, 1, 1, False, 1, 1), (128, 128, 25, 42, 1, 1, False, 1, 1), (128, 192, 17, 23, 2, 1, True, 1, 1),
-    (256, 256, 21, 19, 1, 2, True, 2, 1), (128, 128, 25, 42, 1, 1, False, 1, 2)])
+    (256, 256, 21, 19, 1, 2, True, 2, 1), (128, 128, 25, 42, 1, 1, False, 1, 2), (64, 48, 11, 13, 1, 1, True, 1, 1),
+    (64, 80, 19, 9, 1, 1, False, 1, 2)])
 def test_deform_conv_tensor_core_vs_oracle(cin, cout, h, w, grp, dg, mod, stride, prec):
     from detectron2_b200 import ops
 
@@ -860,7 +861,7 @@ def test_deform_conv_tensor_core_vs_oracle(cin, cout, h, w, grp, dg, mod, stride
     (128, 128, 13, 17, 8, 1, True, 1, 1), (256, 256, 9, 11, 8, 1, False, 1, 1), (128, 128, 25, 42, 1, 1, False, 1, 2),
     (256, 256, 50, 84, 1, 1, True, 1, 1)])
 def test_deform_conv_tensor_core_backward_vs_oracle(cin, cout, h, w, grp, dg, mod, stride, prec):
-    # tcgen05 backward (data: grad_x / grad_offset / grad_mask, weight) against the oracle (torchvision CPU autograd);
+    # tensor-core backward (data: grad_x / grad_offset / grad_mask, weight) against the oracle (torchvision CPU autograd);
     # grp=8 with 16 / 32 channels per group exercises the super-group packing, the last row is a cfg-5 layer (R50 res4)
     from detectron2_b200 import _C, ops
     import ctypes as C

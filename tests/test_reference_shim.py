@@ -1,93 +1,52 @@
 """The `detectron2._C`-shaped deform-conv shim (detectron2_b200/_C.py, SURVEY.md 8b "pybind functions").
 
-CPU part (authoring container only, needs /root/reference): the REAL, unmodified reference autograd Functions
-`_DeformConv` / `_ModulatedDeformConv` (detectron2/layers/deform_conv.py:29-184, :205-313) are imported with our shim
-bound as `detectron2._C`.  They refuse CPU tensors, so the tensors are wrapped in a subclass that reports is_cuda, and the
-shim's five entry points are backed by the CPU oracle for this test: what is verified is the CALL PROTOCOL the reference
-uses against our signatures -- argument order (width-first for DCNv1), caller-allocated outputs written in place,
-gradients accumulated into zero-initialised buffers -- by comparing the reference Functions' results with torchvision
-autograd.  GPU part: the same protocol, restated call by call, against the real kernels.
+CPU part: the call protocol of the REAL, unmodified reference autograd Functions `_DeformConv` / `_ModulatedDeformConv`
+(detectron2/layers/deform_conv.py:29-184, :205-313) against our signatures.  tests/golden/make_golden.py ran those Functions
+with a stand-in `detectron2._C` and recorded every call they make into it (tests/golden/shim_protocol.npz): function, the
+positional arguments (scalars as values, tensors as the input they are or as a caller-allocated buffer with its shape and
+whether the caller zero-filled it) and which buffers the Functions returned as the output and the gradients.  The test
+replays that sequence on stand-ins with EXACTLY the parameter lists of the product's shim functions, backed by the CPU oracle
+(torchvision deform_conv2d + autograd), and compares the returned buffers with the reference Functions' recorded results:
+argument order (width-first for DCNv1), caller-allocated outputs written in place, gradients accumulated into
+zero-initialised buffers.  GPU part: the same protocol, restated call by call, against the real kernels.
 """
 import inspect
+import json
 import math
 import os
-import sys
-import types
 
+import numpy as np
 import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+SHIM_FUNCTIONS = ("deform_conv_forward", "deform_conv_backward_input", "deform_conv_backward_filter",
+                  "modulated_deform_conv_forward", "modulated_deform_conv_backward")
 
 
-class FakeCuda(torch.Tensor):
-    """CPU tensor that claims to live on a GPU (the reference wrappers only test the flag)."""
-
-    @property
-    def is_cuda(self):
-        return True
+def _plain(t):
+    return None if t is None else t.detach().as_subclass(torch.Tensor)
 
 
-def _fc(t):
-    return None if t is None else torch.Tensor._make_subclass(FakeCuda, t, t.requires_grad)
-
-
-def _import_reference_deform_conv(shim):
-    def stub(name, **attrs):
-        m = types.ModuleType(name)
-        m.__dict__.update(attrs)
-        sys.modules[name] = m
-        return m
-
-    saved = {k: v for k, v in sys.modules.items() if k.startswith(("detectron2", "fvcore"))}
-    for k in saved:
-        del sys.modules[k]
-    fv = stub("fvcore", __version__="0.1.5")
-    fv.nn = stub("fvcore.nn")
-    stub("fvcore.nn.distributed", differentiable_all_reduce=lambda x: x)
-    fv.nn.weight_init = stub("fvcore.nn.weight_init")
-    sys.path.insert(0, REF)
-    try:
-        import detectron2  # noqa: F401  (the real package __init__)
-
-        sys.modules["detectron2._C"] = shim
-        detectron2._C = shim
-        import importlib
-
-        mod = importlib.import_module("detectron2.layers.deform_conv")
-    finally:
-        sys.path.remove(REF)
-    return mod, saved
-
-
-def _restore(saved):
-    for k in [k for k in sys.modules if k.startswith(("detectron2", "fvcore"))]:
-        del sys.modules[k]
-    sys.modules.update(saved)
-
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present (GPU box)")
-def test_reference_functions_drive_the_shim_signatures():
+def tv_all(x, off, mask, w, bias, stride, pad, dil, go=None):
+    """torchvision deform_conv2d (+ autograd when `go` is given): y, or the gradients of (x, off, mask, w, bias)."""
     import torchvision
 
+    with torch.enable_grad():  # the reference's backward runs under once_differentiable (grad mode off)
+        xs = [_plain(t).clone().requires_grad_(True) if t is not None else None for t in (x, off, mask, w, bias)]
+        y = torchvision.ops.deform_conv2d(xs[0], xs[1], xs[3], xs[4], stride, pad, dil, xs[2])
+        if go is None:
+            return y.detach()
+        y.backward(_plain(go))
+        return [None if t is None else t.grad for t in xs]
+
+
+def oracle_shim(weight):
+    """Stand-ins for the five deform-conv entry points with OUR parameter lists, bodies = the CPU oracle.  `weight` is the
+    DCNv1 weight (deform_conv_backward_filter receives only the gradient buffer).  Returns (functions, call log)."""
     from detectron2_b200 import _C as real_shim
 
-    # a module with OUR signatures whose bodies are the CPU oracle (torchvision deform_conv2d + autograd)
-    shim = types.ModuleType("detectron2._C")
     calls = []
-
-    def plain(t):
-        return None if t is None else t.detach().as_subclass(torch.Tensor)
-
-    def tv_all(x, off, mask, w, bias, stride, pad, dil, go=None):
-        with torch.enable_grad():  # the reference's backward runs under once_differentiable (grad mode off)
-            xs = [plain(t).clone().requires_grad_(True) if t is not None else None for t in (x, off, mask, w, bias)]
-            y = torchvision.ops.deform_conv2d(xs[0], xs[1], xs[3], xs[4], stride, pad, dil, xs[2])
-            if go is None:
-                return y.detach()
-            y.backward(plain(go))
-            return [None if t is None else t.grad for t in xs]
 
     def deform_conv_forward(input, weight, offset, output, columns, ones, kW, kH, dW, dH, padW, padH, dilW, dilH, group,
                             deformable_group, im2col_step):
@@ -108,8 +67,7 @@ def test_reference_functions_drive_the_shim_signatures():
     def deform_conv_backward_filter(input, offset, gradOutput, gradWeight, columns, ones, kW, kH, dW, dH, padW, padH, dilW,
                                     dilH, group, deformable_group, scale, im2col_step):
         calls.append("deform_conv_backward_filter")
-        g = tv_all(input, offset, None, gradWeight.new_zeros(gradWeight.shape) + 0 * plain(gradWeight) + plain(W_HOLDER[0]),
-                   None, (dH, dW), (padH, padW), (dilH, dilW), gradOutput)
+        g = tv_all(input, offset, None, _plain(weight), None, (dH, dW), (padH, padW), (dilH, dilW), gradOutput)
         gradWeight.add_(g[3], alpha=scale)
         return 1
 
@@ -132,45 +90,38 @@ def test_reference_functions_drive_the_shim_signatures():
         if with_bias:
             grad_bias.add_(g[4])
 
-    W_HOLDER = [None]
-    oracle_fns = {f.__name__: f for f in (deform_conv_forward, deform_conv_backward_input, deform_conv_backward_filter,
-                                          modulated_deform_conv_forward, modulated_deform_conv_backward)}
-    for name, fn in oracle_fns.items():
+    fns = {f.__name__: f for f in (deform_conv_forward, deform_conv_backward_input, deform_conv_backward_filter,
+                                   modulated_deform_conv_forward, modulated_deform_conv_backward)}
+    for name in SHIM_FUNCTIONS:
         # the oracle-backed stand-in has EXACTLY the parameter list of the product's shim function
-        assert list(inspect.signature(fn).parameters) == list(inspect.signature(getattr(real_shim, name)).parameters), name
-        setattr(shim, name, fn)
-    shim.get_cuda_version, shim.has_cuda, shim.get_compiler_version = real_shim.get_cuda_version, real_shim.has_cuda, real_shim.get_compiler_version
+        assert list(inspect.signature(fns[name]).parameters) == list(inspect.signature(getattr(real_shim, name)).parameters), name
+    return fns, calls
 
-    mod, saved = _import_reference_deform_conv(shim)
-    try:
-        g = torch.Generator().manual_seed(0)
-        n, c, h, w, co = 2, 4, 7, 9, 6
-        x = torch.randn(n, c, h, w, generator=g)
-        off = torch.randn(n, 18, h, w, generator=g)
-        mask = torch.sigmoid(torch.randn(n, 9, h, w, generator=g))
-        wt = torch.randn(co, c, 3, 3, generator=g) * (1 / math.sqrt(c * 9))
-        bias = torch.randn(co, generator=g)
-        go = torch.randn(n, co, h, w, generator=g)
-        W_HOLDER[0] = wt
-        # ---- DCNv1 through the reference's _DeformConv
-        xs = [_fc(t.clone().requires_grad_(True)) for t in (x, off, wt)]
-        y = mod.deform_conv(xs[0], xs[1], xs[2], 1, 1, 1, 1, 1, 64)
-        y.backward(_fc(go))
-        ref = tv_all(x, off, None, wt, None, (1, 1), (1, 1), (1, 1), go)
-        assert torch.allclose(plain(y), tv_all(x, off, None, wt, None, (1, 1), (1, 1), (1, 1)), atol=1e-5)
-        for a, b in zip(xs, (ref[0], ref[1], ref[3])):
-            assert torch.allclose(plain(a.grad), b, atol=1e-5)
-        # ---- DCNv2 through the reference's _ModulatedDeformConv
-        xs = [_fc(t.clone().requires_grad_(True)) for t in (x, off, mask, wt, bias)]
-        y = mod.modulated_deform_conv(xs[0], xs[1], xs[2], xs[3], xs[4], 1, 1, 1, 1, 1)
-        y.backward(_fc(go))
-        ref = tv_all(x, off, mask, wt, bias, (1, 1), (1, 1), (1, 1), go)
-        for a, b in zip(xs, ref):
-            assert torch.allclose(plain(a.grad), b, atol=1e-5)
-        assert calls == ["deform_conv_forward", "deform_conv_backward_input", "deform_conv_backward_filter",
-                         "modulated_deform_conv_forward", "modulated_deform_conv_backward"]
-    finally:
-        _restore(saved)
+
+def test_reference_functions_drive_the_shim_signatures(golden):
+    d = golden("shim_protocol")
+    t = {k: torch.from_numpy(d[k]) for k in ("x", "offset", "mask", "weight", "bias", "grad_output")}
+    protocol = json.loads(str(d["protocol"]))
+    fns, calls = oracle_shim(t["weight"])
+    for phase in protocol:  # DCNv1 through _DeformConv, then DCNv2 through _ModulatedDeformConv
+        bufs = {}
+
+        def arg(a):
+            if "scalar" in a:
+                return a["scalar"]
+            if "input" in a:
+                return t[a["input"]].clone()
+            if a["buffer"] not in bufs:  # first use: the shape the caller allocated, zero-filled only where it zero-filled
+                fill = 0.0 if a["zeroed"] else float("nan")
+                bufs[a["buffer"]] = torch.full(a["shape"], fill, dtype=torch.float32)
+            return bufs[a["buffer"]]
+
+        for call in phase["calls"]:
+            fns[call["fn"]](*[arg(a) for a in call["args"]])
+        for name, buf in phase["results"].items():
+            ref = torch.from_numpy(d["%s_%s" % (phase["name"], name)])
+            assert torch.allclose(bufs[buf], ref, atol=1e-5), (phase["name"], name)
+    assert calls == list(SHIM_FUNCTIONS)
 
 
 def test_shim_exports_the_reference_pybind_names():

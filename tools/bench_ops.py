@@ -206,7 +206,7 @@ def main():
         flops = 2.0 * n * cin * (cin // grp) * 9 * hh * ww
         from detectron2_b200 import ops as _ops
         tr = timeit(lambda: tv.deform_conv2d(xx, off, wt, None, 1, 1, 1), rep=5, warm=1) if (tv and True) else None
-        for prec, tag in ((0, "fp32 FFMA"), (1, "bf16x3 tcgen05"), (2, "bf16 tcgen05")):
+        for prec, tag in ((0, "fp32 FFMA"), (1, "bf16x3 wgmma"), (2, "bf16 wgmma")):
             try:
                 t = timeit(lambda: _ops.deform_conv_op(xx, off, None, wt, None, [1, 1], [1, 1], [1, 1], grp, 1, prec), rep=10, warm=2)
             except RuntimeError:
@@ -216,7 +216,7 @@ def main():
                 "%.2f TFLOP/s; reference csrc CUDA: %s us" % (flops / t / 1e6, ("%.1f" % rc) if rc else "n/a"))
         try:  # the training forward: also lays x out channels-last once and keeps its sampled columns for the backward
             t = timeit(lambda: _ops.deform_conv_train_op(xx, off, None, wt, None, [1, 1], [1, 1], [1, 1], grp, 1, 1), rep=10, warm=2)
-            add("deform_conv fwd C=%d %dx%d g=%d (bf16x3 tcgen05, training: saves columns)" % (cin, hh, ww, grp), t, tr,
+            add("deform_conv fwd C=%d %dx%d g=%d (bf16x3 wgmma, training: saves columns)" % (cin, hh, ww, grp), t, tr,
                 "%.2f TFLOP/s" % (flops / t / 1e6))
         except RuntimeError:
             pass
@@ -228,11 +228,11 @@ def main():
             y2 = tv.deform_conv2d(xg, og, wg, None, 1, 1, 1)
             tr = timeit(lambda: torch.autograd.grad(y2, (xg, og, wg), go, retain_graph=True), rep=3, warm=1)
         rc = refgpu.get("deform_conv bwd C=%d %dx%d g=%d" % (cin, hh, ww, grp))
-        add("deform_conv bwd C=%d %dx%d g=%d (auto: bf16x3 tcgen05)" % (cin, hh, ww, grp), t, tr if tv else None,
+        add("deform_conv bwd C=%d %dx%d g=%d (auto: bf16x3 wgmma)" % (cin, hh, ww, grp), t, tr if tv else None,
             "%.2f TFLOP/s; reference csrc CUDA: %s us" % (2 * flops / t / 1e6, ("%.1f" % rc) if rc else "n/a"))
 
     with open(args.out, "w") as f:
-        f.write("# Per-op timings on B200 (tools/bench_ops.py) — ours vs the reference's GPU kernels (torchvision %s CUDA ops)\n\n" %
+        f.write("# Per-op timings on H100 (tools/bench_ops.py) — ours vs the reference's GPU kernels (torchvision %s CUDA ops)\n\n" %
                 (getattr(__import__('torchvision'), '__version__', '?') if tv else 'n/a'))
         f.write("Eager launches incl. Python op dispatch (both sides); CUDA events, mean of back-to-back launches.\n\n")
         f.write("| op / shape | ours (us) | reference GPU (us) | speed-up | note |\n|---|---:|---:|---:|---|\n")

@@ -1,6 +1,6 @@
 """Timings of the REFERENCE's own GPU kernels on the box (the kernel-to-beat for the ops torchvision does not cover).
 
-Loads oracle/_ref/d2_ref_cuda.so -- the reference's csrc (CPU + CUDA) compiled for sm_100a by oracle/build.py
+Loads oracle/_ref/d2_ref_cuda.so -- the reference's csrc (CPU + CUDA) compiled for sm_90a by oracle/build.py
 (build_ref_cuda; SURVEY.md Appendix B.2) -- in a process that never imports detectron2_b200, so the two `detectron2::`
 op registrations cannot collide.  Writes gpurun_out/ref_gpu.json: {name: microseconds}.  Shapes match tools/bench_ops.py.
 """

@@ -1,4 +1,4 @@
-// Micro-benchmarks that bound the gather / scatter kernels (run on the B200 box; built by tools/build_microbench.sh):
+// Micro-benchmarks that bound the gather / scatter kernels (run on an H100; built by tools/build_microbench.sh):
 //   gather : random 256-byte runs (16 lanes x LDG.128, the channels-last tap pattern) out of an L2-resident buffer
 //   red    : red.global.add.f32 (scalar) vs red.global.add.v4.f32 with the same addressing
 // Prints GB/s of useful bytes and giga-operations/s.  Results are quoted in DESIGN.md next to the kernels they bound.
@@ -61,7 +61,7 @@ int main() {
     cudaMalloc(&buf, bytes);
     cudaMemset(buf, 0, bytes);
     const uint32_t nruns = (uint32_t)(bytes / 256);
-    const int blocks = 148 * 8, threads = 512, iters = 64;
+    const int blocks = 132 * 8, threads = 512, iters = 64;
     const double halfwarps = (double)blocks * threads / 16;
     // gather
     gather_kernel<<<blocks, threads>>>((const float4*)buf, nruns, iters, (float4*)buf);
