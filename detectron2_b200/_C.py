@@ -72,6 +72,10 @@ def _declare(lib):
         "d2b_roi_align_rotated_backward": (i, [f32p, f32p, i, f, i, i, i, i, i, i, i, f32p, vp]),
         "d2b_roi_align_rotated_forward_nhwc": (i, [f32p, i, i, i, i, f32p, i, f, i, i, i, f32p, vp]),
         "d2b_roi_align_rotated_backward_nhwc": (i, [f32p, f32p, i, f, i, i, i, i, i, i, i, f32p, vp]),
+        "d2b_roi_pooler_rotated_forward": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, f32p, vp]),
+        "d2b_roi_pooler_rotated_backward": (i, [C.POINTER(Pyramid), i, i, f32p, f32p, i, i, i, i, vp]),
+        "d2b_roi_pooler_rotated_forward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, vp, i, vp]),
+        "d2b_roi_pooler_rotated_backward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, vp, i, f32p, i, i, i, i, vp]),
         "d2b_nms_workspace_bytes": (sz, [i64, i, i64]),
         "d2b_nms": (i, [f32p, f32p, i64p, i64, d, i, i64, i64p, i64p, vp, sz, vp]),
         "d2b_rpn_prepare": (i, [C.POINTER(RpnLevels), i, f32p, f, i, f32p, f32p, f32p, f32p, i64p, vp, vp]),

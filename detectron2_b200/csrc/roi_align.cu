@@ -13,7 +13,9 @@
 //     that a whole multi-level ROIPooler call is one launch;
 //   * rotated forward: one CTA per (RoI, channel slab) with a 2-D tap table in shared memory (the sample grid of a
 //     rotated RoI is not a product grid), threads mapped to (channel, bin);
-//   * rotated backward: thread per (channel, bin), red.global.add per tap.
+//   * rotated backward: thread per (channel, bin), red.global.add per tap;
+//   * the rotated kernels (both layouts) pick the FPN level of a RoI in-kernel as well, from its w*h: a multi-level
+//     ROIPooler(pooler_type="ROIAlignRotated") call is one launch per direction.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -86,9 +88,12 @@ struct Pyr {
 
 // FPN level of a box: detectron2/modeling/poolers.py:54-62 (assign_boxes_to_levels), fp32 like torch:
 //   floor(canonical_level + log2(sqrt(area) / canonical_box_size + 1e-8)), clamped to [min_level, max_level]
+// `roi` is a pooler row: (b, x1, y1, x2, y2) with area (x2-x1)(y2-y1), or with ROT (b, cx, cy, w, h, angle) with area w*h
+// (RotatedBoxes.area, structures/rotated_boxes.py:236-245).
+template <bool ROT = false>
 __device__ __forceinline__ int pick_level(const Pyr& P, const float* __restrict__ roi) {
   if (P.num_levels == 1) return 0;
-  const float area = (roi[3] - roi[1]) * (roi[4] - roi[2]);
+  const float area = ROT ? roi[3] * roi[4] : (roi[3] - roi[1]) * (roi[4] - roi[2]);
   const float size = sqrtf(area);
   float lvl = floorf((float)P.canonical_level + log2f(size / P.canonical_box_size + 1e-8f));
   // A NaN level (negative or NaN area: malformed box) survives torch.clamp as NaN and matches no level in the reference's loop
@@ -204,16 +209,21 @@ __device__ __forceinline__ void rot_xy(const RoiGeom& g, int ph, int pw, int iy,
   x = yy * g.sin_t + xx * g.cos_t + g.ctr_w;
 }
 
+// The FPN level of the RoI is picked per CTA (single-level calls: num_levels == 1, level 0); a RoI without a level gets an
+// empty sampling grid, i.e. a zero output.
 template <int MAXTAP>
-__global__ void __launch_bounds__(kThreads) roi_align_rot_fwd_kernel(const float* __restrict__ in,
-                                                                     const float* __restrict__ rois, float scale,
-                                                                     int C, int H, int W, int PH, int PW, int sr,
-                                                                     int c_per_cta, float* __restrict__ out) {
+__global__ void __launch_bounds__(kThreads) roi_align_rot_fwd_kernel(const Pyr P, const float* __restrict__ rois,
+                                                                     int C, int PH, int PW, int sr, int c_per_cta,
+                                                                     float* __restrict__ out) {
   __shared__ Tap2 taps[MAXTAP];
   const int k = blockIdx.x;
   const int c0 = blockIdx.y * c_per_cta;
   const int cn = min(c_per_cta, C - c0);
-  const RoiGeom g = load_geom<true>(rois + (size_t)k * 6, scale, PH, PW, sr, 1);
+  const int lvl_raw = pick_level<true>(P, rois + (size_t)k * 6);
+  const int lvl = max(lvl_raw, 0);
+  const float* __restrict__ in = P.feat[lvl];
+  const int H = P.H[lvl], W = P.W[lvl];
+  const RoiGeom g = load_geom<true>(rois + (size_t)k * 6, P.scale[lvl], PH, PW, sr, 1, lvl_raw < 0);
   const int bins = PH * PW;
   const int spb = g.gh * g.gw;  // samples per bin
   const long long ntap = (long long)bins * spb;
@@ -265,7 +275,8 @@ __global__ void __launch_bounds__(kThreads) roi_align_bwd_kernel(const Pyr P, co
   const int k = blockIdx.x;
   const int c0 = blockIdx.y * c_per_cta;
   const int cn = min(c_per_cta, C - c0);
-  const int lvl_raw = ROT ? 0 : pick_level(P, (P.level_rois ? P.level_rois : rois) + (size_t)k * 5);
+  const int lvl_raw = ROT ? pick_level<true>(P, rois + (size_t)k * 6)  // rotated pyramids carry no level_rois
+                          : pick_level(P, (P.level_rois ? P.level_rois : rois) + (size_t)k * 5);
   const int lvl = max(lvl_raw, 0);
   float* __restrict__ gin = P.grad[lvl];
   const int H = P.H[lvl], W = P.W[lvl];
@@ -1426,19 +1437,25 @@ static int launch_bwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C,
 // scalar atomics per element (ROIAlignRotated_cuda.cu:143-222, :224-323).
 constexpr int kRotMaxTap = 1024;  // (bins x samples) entries of the shared tap table; larger grids compute taps on the fly
 
-template <bool BWD>
-__global__ void __launch_bounds__(kBwdThreads) roi_align_rot_nhwc_kernel(const float* __restrict__ in, float* __restrict__ gin,
-                                                                       const float* __restrict__ rois, float scale, int C,
-                                                                       int H, int W, int PH, int PW, int sr,
-                                                                       const float* __restrict__ gout,
-                                                                       float* __restrict__ out) {
+// The FPN level is picked per CTA (P.feat[l] / P.grad[l] are fp32 [N,H,W,C]); out / gout are [K,C,PH,PW] elements of DT
+// (fp32 arithmetic, half precision converted on load / store).
+template <bool BWD, int DT>
+__global__ void __launch_bounds__(kBwdThreads) roi_align_rot_nhwc_kernel(const Pyr P, const float* __restrict__ rois, int C,
+                                                                       int PH, int PW, int sr, const void* __restrict__ gout,
+                                                                       void* __restrict__ out) {
+  using E = Elem<DT>;
   extern __shared__ __align__(16) float tile[];  // forward: [128 ch][bins | 1] results; backward: [bin][128 ch] swizzled grads
   __shared__ Tap2 taps[kRotMaxTap];
   const int k = blockIdx.x;
   const int c0 = blockIdx.y * kNhwcCh;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int kWarps = kBwdThreads / 32;
-  const RoiGeom g = load_geom<true>(rois + (size_t)k * 6, scale, PH, PW, sr, 1);
+  const int lvl_raw = pick_level<true>(P, rois + (size_t)k * 6);
+  const int lvl = max(lvl_raw, 0);
+  const float* __restrict__ in = BWD ? nullptr : P.feat[lvl];
+  float* __restrict__ gin = BWD ? P.grad[lvl] : nullptr;
+  const int H = P.H[lvl], W = P.W[lvl];
+  const RoiGeom g = load_geom<true>(rois + (size_t)k * 6, P.scale[lvl], PH, PW, sr, 1, lvl_raw < 0);
   const int bins = PH * PW;
   const int spb = g.gh * g.gw;
   const int ncta = min(kNhwcCh, C - c0);
@@ -1455,10 +1472,10 @@ __global__ void __launch_bounds__(kBwdThreads) roi_align_rot_nhwc_kernel(const f
     }
   }
   if (BWD) {
-    const float* __restrict__ go = gout + ((size_t)k * C + c0) * bins;
+    const typename E::T* __restrict__ go = reinterpret_cast<const typename E::T*>(gout) + ((size_t)k * C + c0) * bins;
     for (int e = tid; e < ncta * bins; e += kBwdThreads) {
       const int c = e / bins, bin = e - c * bins;
-      tile[bin * kNhwcCh + ((((c >> 2) ^ bin) & 31) << 2) + (c & 3)] = __ldg(go + e) / g.count_raw;
+      tile[bin * kNhwcCh + ((((c >> 2) ^ bin) & 31) << 2) + (c & 3)] = E::ld(go + e) / g.count_raw;
     }
   }
   __syncthreads();
@@ -1508,23 +1525,41 @@ __global__ void __launch_bounds__(kBwdThreads) roi_align_rot_nhwc_kernel(const f
   }
   if (!BWD) {
     __syncthreads();
-    float* __restrict__ obase = out + ((size_t)k * C + c0) * bins;
+    typename E::T* __restrict__ obase = reinterpret_cast<typename E::T*>(out) + ((size_t)k * C + c0) * bins;
     for (int i = tid; i < ncta * bins; i += kBwdThreads) {  // channel-major write-out: contiguous runs of the NCHW-shaped output
       const int cl = i / bins, bl = i - cl * bins;
-      obase[i] = tile[((cl & 3) * 32 + (cl >> 2)) * pitch + bl];
+      E::st(obase + i, tile[((cl & 3) * 32 + (cl >> 2)) * pitch + bl]);
     }
   }
 }
 
+// dt: element type of `out` (forward) / `gout` (backward).  Every level's feature map (forward) or gradient map (backward)
+// must be 16-byte aligned -- checked by the callers.
 template <bool BWD>
-static int launch_rot_nhwc(const float* in, float* gin, const float* rois, int K, float scale, int C, int H, int W, int PH,
-                           int PW, int sr, const float* gout, float* out, cudaStream_t stream) {
-  if (C % 4 != 0 || (long long)H * W * (C / 4) >= (1LL << 28)) return D2B_EUNSUPPORTED;
-  const size_t smem = sizeof(float) * 128 * (size_t)(BWD ? PH * PW : ((PH * PW) | 1));
-  if (smem > 150 * 1024) return D2B_EUNSUPPORTED;
-  D2B_ALLOW_BIG_SMEM(roi_align_rot_nhwc_kernel<BWD>);
+static size_t rot_nhwc_smem(int PH, int PW) {
+  return sizeof(float) * 128 * (size_t)(BWD ? PH * PW : ((PH * PW) | 1));
+}
+
+// Shapes the channels-last rotated kernel takes (D2B_OK) or not (D2B_EUNSUPPORTED); host-only, launches nothing.
+template <bool BWD>
+static int rot_nhwc_supported(const Pyr& P, int C, int PH, int PW) {
+  if (C % 4 != 0) return D2B_EUNSUPPORTED;
+  for (int l = 0; l < P.num_levels; ++l)
+    if ((long long)P.H[l] * P.W[l] * (C / 4) >= (1LL << 28)) return D2B_EUNSUPPORTED;
+  if (rot_nhwc_smem<BWD>(PH, PW) > 150 * 1024) return D2B_EUNSUPPORTED;
+  return D2B_OK;
+}
+
+template <bool BWD>
+static int launch_rot_nhwc(const Pyr& P, const float* rois, int K, int C, int PH, int PW, int sr, const void* gout, void* out,
+                           cudaStream_t stream, int dt = D2B_F32) {
+  if (int rc = rot_nhwc_supported<BWD>(P, C, PH, PW)) return rc;
+  const size_t smem = rot_nhwc_smem<BWD>(PH, PW);
   dim3 grid(K, d2b_cdiv(C, kNhwcCh));
-  roi_align_rot_nhwc_kernel<BWD><<<grid, kBwdThreads, smem, stream>>>(in, gin, rois, scale, C, H, W, PH, PW, sr, gout, out);
+  D2B_DISPATCH_DTYPE(dt, {
+    D2B_ALLOW_BIG_SMEM((roi_align_rot_nhwc_kernel<BWD, DT>));
+    roi_align_rot_nhwc_kernel<BWD, DT><<<grid, kBwdThreads, smem, stream>>>(P, rois, C, PH, PW, sr, gout, out);
+  });
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }
@@ -1759,8 +1794,13 @@ D2B_API int d2b_roi_align_rotated_forward_nhwc(const float* input, int N, int C,
   if (K == 0 || C == 0) return D2B_OK;
   if (!input || !rois || !out || N <= 0 || H <= 0 || W <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0) return D2B_EINVAL;
   if ((reinterpret_cast<uintptr_t>(input) & 15) != 0) return D2B_EINVAL;
-  return launch_rot_nhwc<false>(input, nullptr, rois, K, spatial_scale, C, H, W, pooled_h, pooled_w, sampling_ratio, nullptr,
-                                out, (cudaStream_t)stream);
+  Pyr P = {};
+  P.num_levels = 1;
+  P.feat[0] = input;
+  P.H[0] = H;
+  P.W[0] = W;
+  P.scale[0] = spatial_scale;
+  return launch_rot_nhwc<false>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, nullptr, out, (cudaStream_t)stream);
 }
 
 D2B_API int d2b_roi_align_rotated_backward_nhwc(const float* grad_out, const float* rois, int K, float spatial_scale,
@@ -1772,8 +1812,13 @@ D2B_API int d2b_roi_align_rotated_backward_nhwc(const float* grad_out, const flo
   if (bytes) D2B_CUDA(cudaMemsetAsync(grad_in, 0, bytes, (cudaStream_t)stream));
   if (K == 0 || bytes == 0) return D2B_OK;
   if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  return launch_rot_nhwc<true>(nullptr, grad_in, rois, K, spatial_scale, C, H, W, pooled_h, pooled_w, sampling_ratio, grad_out,
-                               nullptr, (cudaStream_t)stream);
+  Pyr P = {};
+  P.num_levels = 1;
+  P.grad[0] = grad_in;
+  P.H[0] = H;
+  P.W[0] = W;
+  P.scale[0] = spatial_scale;
+  return launch_rot_nhwc<true>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, grad_out, nullptr, (cudaStream_t)stream);
 }
 
 D2B_API int d2b_roi_pooler_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
@@ -1845,10 +1890,16 @@ D2B_API int d2b_roi_align_rotated_forward(const float* input, int N, int C, int 
   if (K == 0 || C == 0) return D2B_OK;
   if (!input || !rois || !out || N <= 0 || H <= 0 || W <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0)
     return D2B_EINVAL;
+  Pyr P = {};
+  P.num_levels = 1;
+  P.feat[0] = input;
+  P.H[0] = H;
+  P.W[0] = W;
+  P.scale[0] = spatial_scale;
   int cpc = pick_c_per_cta(K, C);
   dim3 grid(K, d2b_cdiv(C, cpc));
-  roi_align_rot_fwd_kernel<1024><<<grid, kThreads, 0, (cudaStream_t)stream>>>(
-      input, rois, spatial_scale, C, H, W, pooled_h, pooled_w, sampling_ratio, cpc, out);
+  roi_align_rot_fwd_kernel<1024><<<grid, kThreads, 0, (cudaStream_t)stream>>>(P, rois, C, pooled_h, pooled_w, sampling_ratio,
+                                                                               cpc, out);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }
@@ -1890,4 +1941,87 @@ D2B_API int d2b_roi_align_rotated_backward(const float* grad_out, const float* r
                                            float* grad_in, void* stream) {
   return roi_bwd_launch<true>(grad_out, rois, K, spatial_scale, pooled_h, pooled_w, N, C, H, W, sampling_ratio, 1,
                               grad_in, stream);
+}
+
+// ------------------------------------------------------------------ multi-level rotated pooler
+// ROIPooler(pooler_type="ROIAlignRotated") with several levels: the per-level loop of detectron2/modeling/poolers.py:245-263 as
+// one launch per direction, the level of each RoI picked in-kernel from its w*h.  The reference samples rotated RoIs in fp32
+// whatever the feature dtype (layers/roi_align_rotated.py:81-83), so there are no separate level boxes: level_rois must be
+// NULL.  Every argument is checked before anything is launched.
+static int rot_pooler_args(const d2b_pyramid* pyr, int N, int C, int K, int dtype, Pyr& P) {
+  if (!make_pyr(pyr, P) || P.level_rois || N < 0 || C < 0 || K < 0 || !dtype_ok(dtype)) return D2B_EINVAL;
+  if (N == 0 && K > 0) return D2B_EINVAL;  // RoIs of images that do not exist
+  return D2B_OK;
+}
+
+static int rot_pooler_zero_grads(const Pyr& P, int N, int C, cudaStream_t stream) {
+  void* zp[D2B_MAX_LEVELS];
+  size_t zb[D2B_MAX_LEVELS];
+  for (int l = 0; l < P.num_levels; ++l) {
+    zp[l] = P.grad[l];
+    zb[l] = sizeof(float) * (size_t)N * C * P.H[l] * P.W[l];
+  }
+  return d2b_zero_buffers(zp, zb, P.num_levels, stream);  // all levels zero-filled by one launch
+}
+
+D2B_API int d2b_roi_pooler_rotated_forward(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
+                                           int pooled_w, int sampling_ratio, float* out, void* stream) {
+  Pyr P;
+  if (rot_pooler_args(pyr, N, C, K, D2B_F32, P)) return D2B_EINVAL;
+  if (K == 0 || C == 0) return D2B_OK;
+  if (!rois || !out || N <= 0 || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
+  for (int l = 0; l < P.num_levels; ++l)
+    if (!P.feat[l]) return D2B_EINVAL;
+  int cpc = pick_c_per_cta(K, C);
+  dim3 grid(K, d2b_cdiv(C, cpc));
+  roi_align_rot_fwd_kernel<1024><<<grid, kThreads, 0, (cudaStream_t)stream>>>(P, rois, C, pooled_h, pooled_w, sampling_ratio,
+                                                                               cpc, out);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
+}
+
+D2B_API int d2b_roi_pooler_rotated_forward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
+                                                  int pooled_w, int sampling_ratio, void* out, int out_dtype, void* stream) {
+  Pyr P;
+  if (rot_pooler_args(pyr, N, C, K, out_dtype, P)) return D2B_EINVAL;
+  if (K == 0 || C == 0) return D2B_OK;
+  if (!rois || !out || N <= 0 || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
+  for (int l = 0; l < P.num_levels; ++l)
+    if (!P.feat[l] || (reinterpret_cast<uintptr_t>(P.feat[l]) & 15) != 0) return D2B_EINVAL;
+  return launch_rot_nhwc<false>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, nullptr, out, (cudaStream_t)stream,
+                                out_dtype);
+}
+
+D2B_API int d2b_roi_pooler_rotated_backward(const d2b_pyramid* pyr, int N, int C, const float* grad_out, const float* rois,
+                                            int K, int pooled_h, int pooled_w, int sampling_ratio, void* stream) {
+  Pyr P;
+  if (rot_pooler_args(pyr, N, C, K, D2B_F32, P)) return D2B_EINVAL;
+  if (N == 0 || C == 0) return D2B_OK;  // no gradient element to write
+  for (int l = 0; l < P.num_levels; ++l)
+    if (!P.grad[l]) return D2B_EINVAL;
+  if (K > 0 && (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0)) return D2B_EINVAL;
+  int rc = rot_pooler_zero_grads(P, N, C, (cudaStream_t)stream);
+  if (rc || K == 0) return rc;
+  int cpc = pick_c_per_cta(K, C);
+  dim3 grid(K, d2b_cdiv(C, cpc));
+  roi_align_bwd_kernel<true><<<grid, kThreads, 0, (cudaStream_t)stream>>>(P, grad_out, rois, C, pooled_h, pooled_w,
+                                                                          sampling_ratio, 1, cpc);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
+}
+
+D2B_API int d2b_roi_pooler_rotated_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
+                                                   const float* rois, int K, int pooled_h, int pooled_w, int sampling_ratio,
+                                                   void* stream) {
+  Pyr P;
+  if (rot_pooler_args(pyr, N, C, K, grad_dtype, P)) return D2B_EINVAL;
+  if (N == 0 || C == 0) return D2B_OK;
+  for (int l = 0; l < P.num_levels; ++l)
+    if (!P.grad[l] || (reinterpret_cast<uintptr_t>(P.grad[l]) & 15) != 0) return D2B_EINVAL;
+  if (K > 0 && (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0)) return D2B_EINVAL;
+  if (int rc = K > 0 ? rot_nhwc_supported<true>(P, C, pooled_h, pooled_w) : D2B_OK) return rc;  // before the zero-fill
+  int rc = rot_pooler_zero_grads(P, N, C, (cudaStream_t)stream);
+  if (rc || K == 0) return rc;
+  return launch_rot_nhwc<true>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, grad_out, nullptr, (cudaStream_t)stream,
+                               grad_dtype);
 }

@@ -365,14 +365,24 @@ _ROT_NHWC_PS = (10.0, 16.0)  # rotated channels-last kernels
 
 
 def _rot_layout(n: int, c: int, h: int, w: int, n_out: int, channels_last: bool, bwd: bool) -> str:
-    if c % 4 != 0 or POOLER_LAYOUT == "nchw" or h * w * (c // 4) >= 2 ** 28:
+    return _rot_pyramid_layout([(n, c, h, w)], n_out, channels_last, bwd)
+
+
+def _rot_pyramid_layout(shapes_nchw, n_out: int, channels_last: bool, bwd: bool, bins: int = 0) -> str:
+    """Rotated kernels: 'cl', 'xpose' or 'nchw' as in _bwd_layout, for a pyramid of (n, c, h, w) levels.  bins: pooled
+    h * w when known; the channels-last kernel keeps a [128 channels][bins] fp32 tile in shared memory (<= 150 KB)."""
+    c = shapes_nchw[0][1]
+    if c % 4 != 0 or POOLER_LAYOUT == "nchw" or any(h * w * (c // 4) >= 2 ** 28 for (_, _, h, w) in shapes_nchw):
+        return "nchw"
+    if 4 * 128 * (bins | 1) > 150 * 1024:
         return "nchw"
     if channels_last:
         return "cl"
     if POOLER_LAYOUT == "nhwc":
         return "xpose"
     i = 1 if bwd else 0
-    return "xpose" if n_out * _ROT_NHWC_PS[i] + 4 * n * c * h * w * _XPOSE_PS_PER_BYTE < n_out * _ROT_NCHW_PS[i] else "nchw"
+    feat_bytes = 4 * sum(n * c * h * w for (n, c, h, w) in shapes_nchw)
+    return "xpose" if n_out * _ROT_NHWC_PS[i] + feat_bytes * _XPOSE_PS_PER_BYTE < n_out * _ROT_NCHW_PS[i] else "nchw"
 
 
 @torch.library.custom_op("d2b200::roi_align_rotated", mutates_args=(), device_types="cuda")
@@ -447,6 +457,122 @@ def _roi_rot_bwd(ctx, grad):
 
 
 roi_align_rotated_op.register_autograd(_roi_rot_bwd, setup_context=_roi_rot_setup)
+
+
+# ----------------------------------------------------------------------------------- fused multi-level rotated pooler
+@torch.library.custom_op("d2b200::roi_pooler_rotated", mutates_args=(), device_types="cuda")
+def roi_pooler_rotated_op(feats: List[Tensor], rois: Tensor, scales: List[float], pooled_h: int, pooled_w: int,
+                          sampling_ratio: int, min_level: int, max_level: int, canonical_level: int,
+                          canonical_box_size: float) -> Tensor:
+    """ROIPooler(pooler_type="ROIAlignRotated") over several levels in one launch: rois [K,6] = (batch, cx, cy, w, h, angle),
+    the level of each from w*h.  The rois are used in fp32 whatever the feature dtype (layers/roi_align_rotated.py:81-83)."""
+    _C.require_cuda(rois, *feats)
+    if len(feats) < 1 or len(feats) > _C.MAX_LEVELS or len(feats) != len(scales):
+        raise RuntimeError("roi_pooler_rotated: need 1..%d feature levels with one scale each" % _C.MAX_LEVELS)
+    _roi_common(feats[0], rois, 6)
+    r = _f32c(rois)
+    n, c = feats[0].shape[:2]
+    k = r.shape[0]
+    numel = k * c * pooled_h * pooled_w
+    cl = all(_is_channels_last(t) and t.data_ptr() % 16 == 0 for t in feats)
+    layout = (_rot_pyramid_layout([(n, c, t.shape[2], t.shape[3]) for t in feats], numel, cl, False, pooled_h * pooled_w)
+              if numel else "nchw")
+    # half-precision NCHW levels: the layout-change launch reads them as they are (it is also the up-cast) and the pooling
+    # kernel writes the result in their dtype; every other combination computes on fp32 copies
+    fused_half = layout == "xpose" and _same_half_dtype(feats)
+    fs = list(feats) if fused_half else [t.to(dtype=torch.float32) for t in feats]
+    out_dt = feats[0].dtype if (layout != "nchw" and feats[0].dtype in _C.DTYPE_CODE) else torch.float32
+    out = torch.empty((k, c, pooled_h, pooled_w), dtype=out_dt, device=r.device)
+    if numel:
+        with torch.cuda.device(r.device):
+            if layout != "cl":
+                fs = [t.contiguous() for t in fs]
+            P = _pyramid(fs, None, scales, min_level, max_level, canonical_level, canonical_box_size)
+            if layout == "nchw":
+                check(_C.lib().d2b_roi_pooler_rotated_forward(C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w, sampling_ratio,
+                                                              ptr(out), stream_ptr(r.device)), "roi_pooler_rotated_forward")
+            else:
+                if layout == "xpose":
+                    bufs = _to_nhwc(fs, P, n, c, r.device)
+                    for l, b in enumerate(bufs):
+                        P.feat[l] = b.data_ptr()
+                check(_C.lib().d2b_roi_pooler_rotated_forward_nhwc_t(C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w,
+                                                                     sampling_ratio, ptr(out), _C.DTYPE_CODE[out_dt],
+                                                                     stream_ptr(r.device)), "roi_pooler_rotated_forward_nhwc")
+    return out if out.dtype == feats[0].dtype else out.to(feats[0].dtype)
+
+
+@roi_pooler_rotated_op.register_fake
+def _(feats, rois, scales, pooled_h, pooled_w, sampling_ratio, min_level, max_level, canonical_level, canonical_box_size):
+    return feats[0].new_empty((rois.shape[0], feats[0].shape[1], pooled_h, pooled_w))
+
+
+@torch.library.custom_op("d2b200::roi_pooler_rotated_backward", mutates_args=(), device_types="cuda")
+def roi_pooler_rotated_backward_op(grad: Tensor, rois: Tensor, shapes: List[int], scales: List[float], pooled_h: int,
+                                   pooled_w: int, sampling_ratio: int, min_level: int, max_level: int, canonical_level: int,
+                                   canonical_box_size: float, channels_last: bool = False,
+                                   half_grads: bool = False) -> List[Tensor]:
+    """Gradients of roi_pooler_rotated for every level; shapes = [n, c, h0, w0, h1, w1, ...].  `half_grads`: return NCHW
+    gradients in `grad`'s fp16 / bf16 dtype (written by the layout-change launch) instead of fp32."""
+    _C.require_cuda(grad, rois)
+    r = _f32c(rois)
+    nl = len(scales)
+    n, c = shapes[0], shapes[1]
+    hw = [(shapes[2 + 2 * l], shapes[3 + 2 * l]) for l in range(nl)]
+    layout = (_rot_pyramid_layout([(n, c, h, w) for (h, w) in hw], grad.numel(), channels_last, True, pooled_h * pooled_w)
+              if n * c else "nchw")
+    # the channels-last kernel reads fp16 / bf16 gradients in place; the NCHW kernel takes fp32
+    g = grad.contiguous() if (layout != "nchw" and grad.dtype in _C.DTYPE_CODE) else _f32c(grad)
+    with torch.cuda.device(g.device):
+        if layout == "nchw":
+            grads = [torch.empty((n, c, h, w), dtype=torch.float32, device=g.device) for (h, w) in hw]
+            P = _pyramid(grads, grads, scales, min_level, max_level, canonical_level, canonical_box_size)
+            check(_C.lib().d2b_roi_pooler_rotated_backward(C.byref(P), n, c, ptr(g), ptr(r), r.shape[0], pooled_h, pooled_w,
+                                                           sampling_ratio, stream_ptr(g.device)), "roi_pooler_rotated_backward")
+        else:
+            bufs = [torch.empty((n, h, w, c), dtype=torch.float32, device=g.device) for (h, w) in hw]
+            views = [b.permute(0, 3, 1, 2) for b in bufs]  # logical NCHW shape: _pyramid reads H, W from dims 2, 3
+            P = _pyramid(views, views, scales, min_level, max_level, canonical_level, canonical_box_size)
+            check(_C.lib().d2b_roi_pooler_rotated_backward_nhwc_t(C.byref(P), n, c, ptr(g), _C.DTYPE_CODE[g.dtype], ptr(r),
+                                                                  r.shape[0], pooled_h, pooled_w, sampling_ratio,
+                                                                  stream_ptr(g.device)), "roi_pooler_rotated_backward_nhwc")
+            if layout == "cl":
+                grads = views
+            else:
+                grads = _from_nhwc(bufs, n, c, g.device, grad.dtype if (half_grads and grad.dtype in _HALF) else torch.float32)
+    if half_grads and grad.dtype in _HALF:
+        grads = [t if t.dtype == grad.dtype else t.to(grad.dtype) for t in grads]
+    return grads
+
+
+@roi_pooler_rotated_backward_op.register_fake
+def _(grad, rois, shapes, scales, pooled_h, pooled_w, sampling_ratio, min_level, max_level, canonical_level,
+      canonical_box_size, channels_last=False, half_grads=False):
+    n, c = shapes[0], shapes[1]
+    dt = grad.dtype if half_grads else torch.float32
+    outs = [grad.new_empty((n, c, shapes[2 + 2 * l], shapes[3 + 2 * l]), dtype=dt) for l in range(len(scales))]
+    return [o.contiguous(memory_format=torch.channels_last) for o in outs] if channels_last else outs
+
+
+def _pooler_rot_setup(ctx, inputs, output):
+    feats, rois, scales, ph, pw, sr, lo, hi, cl, cs = inputs
+    ctx.save_for_backward(rois)
+    shapes = [feats[0].shape[0], feats[0].shape[1]]
+    for t in feats:
+        shapes += [t.shape[2], t.shape[3]]
+    ctx.args = (shapes, scales, ph, pw, sr, lo, hi, cl, cs, [t.dtype for t in feats],
+                all(_is_channels_last(t) for t in feats))
+
+
+def _pooler_rot_bwd(ctx, grad):
+    (rois,) = ctx.saved_tensors
+    shapes, scales, ph, pw, sr, lo, hi, cl, cs, dts, chl = ctx.args
+    half = dts[0] in _HALF and grad.dtype == dts[0] and all(d == dts[0] for d in dts)
+    grads = roi_pooler_rotated_backward_op(grad, rois, shapes, scales, ph, pw, sr, lo, hi, cl, cs, chl, half)
+    return [g.to(dt) for g, dt in zip(grads, dts)], None, None, None, None, None, None, None, None, None
+
+
+roi_pooler_rotated_op.register_autograd(_pooler_rot_bwd, setup_context=_pooler_rot_setup)
 
 
 # =================================================================================== NMS / rotated IoU

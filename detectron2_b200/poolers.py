@@ -24,9 +24,13 @@ def _tensor_of(b):
 
 
 def assign_boxes_to_levels(box_lists, min_level: int, max_level: int, canonical_box_size: int, canonical_level: int):
-    """Host-side restatement of poolers.py:23-59 for callers that want the assignment vector itself."""
+    """Host-side restatement of poolers.py:23-59 for callers that want the assignment vector itself.  Boxes are (x1, y1, x2, y2)
+    or rotated (cx, cy, w, h, angle), whose area is w*h (RotatedBoxes.area, structures/rotated_boxes.py:236-245)."""
     boxes = torch.cat([_tensor_of(b) for b in box_lists], dim=0)
-    sizes = torch.sqrt((boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1]))
+    if boxes.shape[1] == 5:
+        sizes = torch.sqrt(boxes[:, 2] * boxes[:, 3])
+    else:
+        sizes = torch.sqrt((boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1]))
     lv = torch.floor(canonical_level + torch.log2(sizes / canonical_box_size + 1e-8))
     return torch.clamp(lv, min=min_level, max=max_level).to(torch.int64) - min_level
 
@@ -82,15 +86,10 @@ class ROIPooler(nn.Module):
                                  self.max_level, self.canonical_level, float(self.canonical_box_size))
 
     def _forward_rotated(self, x, box_lists, rois):
-        # rotated boxes: area = w*h (RotatedBoxes.area); per-level loop as in the reference (not a BASELINE config)
+        # one level: the ROIAlignRotated layer, as in the reference (poolers.py:245-246); several: one fused launch per
+        # direction, the level of each rotated box (area = w*h, RotatedBoxes.area) picked in-kernel
         if len(self.scales) == 1:
             return self.level_poolers[0](x[0], rois)
-        boxes = rois[:, 1:]
-        sizes = torch.sqrt(boxes[:, 2] * boxes[:, 3])
-        lv = torch.floor(self.canonical_level + torch.log2(sizes / self.canonical_box_size + 1e-8))
-        lv = torch.clamp(lv, min=self.min_level, max=self.max_level).to(torch.int64) - self.min_level
-        out = x[0].new_zeros((rois.shape[0], x[0].shape[1]) + tuple(self.output_size))
-        for level, pooler in enumerate(self.level_poolers):
-            inds = torch.nonzero(lv == level, as_tuple=True)[0]
-            out.index_put_((inds,), pooler(x[level], rois[inds]))
-        return out
+        return ops.roi_pooler_rotated_op(list(x), rois, self.scales, self.output_size[0], self.output_size[1],
+                                         int(self.sampling_ratio), self.min_level, self.max_level, self.canonical_level,
+                                         float(self.canonical_box_size))

@@ -137,6 +137,30 @@ int d2b_roi_align_rotated_backward_nhwc(const float* grad_out, const float* rois
                                         float spatial_scale, int pooled_h, int pooled_w, int N, int C,
                                         int H, int W, int sampling_ratio, float* grad_in, void* stream);
 
+/* ---- Multi-level rotated RoI pooler (fused) ------------------------------------------------
+ * Replaces the per-level loop of detectron2/modeling/poolers.py:245-263 for pooler_type "ROIAlignRotated" (nonzero /
+ * gather / roi_align_rotated / index_put_ per level): one launch per direction, no host synchronisation.  Level rule of
+ * d2b_roi_pooler_forward with area = w*h of the (batch_idx,cx,cy,w,h,angle_degrees) row (RotatedBoxes.area,
+ * structures/rotated_boxes.py:236-245); a negative or NaN area matches no level: zero output, no gradient.
+ * rois [K,6]; pyr->level_rois must be NULL (the reference samples rotated RoIs in fp32 whatever the feature dtype,
+ * layers/roi_align_rotated.py:81-83).  pyr->grad[l] are fully written by the backward (all levels zero-filled by one launch,
+ * then accumulated).  Every argument is checked before anything is launched.
+ *   d2b_roi_pooler_rotated_forward / _backward            feat[l] / grad[l] NCHW fp32, out / grad_out [K,C,PH,PW] fp32
+ *   d2b_roi_pooler_rotated_forward_nhwc_t / _backward_nhwc_t
+ *       feat[l] / grad[l] fp32 [N,H,W,C] storage, 16-byte aligned, C % 4 == 0; out / grad_out [K,C,PH,PW] elements of
+ *       out_dtype / grad_dtype (D2B_F32 / D2B_F16 / D2B_BF16 above; fp32 arithmetic, grad[l] stay fp32); D2B_EUNSUPPORTED
+ *       when a [128][PH*PW] fp32 tile exceeds 150 KB of shared memory (use the NCHW form).
+ * N == 0 with K > 0 is D2B_EINVAL (RoIs of images that do not exist). */
+int d2b_roi_pooler_rotated_forward(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
+                                   int pooled_w, int sampling_ratio, float* out, void* stream);
+int d2b_roi_pooler_rotated_backward(const d2b_pyramid* pyr, int N, int C, const float* grad_out, const float* rois,
+                                    int K, int pooled_h, int pooled_w, int sampling_ratio, void* stream);
+int d2b_roi_pooler_rotated_forward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
+                                          int pooled_w, int sampling_ratio, void* out, int out_dtype, void* stream);
+int d2b_roi_pooler_rotated_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
+                                           const float* rois, int K, int pooled_h, int pooled_w, int sampling_ratio,
+                                           void* stream);
+
 /* ---- NMS --------------------------------------------------------------------------------
  * Replaces torchvision::nms reached from detectron2/layers/nms.py:5-22 (nms, batched_nms) and
  * torch.ops.detectron2.nms_rotated (csrc/vision.cpp:116, csrc/nms_rotated/nms_rotated.h:22-37).

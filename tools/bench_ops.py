@@ -48,6 +48,42 @@ def ref_pooler_grad(fg, b, out, scales, tv):
     return res
 
 
+def per_level_rotated_pooler(feats, rois, scales, out):
+    """This library's multi-level rotated ROIPooler before the fused kernels: the reference's per-level loop
+    (poolers.py:245-263) over the single-level ROIAlignRotated layer."""
+    sizes = torch.sqrt(rois[:, 3] * rois[:, 4])
+    lv = torch.floor(4 + torch.log2(sizes / 224 + 1e-8)).clamp(2, 5).to(torch.int64) - 2
+    res = feats[0].new_zeros((rois.shape[0], feats[0].shape[1], out, out))
+    for l, s in enumerate(scales):
+        inds = torch.nonzero(lv == l, as_tuple=True)[0]
+        res.index_put_((inds,), L.ROIAlignRotated((out, out), s, 0)(feats[l], rois[inds]))
+    return res
+
+
+def bench_rotated_pooler(add, refgpu):
+    """Rotated ROIPooler, 2 images x 512 RoIs, 7x7, p2..p5 at 256 channels: the fused op, this library's former per-level loop
+    and (tools/bench_ref_gpu.py) the same loop over the reference's CUDA roi_align_rotated kernels."""
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    from bench_ref_gpu import rotated_pooler_inputs
+
+    feats, boxes, scales = rotated_pooler_inputs()
+    rois = torch.cat([torch.cat([torch.full((len(b), 1), float(i), device=DEV), b], 1) for i, b in enumerate(boxes)])
+    pooler = ROIPooler(7, scales, 0, "ROIAlignRotated")
+    name = "ROIPooler ROIAlignRotated %s 7x7 K=2x512 (p2..p5)"
+    t = timeit(lambda: pooler(feats, boxes))
+    add(name % "fwd", t, refgpu.get(name % "fwd"), "fused; ref = per-level loop over reference csrc CUDA")
+    t = timeit(lambda: per_level_rotated_pooler(feats, rois, scales, 7))
+    add(name % "fwd" + " former loop", t, refgpu.get(name % "fwd"), "per-level loop over our ROIAlignRotated")
+    fg = [f.clone().requires_grad_(True) for f in feats]
+    y = pooler(fg, boxes)
+    go = torch.randn_like(y)
+    t = timeit(lambda: torch.autograd.grad(y, fg, go, retain_graph=True))
+    add(name % "bwd", t, refgpu.get(name % "bwd"), "fused; ref = per-level reference csrc CUDA backward")
+    y2 = per_level_rotated_pooler(fg, rois, scales, 7)
+    t = timeit(lambda: torch.autograd.grad(y2, fg, go, retain_graph=True))
+    add(name % "bwd" + " former loop", t, refgpu.get(name % "bwd"), "autograd of the per-level loop over our ROIAlignRotated")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "r2_ops.md"))
@@ -192,6 +228,7 @@ def main():
     gor = torch.randn_like(yr)
     t = timeit(lambda: torch.autograd.grad(yr, xrg, gor, retain_graph=True))
     add("roi_align_rotated bwd 512 boxes, 2x256x50x84", t, refgpu.get("roi_align_rotated bwd 512 boxes, 2x256x50x84"), "ref = reference csrc CUDA")
+    bench_rotated_pooler(add, refgpu)
     # ---- paste
     masks, det = d["masks"].to(DEV), d["det_boxes"][:100].to(DEV)
     t = timeit(lambda: L.paste_masks_in_image(masks, det, (800, 1333), 0.5))

@@ -53,10 +53,60 @@ def paste_gpu_branch(masks, boxes, img_h, img_w, threshold=0.5):
     return out
 
 
+def rotated_pooler_inputs(device=DEV):
+    """Rotated ROIPooler bench shape (also used by tools/bench_ops.py): 2 images x 512 rotated RoIs, p2..p5 of an 800x1344
+    image at 256 channels, sizes log-uniform in [16, 800], angles uniform in (-180, 180]."""
+    g = torch.Generator().manual_seed(31)
+    feats = [torch.randn(2, 256, 200 // 2 ** l, 336 // 2 ** l, generator=g).to(device) for l in range(4)]
+    boxes = []
+    for _ in range(2):
+        s = torch.exp(torch.rand(512, generator=g) * (math.log(800) - math.log(16)) + math.log(16))
+        ar = torch.exp((torch.rand(512, generator=g) - 0.5) * 1.4)
+        ctr = torch.rand(512, 2, generator=g) * torch.tensor([1344.0, 800.0])
+        ang = 180.0 - torch.rand(512, generator=g) * 360.0
+        boxes.append(torch.cat([ctr, (s * ar.sqrt())[:, None], (s / ar.sqrt())[:, None], ang[:, None]], 1).to(device))
+    return feats, boxes, [1 / 4, 1 / 8, 1 / 16, 1 / 32]
+
+
+def time_rotated_pooler(D, res):
+    """The reference's ROIPooler(pooler_type="ROIAlignRotated") structure (poolers.py:245-263): level assignment, then per level
+    nonzero / gather / roi_align_rotated_forward / index_put_; the backward as its autograd does it (per level: gather of the
+    output gradient rows, zero-filled gradient map, roi_align_rotated_backward)."""
+    feats, boxes, scales = rotated_pooler_inputs()
+    rois = torch.cat([torch.cat([torch.full((len(b), 1), float(i), device=DEV), b], 1) for i, b in enumerate(boxes)])
+
+    def levels():
+        sizes = torch.sqrt(rois[:, 3] * rois[:, 4])
+        return torch.floor(4 + torch.log2(sizes / 224 + 1e-8)).clamp(2, 5).to(torch.int64) - 2
+
+    def fwd():
+        lv = levels()
+        out = torch.zeros(len(rois), 256, 7, 7, device=DEV)
+        for l, s in enumerate(scales):
+            inds = torch.nonzero(lv == l, as_tuple=True)[0]
+            out.index_put_((inds,), D.roi_align_rotated_forward(feats[l], rois[inds], s, 7, 7, 0))
+        return out
+
+    go = torch.randn(len(rois), 256, 7, 7, device=DEV)
+
+    def bwd():
+        lv = levels()
+        grads = []
+        for l, s in enumerate(scales):
+            inds = torch.nonzero(lv == l, as_tuple=True)[0]
+            n, c, h, w = feats[l].shape
+            grads.append(D.roi_align_rotated_backward(go[inds], rois[inds], s, 7, 7, n, c, h, w, 0))
+        return grads
+
+    res["ROIPooler ROIAlignRotated fwd 7x7 K=2x512 (p2..p5)"] = timeit(fwd)
+    res["ROIPooler ROIAlignRotated bwd 7x7 K=2x512 (p2..p5)"] = timeit(bwd)
+
+
 def main():
     res = {}
     torch.ops.load_library(SO)
     D = torch.ops.detectron2
+    time_rotated_pooler(D, res)
     spec = importlib.util.spec_from_loader("d2_ref_cuda", importlib.machinery.ExtensionFileLoader("d2_ref_cuda", SO))
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)
