@@ -199,13 +199,24 @@ __device__ __forceinline__ unsigned enc_f(float f) {
 __device__ __forceinline__ float dec_f(unsigned u) {
   return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
 }
+// canonical value for the ordered encoding: -0.0 becomes +0.0 and every NaN the one positive NaN, which enc_f places above
+// +inf.  This is the score order of torch.sort(descending=True, stable=True): NaN first, +-0 equal.
+__device__ __forceinline__ float canon_f(float f) { return f != f ? __uint_as_float(0x7fc00000u) : (f == 0.f ? 0.f : f); }
+// 64-bit key of box i in the stable descending score order (ascending key == score order; distinct for distinct i)
+__device__ __forceinline__ unsigned long long score_key(float s, int i) {
+  return ((unsigned long long)(~enc_f(canon_f(s))) << 32) | (unsigned)i;
+}
+// max / min that return NaN when either operand is NaN, like torch.max / torch.min (fmaxf / fminf drop the NaN)
+__device__ __forceinline__ float max_nan(float a, float b) { return (a > b || a != a) ? a : b; }
+__device__ __forceinline__ float min_nan(float a, float b) { return (a < b || a != a) ? a : b; }
 
 // ---- kernel 1: order by counting.  One warp per TWO boxes; the scores / categories of all boxes stream through shared
-// memory once per CTA.  For box i:
-//   grank = #{j : s_j > s_i or (s_j == s_i and j < i)}                 position in the stable descending score order
-//   pos   = #{j : c_j < c_i} + #{j : c_j == c_i and j before i}        position in the category-major order
+// memory once per CTA.  For box i, with k_i = score_key(s_i, i):
+//   grank = #{j : k_j < k_i}                                           position in the stable descending score order
+//   pos   = #{j : c_j < c_i} + #{j : c_j == c_i and k_j < k_i}         position in the category-major order
 // which is what two stable radix sorts would produce -- but in one launch, with the segment bounds of every position and
-// the segment list as by-products.  O(M^2 / 32) warp steps: 3 us at M = 8819, ~3 ms at M = 100 000.
+// the segment list as by-products.  The keys are distinct, so grank and pos are permutations of [0, M) whatever the scores
+// (NaN, +-0): the scan indexes with them.  O(M^2 / 32) warp steps: 3 us at M = 8819, ~3 ms at M = 100 000.
 constexpr int kRankTile = 1792;
 constexpr int kRankWarps = 8;
 constexpr int kRankHist = 4096;  // category ids in [-1, kRankHist) take the histogram path
@@ -214,12 +225,12 @@ template <bool ROT>
 __global__ void __launch_bounds__(kRankWarps * 32) nms_rank_kernel(const float* __restrict__ boxes,
                                                                    const float* __restrict__ scores,
                                                                    const int64_t* __restrict__ idxs, int M, int max_segment,
-                                                                   int use_range, NmsCtrl* __restrict__ ctrl,
+                                                                   int use_range, int one_segment, NmsCtrl* __restrict__ ctrl,
                                                                    int* __restrict__ grank_of_pos, int* __restrict__ orig_of_grank,
                                                                    int* __restrict__ seg_hi_of_pos, float* __restrict__ clsf_of_pos,
                                                                    float* __restrict__ sorted_boxes, int* __restrict__ seg_start,
                                                                    int* __restrict__ seg_end, unsigned char* __restrict__ keepflag) {
-  // tile of the streamed boxes: generic path {score, int64 category}; histogram path {64-bit order key, int32 category}
+  // tile of the streamed boxes: {64-bit order key, category} (int64 on the generic path, int32 on the histogram path)
   __shared__ unsigned long long s_key[kRankTile];
   __shared__ long long s_cls[kRankTile];
   __shared__ int s_hist[kRankHist + 2];  // [c + 1] = number of boxes of category c, then exclusive prefix = #{smaller category}
@@ -231,7 +242,12 @@ __global__ void __launch_bounds__(kRankWarps * 32) nms_rank_kernel(const float* 
   const int i0 = (blockIdx.x * kRankWarps + warp) * 2, i1 = i0 + 1;
   const bool ok0 = i0 < M, ok1 = i1 < M;
   const float sa = ok0 ? scores[i0] : 0.f, sb = ok1 ? scores[i1] : 0.f;
-  const long long ca = (ok0 && idxs) ? idxs[i0] : 0, cb = (ok1 && idxs) ? idxs[i1] : 0;
+  // category ids set the coordinate offsets; segment ids group the boxes for the mask and the scan.  They are the same
+  // unless one_segment puts every non-ignored box into segment 0.
+  auto seg = [one_segment](long long c) { return (one_segment && c >= 0) ? 0LL : c; };
+  const long long ida = (ok0 && idxs) ? idxs[i0] : 0, idb = (ok1 && idxs) ? idxs[i1] : 0;
+  const long long ca = seg(ida), cb = seg(idb);
+  const unsigned long long ka = score_key(sa, i0), kb = score_key(sb, i1);
   int ga = 0, gb = 0, sma = 0, smb = 0, bea = 0, beb = 0, na = 0, nb = 0;  // grank, smaller-class, before-in-class, class size
   // ---- category histogram (every CTA builds its own: M small loads from L2): when all ids fit, the O(M^2) loop below only
   //      has to count "before me in the score order" and "... and of my category" -- two compares per pair.
@@ -240,7 +256,7 @@ __global__ void __launch_bounds__(kRankWarps * 32) nms_rank_kernel(const float* 
   int small = 1;
   if (idxs) {
     for (int j = tid; j < M; j += kT) {
-      const long long c = idxs[j];
+      const long long c = seg(idxs[j]);
       if (c < -1 || c >= kRankHist) small = 0;
       else atomicAdd(&s_hist[(int)c + 1], 1);
     }
@@ -277,16 +293,14 @@ __global__ void __launch_bounds__(kRankWarps * 32) nms_rank_kernel(const float* 
         base += loc[e];
       }
     __syncthreads();
-    const unsigned long long ka = ((unsigned long long)(~enc_f(sa)) << 32) | (unsigned)i0;  // ascending key == score order
-    const unsigned long long kb = ((unsigned long long)(~enc_f(sb)) << 32) | (unsigned)i1;
     const int ca32 = (int)ca, cb32 = (int)cb;
     int* s_c32 = reinterpret_cast<int*>(s_cls);
     for (int t0 = 0; t0 < M; t0 += kRankTile) {
       const int tn = min(kRankTile, M - t0);
       __syncthreads();
       for (int j = tid; j < tn; j += kT) {
-        s_key[j] = ((unsigned long long)(~enc_f(scores[t0 + j])) << 32) | (unsigned)(t0 + j);
-        s_c32[j] = idxs ? (int)idxs[t0 + j] : 0;
+        s_key[j] = score_key(scores[t0 + j], t0 + j);
+        s_c32[j] = idxs ? (int)seg(idxs[t0 + j]) : 0;
       }
       __syncthreads();
       for (int jl = lane; jl < tn; jl += 32) {
@@ -300,20 +314,18 @@ __global__ void __launch_bounds__(kRankWarps * 32) nms_rank_kernel(const float* 
       }
     }
   } else {
-    float* s_score = reinterpret_cast<float*>(s_key);
     for (int t0 = 0; t0 < M; t0 += kRankTile) {
       const int tn = min(kRankTile, M - t0);
       __syncthreads();
       for (int j = tid; j < tn; j += kT) {
-        s_score[j] = scores[t0 + j];
-        s_cls[j] = idxs ? idxs[t0 + j] : 0;
+        s_key[j] = score_key(scores[t0 + j], t0 + j);
+        s_cls[j] = idxs ? seg(idxs[t0 + j]) : 0;
       }
       __syncthreads();
       for (int jl = lane; jl < tn; jl += 32) {
-        const float s = s_score[jl];
+        const unsigned long long kj = s_key[jl];
         const long long c = s_cls[jl];
-        const int j = t0 + jl;
-        const bool fa = s > sa || (s == sa && j < i0), fb = s > sb || (s == sb && j < i1);
+        const bool fa = kj < ka, fb = kj < kb;
         ga += fa;
         gb += fb;
         sma += c < ca;
@@ -352,20 +364,20 @@ __global__ void __launch_bounds__(kRankWarps * 32) nms_rank_kernel(const float* 
 #pragma unroll
     for (int q = 0; q < D; ++q) b[q] = boxes[(size_t)i * D + q];
     const bool ignored = c < 0;  // negative category: the box takes part in nothing and is never kept
-    if (!ignored) {
+    if (!ignored) {  // NaN-propagating like the reference's torch reductions: one NaN coordinate makes every offset NaN
       if (ROT) {  // detectron2/layers/nms.py:137-143
-        const float half = fmaxf(b[2], b[3]) / 2;
-        mx = fmaxf(mx, fmaxf(b[0], b[1]) + half);
-        mn = fminf(mn, fminf(b[0], b[1]) - half);
+        const float half = max_nan(b[2], b[3]) / 2;
+        mx = max_nan(mx, max_nan(b[0], b[1]) + half);
+        mn = min_nan(mn, min_nan(b[0], b[1]) - half);
       } else {  // torchvision _batched_nms_coordinate_trick: boxes.max()
-        mx = fmaxf(mx, fmaxf(fmaxf(b[0], b[1]), fmaxf(b[2], b[3])));
+        mx = max_nan(mx, max_nan(max_nan(b[0], b[1]), max_nan(b[2], b[3])));
       }
     }
     if (lane == 0) {
       grank_of_pos[pos] = g;
       orig_of_grank[g] = i;
       seg_hi_of_pos[pos] = (ignored || n == 1) ? pos : sm + n;  // empty column range: the mask kernel skips the row
-      clsf_of_pos[pos] = (float)c;
+      clsf_of_pos[pos] = (float)(e ? idb : ida);
 #pragma unroll
       for (int q = 0; q < D; ++q) sorted_boxes[(size_t)pos * D + q] = b[q];
       if (ignored) {
@@ -387,11 +399,12 @@ __global__ void __launch_bounds__(kRankWarps * 32) nms_rank_kernel(const float* 
     __syncthreads();
     if (tid == 0) {
       for (int q = 1; q < kRankWarps; ++q) {
-        mx = fmaxf(mx, s_mx[q]);
-        mn = fminf(mn, s_mn[q]);
+        mx = max_nan(mx, s_mx[q]);
+        mn = min_nan(mn, s_mn[q]);
       }
-      if (mx > -INFINITY) atomicMax(&ctrl->mx, enc_f(mx));
-      if (ROT && mn < INFINITY) atomicMax(&ctrl->mn_neg, enc_f(-mn));
+      // the canonical NaN encodes above +inf, so a NaN wins the atomicMax and decodes back to NaN
+      if (mx != -INFINITY) atomicMax(&ctrl->mx, enc_f(canon_f(mx)));
+      if (ROT && mn != INFINITY) atomicMax(&ctrl->mn_neg, enc_f(canon_f(-mn)));
     }
   }
 }
@@ -526,7 +539,9 @@ __global__ void __launch_bounds__(kScanThreads, 1) nms_scan_kernel(const unsigne
   for (int seg = blockIdx.x; seg < nseg; seg += gridDim.x) {
     const int p0 = seg_start[seg], p1 = seg_end[seg];
     const int b0 = p0 >> 6, nb = ((p1 - 1) >> 6) + 1;  // blocks [b0, nb) of the global tiling touch this segment
-    if (nb - b0 > wcap + 1) continue;                    // larger than the caller's bound (error already flagged): skipped
+    // n <= ms boxes from row (p0 & 63) <= 63 span nb - b0 <= (63 + ms + 63) / 64 = wcap blocks; word planes w - b and
+    // removed[] slots then stay below wcap.  A longer span is a segment over the caller's bound (error already flagged).
+    if (nb - b0 > wcap) continue;
     __syncthreads();                                     // previous segment done with removed[] / s_diag
     for (int i = b0 + tid; i < nb; i += kScanThreads) removed[i - b0] = 0ull;
 
@@ -715,19 +730,23 @@ D2B_API int d2b_nms(const float* boxes, const float* scores, const int64_t* idxs
   NmsWorkspace w = carve(workspace, M, rotated, max_segment);
   if (workspace_bytes < w.total) return D2B_EWORKSPACE;
   const int m = (int)M, nb = (m + 63) / 64;
-  const size_t smem = (size_t)(w.wcap + 1) * sizeof(unsigned long long);
+  const size_t smem = (size_t)w.wcap * sizeof(unsigned long long);  // removed[]: one word per block of a segment
   if (smem > 200 * 1024 || w.wcap > 65535) return D2B_EUNSUPPORTED;
   D2B_CUDA(cudaMemsetAsync(w.ctrl, 0, w.zero_bytes, stream));
   const int apply_offsets = (idxs && !no_offset) ? 1 : 0;
+  // The reference runs ONE nms over the offset boxes, so two boxes of different categories meet with IoU 0 (or NaN when an
+  // offset is NaN).  A threshold that IoU 0 passes (rotated iou >= thr, axis-aligned iou > thr) therefore suppresses
+  // across categories: all non-ignored boxes then form one segment, still with their categories' offsets.
+  const int one_segment = (apply_offsets && (rotated ? iou_threshold <= 0.0 : iou_threshold < 0.0)) ? 1 : 0;
   // 1. positions in the score order and in the category-major order, segments, coordinate range
   const int rank_grid = d2b_cdiv(m, 2 * kRankWarps);
   if (rotated)
-    nms_rank_kernel<true><<<rank_grid, kRankWarps * 32, 0, stream>>>(boxes, scores, idxs, m, (int)max_segment, apply_offsets, w.ctrl,
-                                                                     w.grank_of_pos, w.orig_of_grank, w.seg_hi_of_pos,
+    nms_rank_kernel<true><<<rank_grid, kRankWarps * 32, 0, stream>>>(boxes, scores, idxs, m, (int)max_segment, apply_offsets,
+                                                                     one_segment, w.ctrl, w.grank_of_pos, w.orig_of_grank, w.seg_hi_of_pos,
                                                                      w.clsf_of_pos, w.sorted_boxes, w.seg_start, w.seg_end, w.keepflag);
   else
-    nms_rank_kernel<false><<<rank_grid, kRankWarps * 32, 0, stream>>>(boxes, scores, idxs, m, (int)max_segment, apply_offsets, w.ctrl,
-                                                                      w.grank_of_pos, w.orig_of_grank, w.seg_hi_of_pos,
+    nms_rank_kernel<false><<<rank_grid, kRankWarps * 32, 0, stream>>>(boxes, scores, idxs, m, (int)max_segment, apply_offsets,
+                                                                      one_segment, w.ctrl, w.grank_of_pos, w.orig_of_grank, w.seg_hi_of_pos,
                                                                       w.clsf_of_pos, w.sorted_boxes, w.seg_start, w.seg_end, w.keepflag);
   D2B_CHECK_LAUNCH();
   // 2. IoU bitmask inside the categories (coordinate offsets of the reference's batched-NMS trick applied in fp32)

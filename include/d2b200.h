@@ -164,12 +164,20 @@ int d2b_roi_pooler_rotated_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C,
 /* ---- NMS --------------------------------------------------------------------------------
  * Replaces torchvision::nms reached from detectron2/layers/nms.py:5-22 (nms, batched_nms) and
  * torch.ops.detectron2.nms_rotated (csrc/vision.cpp:116, csrc/nms_rotated/nms_rotated.h:22-37).
- * Greedy NMS in stable descending-score order (equal scores: lower index first).
+ * Greedy NMS in stable descending-score order (equal scores: lower index first), the order of
+ * torch.sort(scores, descending=True, stable=True): a NaN score of either sign ranks above +inf, NaNs among
+ * themselves by index; -0.0 and +0.0 are equal scores.
  *   boxes  [M,4] xyxy fp32 (rotated: [M,5] cx,cy,w,h,angle_deg), scores [M] fp32
  *   idxs   [M] int64 category ids or NULL (plain nms).  When non-NULL the reference's coordinate
  *          trick is applied on the fly:  axis-aligned  box + idx*(max_coord+1)   (torchvision
  *          ops/boxes.py _batched_nms_coordinate_trick);  rotated  centre + idx*(max-min+1)
- *          (detectron2/layers/nms.py:137-146), all in fp32 like the reference.
+ *          (detectron2/layers/nms.py:137-146), all in fp32 like the reference.  The range propagates
+ *          NaN like torch's max / min: a NaN coordinate makes every offset box NaN, so nothing is suppressed.
+ *          Boxes of different categories meet in the reference's single NMS with IoU 0, so a threshold that 0 passes
+ *          (rotated thr <= 0, axis-aligned thr < 0) suppresses across categories too; that case runs as one segment
+ *          of all non-ignored boxes (max_segment must then bound their number).
+ *          The range covers the non-ignored boxes only (see below); torchvision has no ignored ids and
+ *          treats a negative id as an ordinary category, so public batched_nms callers pass ids >= 0.
  *   keep   [M] int64 out: kept ORIGINAL indices, score-descending; num_keep [1] int64 out (device).
  * Suppression rule: axis-aligned  iou >  thr (torchvision);  rotated  iou >= thr (nms_rotated_cpu.cpp:54).
  * flags: D2B_NMS_ROTATED selects the rotated variant; D2B_NMS_NO_OFFSET makes `idxs` pure segment ids -- the

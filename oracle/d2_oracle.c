@@ -200,10 +200,16 @@ ORC_API void orc_roi_align_rotated_backward(const float* gout, const float* rois
  * suppress iff inter/(a_i+a_j-inter) > thr (strict; float ovr vs double thr).
  * ---------------------------------------------------------------------------------------- */
 typedef struct { float s; int64_t i; } orc_si;
+/* torch.sort(descending=True, stable=True): NaN (either sign) above every number, -0 == +0, then lower index first.
+ * A total order for any input, as qsort requires. */
 static int orc_cmp_desc(const void* a, const void* b) {
   const orc_si *x = (const orc_si*)a, *y = (const orc_si*)b;
-  if (x->s > y->s) return -1;
-  if (x->s < y->s) return 1;
+  const int xn = isnan(x->s), yn = isnan(y->s);
+  if (xn != yn) return xn ? -1 : 1;
+  if (!xn) {
+    if (x->s > y->s) return -1;
+    if (x->s < y->s) return 1;
+  }
   return (x->i > y->i) - (x->i < y->i); /* stable: lower index first on ties */
 }
 static int64_t* orc_order_desc(const float* scores, int64_t M) {

@@ -318,3 +318,78 @@ def test_sweep_roi_align_rotated_vs_compiled_reference(seed, golden):
     ph, pw, sr = [(7, 7, 0), (3, 5, 2), (2, 2, 3)][seed]
     assert torch.allclose(orc.roi_align_rotated_forward(x, rois, 0.25, ph, pw, sr), ref, rtol=1e-4, atol=1e-5)
     assert torch.allclose(orc.roi_align_rotated_backward(go, rois, 0.25, ph, pw, n, c, h, w, sr), gref, rtol=1e-4, atol=1e-4)
+
+
+# ---------------------------------------------------------------- 5. NMS score order (NaN, signed zeros, infinities, ties)
+def edge_scores():
+    """Scores every NMS path must order like torch.sort(descending=True, stable=True): NaNs of both signs and with a
+    payload (all above +inf, by index), -0.0 / +0.0 (equal, by index), +-inf and exact ties."""
+    bits = [0x3F800000, 0xFFC00000, 0x40000000, 0x00000000, 0x80000000, 0x7F800000, 0x00000000, 0x7FC00000,
+            0xFF800000, 0x40000000, 0x80000000, 0x3F800000, 0xFF800000, 0xFF800123, 0x3F000000, 0xBF800000]
+    return torch.from_numpy(np.array(bits, dtype=np.uint32).view(np.float32).copy())
+
+
+def score_order(scores):
+    return torch.sort(scores, descending=True, stable=True).indices
+
+
+def test_torch_score_order_of_the_edge_scores():
+    # the contract itself: every NaN first (by index), then +inf, ..., -0.0 and +0.0 as equals, ..., -inf
+    assert score_order(edge_scores()).tolist() == [1, 7, 13, 5, 2, 9, 0, 11, 14, 3, 4, 6, 10, 15, 8, 12]
+
+
+def disjoint_boxes(m, rotated=False):
+    x = torch.arange(m, dtype=torch.float32) * 10
+    if rotated:
+        return torch.stack([x + 2.5, torch.full_like(x, 2.5), torch.full_like(x, 5.0), torch.full_like(x, 5.0),
+                            torch.zeros_like(x)], 1)
+    return torch.stack([x, torch.zeros_like(x), x + 5, torch.full_like(x, 5.0)], 1)
+
+
+def test_oracle_score_order_pin():
+    s = edge_scores()
+    m = s.numel()
+    order = score_order(s)
+    zeros = torch.zeros(m, dtype=torch.int64)
+    assert torch.equal(orc.nms(disjoint_boxes(m), s, 0.5), order)
+    assert torch.equal(orc.nms_rotated(disjoint_boxes(m, True), s, 0.5), order)
+    assert torch.equal(orc.batched_nms(disjoint_boxes(m), s, zeros, 0.5), order)
+    assert torch.equal(orc.batched_nms_rotated(disjoint_boxes(m, True), s, zeros, 0.5), order)
+
+
+def _greedy(order, iou, thr, strict):
+    keep, dead = [], set()
+    for i in order:
+        if i in dead:
+            continue
+        keep.append(i)
+        dead.update(j for j in order if j not in dead and j != i and (iou[i][j] > thr if strict else iou[i][j] >= thr))
+    return keep
+
+
+def _iou_xyxy(a, b):  # torchvision's CPU expression, fp32 step by step
+    f = np.float32
+    xx1, yy1, xx2, yy2 = max(a[0], b[0]), max(a[1], b[1]), min(a[2], b[2]), min(a[3], b[3])
+    w, h = max(f(0), f(xx2 - xx1)), max(f(0), f(yy2 - yy1))
+    inter = f(w * h)
+    area_a, area_b = f(f(a[2] - a[0]) * f(a[3] - a[1])), f(f(b[2] - b[0]) * f(b[3] - b[1]))
+    return float(f(inter / f(f(area_a + area_b) - inter)))
+
+
+def test_oracle_score_order_overlapping_boxes():
+    """Overlapping boxes with the edge scores: the oracle is the greedy rule applied in the torch.sort order."""
+    s = torch.cat([edge_scores()] * 3)
+    m = s.numel()
+    g = torch.Generator().manual_seed(4)
+    xy = (torch.rand(m, 2, generator=g) * 40).round()
+    boxes = torch.cat([xy, xy + 8 + (torch.rand(m, 2, generator=g) * 16).round()], 1)
+    order = score_order(s).tolist()
+    bn = boxes.numpy()
+    iou = [[_iou_xyxy(bn[i], bn[j]) for j in range(m)] for i in range(m)]
+    for thr in (0.0, 0.3, 0.6):
+        assert orc.nms(boxes, s, thr).tolist() == _greedy(order, iou, thr, True), thr
+    rot = torch.cat([(boxes[:, :2] + boxes[:, 2:]) / 2, boxes[:, 2:] - boxes[:, :2],
+                     (torch.rand(m, 1, generator=g) * 180 - 90).round()], 1)
+    riou = orc.box_iou_rotated(rot, rot).tolist()
+    for thr in (0.3, 0.6):
+        assert orc.nms_rotated(rot, s, thr).tolist() == _greedy(order, riou, thr, False), thr
