@@ -84,6 +84,10 @@ def _declare(lib):
                                   i64p, i64p, vp]),
         "d2b_dense_prepare": (i, [C.POINTER(DenseLevels), i, i, C.POINTER(C.c_float), f, f32p, f32p, f32p, f32p, i64p, i64p,
                                   vp]),
+        "d2b_rrpn_prepare": (i, [C.POINTER(RpnLevels), i, f32p, f, i, f32p, f32p, f32p, f32p, i64p, vp, vp]),
+        "d2b_frcnn_rotated_prepare": (i, [f32p, f32p, C.POINTER(C.c_int), i, i, i, f32p, f, i, i, f32p, f32p, f32p, f32p, i64p,
+                                          i64p, i64p, i64p, vp]),
+        "d2b_rpn_select_rotated": (i, [i64p, i64p, i, i, i, f32p, f32p, i64p, f32p, f32p, i64p, i64p, vp]),
         "d2b_mask_loss_forward": (i, [f32p, i, i, i, u8p, i, i, i, f32p, i64p, i64p, f32p, u8p, vp]),
         "d2b_mask_loss_backward": (i, [f32p, i, i, i, u8p, i64p, f32p, f32p, vp]),
         "d2b_box_iou_rotated": (i, [f32p, i64, f32p, i64, f32p, vp]),

@@ -11,6 +11,13 @@
 // Together with d2b_nms (category = image * L + level, per-category bound = pre_nms_topk) the whole selection is a
 // sync-free launch sequence with static shapes: capturable in a CUDA graph; the reference loops over images in Python
 // with boolean indexing and one `.item()` per image.  Compiled with -fmad=false like nms.cu (bit-exact clip / offsets).
+//
+// The rotated pipeline has the same shape (rrpn.py:20-127, rotated_fast_rcnn.py:46-132): d2b_rrpn_prepare /
+// d2b_frcnn_rotated_prepare -> d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET) -> d2b_rpn_select_rotated.  The box type is a
+// template policy (XyxyBox / RotBox below) of the shared candidate and selection kernels.
+#include <climits>
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace {
@@ -26,6 +33,94 @@ struct RpnLevels {
 };
 
 __device__ __forceinline__ bool finitef(float v) { return fabsf(v) <= 3.402823466e38f; }  // false for inf and NaN
+
+// Box policies of the candidate kernels: layout, the reference's clip, and the batched-NMS coordinate offsets, per box type.
+//   XyxyBox  Boxes (x1, y1, x2, y2): clip = clamp to the image; torchvision's offsets idx * (max coordinate + 1) on all four.
+//   RotBox   RotatedBoxes (cx, cy, w, h, angle_deg): RotatedBoxes.clip (structures/rotated_boxes.py:248-303); the offsets of
+//            batched_nms_rotated (layers/nms.py:137-146), idx * (max - min + 1), on the centre only.
+struct XyxyBox {
+  static constexpr int D = 4;
+  static constexpr bool kRotated = false;
+  float v[4];
+  __device__ __forceinline__ void clip(float ih, float iw) {  // clamp(min=0, max=w / h)
+    v[0] = fminf(fmaxf(v[0], 0.f), iw);
+    v[1] = fminf(fmaxf(v[1], 0.f), ih);
+    v[2] = fminf(fmaxf(v[2], 0.f), iw);
+    v[3] = fminf(fmaxf(v[3], 0.f), ih);
+  }
+  __device__ __forceinline__ float hi() const { return fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])); }  // boxes.max()
+  __device__ __forceinline__ float lo() const { return 0.f; }                                          // not part of the range
+  static __device__ __forceinline__ float scale(bool any, float mx, float) { return (any ? mx : 0.f) + 1.0f; }
+  __device__ __forceinline__ void shift(float off) {
+    v[0] += off;
+    v[1] += off;
+    v[2] += off;
+    v[3] += off;
+  }
+};
+
+struct RotBox {
+  static constexpr int D = 5;
+  static constexpr bool kRotated = true;
+  float v[5];
+  __device__ __forceinline__ void clip(float ih, float iw) {
+    // normalize_angles: (a + 180) % 360 - 180 with torch's float remainder (the result takes the divisor's sign)
+    float m = fmodf(v[4] + 180.f, 360.f);
+    if (m < 0.f) m += 360.f;
+    v[4] = m - 180.f;
+    if (fabsf(v[4]) <= 1.0f) {  // clip_angle_threshold: only near-horizontal boxes are clipped, as xyxy boxes
+      const float x1 = fminf(fmaxf(v[0] - v[2] / 2.f, 0.f), iw), y1 = fminf(fmaxf(v[1] - v[3] / 2.f, 0.f), ih);
+      const float x2 = fminf(fmaxf(v[0] + v[2] / 2.f, 0.f), iw), y2 = fminf(fmaxf(v[1] + v[3] / 2.f, 0.f), ih);
+      v[0] = (x1 + x2) / 2.f;
+      v[1] = (y1 + y2) / 2.f;
+      v[2] = fminf(v[2], x2 - x1);  // widths and heights never grow through rounding
+      v[3] = fminf(v[3], y2 - y1);
+    }
+  }
+  __device__ __forceinline__ float hi() const { return fmaxf(v[0], v[1]) + fmaxf(v[2], v[3]) / 2; }
+  __device__ __forceinline__ float lo() const { return fminf(v[0], v[1]) - fmaxf(v[2], v[3]) / 2; }
+  static __device__ __forceinline__ float scale(bool any, float mx, float mn) { return (any ? mx - mn : 0.f) + 1.0f; }
+  __device__ __forceinline__ void shift(float off) {
+    v[0] += off;
+    v[1] += off;
+  }
+};
+
+template <class Box>
+__device__ __forceinline__ Box load_box(const float* __restrict__ p) {  // scalar loads: rows of the inputs need no alignment
+  Box b;
+#pragma unroll
+  for (int q = 0; q < Box::D; ++q) b.v[q] = p[q];
+  return b;
+}
+
+template <class Box>
+__device__ __forceinline__ Box load_box_aligned(const float* __restrict__ p) {  // xyxy buffers are 16-byte aligned
+  if constexpr (Box::D == 4) {
+    const float4 q = *reinterpret_cast<const float4*>(p);
+    return Box{{q.x, q.y, q.z, q.w}};
+  } else {
+    return load_box<Box>(p);
+  }
+}
+
+template <class Box>
+__device__ __forceinline__ void store_box(float* __restrict__ p, const Box& b) {  // xyxy buffers are 16-byte aligned
+  if constexpr (Box::D == 4) {
+    *reinterpret_cast<float4*>(p) = make_float4(b.v[0], b.v[1], b.v[2], b.v[3]);
+  } else {
+#pragma unroll
+    for (int q = 0; q < Box::D; ++q) p[q] = b.v[q];
+  }
+}
+
+template <class Box>
+__device__ __forceinline__ Box zero_box() {
+  Box b;
+#pragma unroll
+  for (int q = 0; q < Box::D; ++q) b.v[q] = 0.f;
+  return b;
+}
 
 __global__ void __launch_bounds__(kThreads) rpn_prepare_kernel(const RpnLevels P, int T, const float* __restrict__ image_hw,
                                                                float min_box_size, int use_offsets,
@@ -109,6 +204,8 @@ __device__ __forceinline__ int block_scan(int v, int* __restrict__ warp_tot, int
   return wbase + inc - v;
 }
 
+// D = 4: xyxy boxes (d2b_rpn_select), D = 5: rotated boxes (d2b_rpn_select_rotated).
+template <int D>
 __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* __restrict__ keep,
                                                               const long long* __restrict__ num_keep, int T, int post_topk,
                                                               const float* __restrict__ flat_boxes,
@@ -116,6 +213,7 @@ __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* _
                                                               const long long* __restrict__ cat_ids,
                                                               float* __restrict__ out_boxes, float* __restrict__ out_scores,
                                                               long long* __restrict__ out_index, long long* __restrict__ counts) {
+  using Box = std::conditional_t<D == 4, XyxyBox, RotBox>;
   __shared__ int warp_tot[32];
   const int n = blockIdx.x, tid = threadIdx.x;
   const long long nk = max(0LL, *num_keep);
@@ -132,7 +230,7 @@ __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* _
     const int rank = have + block_scan(mine, warp_tot, total);
     if (mine && rank < post_topk) {
       const size_t o = (size_t)n * post_topk + rank;
-      *reinterpret_cast<float4*>(out_boxes + o * 4) = *reinterpret_cast<const float4*>(flat_boxes + (size_t)kidx * 4);
+      store_box(out_boxes + o * D, load_box_aligned<Box>(flat_boxes + (size_t)kidx * D));
       out_scores[o] = raw_scores[kidx];
       out_index[o] = kidx;
     }
@@ -141,7 +239,7 @@ __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* _
   const int cnt = min(have, post_topk);
   for (int r = cnt + tid; r < post_topk; r += kThreads) {  // deterministic padding
     const size_t o = (size_t)n * post_topk + r;
-    *reinterpret_cast<float4*>(out_boxes + o * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+    store_box(out_boxes + o * D, zero_box<Box>());
     out_scores[o] = 0.f;
     out_index[o] = 0;
   }
@@ -181,9 +279,12 @@ D2B_API int d2b_rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_
   return D2B_OK;
 }
 
-D2B_API int d2b_rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
-                           const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
-                           float* out_scores, int64_t* out_index, int64_t* counts, void* stream) {
+namespace {
+
+template <int D>
+int rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk, const float* flat_boxes,
+               const float* raw_scores, const int64_t* cat_ids, float* out_boxes, float* out_scores, int64_t* out_index,
+               int64_t* counts, void* stream) {
   if (N < 0 || T < 0 || post_nms_topk < 0) return D2B_EINVAL;
   if (N == 0) return D2B_OK;
   if (!counts) return D2B_EINVAL;
@@ -192,11 +293,28 @@ D2B_API int d2b_rpn_select(const int64_t* keep, const int64_t* num_keep, int N, 
     return D2B_OK;
   }
   if (!keep || !num_keep || !flat_boxes || !raw_scores || !cat_ids || !out_boxes || !out_scores || !out_index) return D2B_EINVAL;
-  rpn_select_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>((const long long*)keep, (const long long*)num_keep, T, post_nms_topk,
-                                                              flat_boxes, raw_scores, (const long long*)cat_ids, out_boxes,
-                                                              out_scores, (long long*)out_index, (long long*)counts);
+  rpn_select_kernel<D><<<N, kThreads, 0, (cudaStream_t)stream>>>((const long long*)keep, (const long long*)num_keep, T,
+                                                                 post_nms_topk, flat_boxes, raw_scores,
+                                                                 (const long long*)cat_ids, out_boxes, out_scores,
+                                                                 (long long*)out_index, (long long*)counts);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
+}
+
+}  // namespace
+
+D2B_API int d2b_rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
+                           const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
+                           float* out_scores, int64_t* out_index, int64_t* counts, void* stream) {
+  return rpn_select<4>(keep, num_keep, N, T, post_nms_topk, flat_boxes, raw_scores, cat_ids, out_boxes, out_scores, out_index,
+                       counts, stream);
+}
+
+D2B_API int d2b_rpn_select_rotated(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
+                                   const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
+                                   float* out_scores, int64_t* out_index, int64_t* counts, void* stream) {
+  return rpn_select<5>(keep, num_keep, N, T, post_nms_topk, flat_boxes, raw_scores, cat_ids, out_boxes, out_scores, out_index,
+                       counts, stream);
 }
 
 // ================================================================================================ Fast R-CNN / dense-head candidates
@@ -233,31 +351,36 @@ __device__ __forceinline__ float block_max(float v, float* s_red, float* s_out) 
   return *s_out;
 }
 
+// Box = XyxyBox: d2b_frcnn_prepare; RotBox: d2b_frcnn_rotated_prepare (rotated_fast_rcnn.py:84-122, the same steps on
+// RotatedBoxes, with `seg_per_image` for thresholds that IoU 0 passes: every candidate of the image in one NMS segment).
+template <class Box>
 __global__ void __launch_bounds__(kThreads) frcnn_prepare_kernel(const FrcnnImages I, const float* __restrict__ boxes,
                                                                  const float* __restrict__ scores, int K, int kreg,
                                                                  const float* __restrict__ image_hw, float score_thresh, int cap,
-                                                                 float* __restrict__ cand_boxes, float* __restrict__ nms_boxes,
-                                                                 float* __restrict__ nms_scores, float* __restrict__ raw_scores,
-                                                                 long long* __restrict__ cand_flat, long long* __restrict__ cat_ids,
-                                                                 long long* __restrict__ n_cand, long long* __restrict__ row_map) {
+                                                                 int seg_per_image, float* __restrict__ cand_boxes,
+                                                                 float* __restrict__ nms_boxes, float* __restrict__ nms_scores,
+                                                                 float* __restrict__ raw_scores, long long* __restrict__ cand_flat,
+                                                                 long long* __restrict__ cat_ids, long long* __restrict__ n_cand,
+                                                                 long long* __restrict__ row_map) {
+  constexpr int D = Box::D;
   __shared__ int warp_tot[32];
   __shared__ float s_red[32];
-  __shared__ float s_max;
+  __shared__ float s_max, s_min;
   const int n = blockIdx.x, tid = threadIdx.x;
   const int rs = I.row_start[n], R = I.row_start[n + 1] - rs;
   const float ih = image_hw[2 * n], iw = image_hw[2 * n + 1];
   const size_t obase = (size_t)n * cap;
   int have = 0, have_rows = 0;
-  float mx = -INFINITY;
+  float mx = -INFINITY, mn = INFINITY;
   for (int r0 = 0; r0 < R; r0 += kThreads) {
     const int r = r0 + tid;
     int cnt = 0, valid = 0;
     const float* __restrict__ srow = scores + (size_t)(rs + (r < R ? r : 0)) * (K + 1);
-    const float* __restrict__ brow = boxes + (size_t)(rs + (r < R ? r : 0)) * kreg * 4;
+    const float* __restrict__ brow = boxes + (size_t)(rs + (r < R ? r : 0)) * kreg * D;
     if (r < R) {
       valid = 1;
       for (int c = 0; c <= K; ++c) valid &= finitef(srow[c]) ? 1 : 0;
-      for (int c = 0; c < kreg * 4; ++c) valid &= finitef(brow[c]) ? 1 : 0;
+      for (int c = 0; c < kreg * D; ++c) valid &= finitef(brow[c]) ? 1 : 0;
       if (valid)
         for (int c = 0; c < K; ++c) cnt += srow[c] > score_thresh ? 1 : 0;
     }
@@ -270,16 +393,15 @@ __global__ void __launch_bounds__(kThreads) frcnn_prepare_kernel(const FrcnnImag
       for (int c = 0; c < K && pos < cap; ++c) {
         const float sc = srow[c];
         if (!(sc > score_thresh)) continue;
-        const float* __restrict__ b = brow + (kreg == 1 ? 0 : c * 4);
-        // Boxes.clip: clamp(min=0, max=w / h)
-        const float x1 = fminf(fmaxf(b[0], 0.f), iw), y1 = fminf(fmaxf(b[1], 0.f), ih);
-        const float x2 = fminf(fmaxf(b[2], 0.f), iw), y2 = fminf(fmaxf(b[3], 0.f), ih);
-        *reinterpret_cast<float4*>(cand_boxes + (obase + pos) * 4) = make_float4(x1, y1, x2, y2);
+        Box b = load_box<Box>(brow + (kreg == 1 ? 0 : c * D));
+        b.clip(ih, iw);
+        store_box(cand_boxes + (obase + pos) * D, b);
         raw_scores[obase + pos] = sc;
         nms_scores[obase + pos] = sc;
         cand_flat[obase + pos] = (long long)r * K + c;
         cat_ids[obase + pos] = (long long)n * (K + 1) + c;
-        mx = fmaxf(mx, fmaxf(fmaxf(x1, y1), fmaxf(x2, y2)));
+        mx = fmaxf(mx, b.hi());
+        if constexpr (Box::kRotated) mn = fminf(mn, b.lo());
         ++pos;
       }
     }
@@ -289,26 +411,81 @@ __global__ void __launch_bounds__(kThreads) frcnn_prepare_kernel(const FrcnnImag
   if (tid == 0) n_cand[n] = have;  // > cap: the list was truncated, the caller redoes the image
   const int live = min(have, cap);
   mx = block_max(mx, s_red, &s_max);
-  const float scale = (live > 0 ? mx : 0.f) + 1.0f;  // torchvision _batched_nms_coordinate_trick: idxs * (boxes.max() + 1)
+  if constexpr (Box::kRotated) mn = -block_max(-mn, s_red, &s_min);
+  const float scale = Box::scale(live > 0, mx, mn);  // idxs * (max + 1) (torchvision) or idxs * (max - min + 1) (rotated)
   __threadfence_block();
   for (int t = tid; t < cap; t += kThreads) {
     const size_t o = obase + t;
     if (t < live) {
-      float4 b = *reinterpret_cast<const float4*>(cand_boxes + o * 4);
-      const float offv = (float)(cat_ids[o] - (long long)n * (K + 1)) * scale;
-      b.x += offv;
-      b.y += offv;
-      b.z += offv;
-      b.w += offv;
-      *reinterpret_cast<float4*>(nms_boxes + o * 4) = b;
+      Box b = load_box_aligned<Box>(cand_boxes + o * D);
+      b.shift((float)(cat_ids[o] - (long long)n * (K + 1)) * scale);
+      store_box(nms_boxes + o * D, b);
+      if constexpr (Box::kRotated)
+        if (seg_per_image) cat_ids[o] = n;
     } else {  // dead slot: ignored by the NMS kernels
-      *reinterpret_cast<float4*>(cand_boxes + o * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-      *reinterpret_cast<float4*>(nms_boxes + o * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      store_box(cand_boxes + o * D, zero_box<Box>());
+      store_box(nms_boxes + o * D, zero_box<Box>());
       raw_scores[o] = 0.f;
       nms_scores[o] = -INFINITY;
       cand_flat[o] = 0;
       cat_ids[o] = -1;
     }
+  }
+}
+
+// find_top_rrpn_proposals (detectron2/modeling/proposal_generator/rrpn.py:59-113) up to the NMS, one CTA per image: the
+// per-level top-k gather, the finiteness check (:97-105), RotatedBoxes.clip (:106), nonempty (:109) and the per-image
+// offsets of batched_nms_rotated (layers/nms.py:137-146) over the surviving boxes.  Removed boxes get category -1.
+__global__ void __launch_bounds__(kThreads) rrpn_prepare_kernel(const RpnLevels P, int T, const float* __restrict__ image_hw,
+                                                                float min_box_size, int seg_per_image,
+                                                                float* __restrict__ flat_boxes, float* __restrict__ nms_boxes,
+                                                                float* __restrict__ nms_scores, float* __restrict__ raw_scores,
+                                                                long long* __restrict__ cat_ids, int* __restrict__ nonfinite) {
+  __shared__ float s_red[32];
+  __shared__ float s_max, s_min;
+  const int n = blockIdx.x, tid = threadIdx.x;
+  const float ih = image_hw[2 * n], iw = image_hw[2 * n + 1];
+  float mx = -INFINITY, mn = INFINITY;
+  int bad = 0, any = 0;
+  for (int t = tid; t < T; t += kThreads) {
+    int l = 0;
+    while (l + 1 < P.L && t >= P.t0[l + 1]) ++l;
+    const int j = t - P.t0[l];
+    const long long a = P.topk_idx[l][(size_t)n * P.k[l] + j];
+    const float s = P.topk_scores[l][(size_t)n * P.k[l] + j];
+    RotBox b = load_box<RotBox>(P.proposals[l] + ((size_t)n * P.A[l] + a) * 5);
+    bool fin = finitef(s);
+#pragma unroll
+    for (int q = 0; q < 5; ++q) fin = fin && finitef(b.v[q]);
+    b.clip(ih, iw);
+    const bool valid = fin && b.v[2] > min_box_size && b.v[3] > min_box_size;
+    const size_t o = (size_t)n * T + t;
+    store_box(flat_boxes + o * 5, valid ? b : zero_box<RotBox>());
+    raw_scores[o] = s;
+    nms_scores[o] = valid ? s : -INFINITY;
+    cat_ids[o] = valid ? (long long)n * P.L + l : -1LL;
+    if (valid) {
+      mx = fmaxf(mx, b.hi());
+      mn = fminf(mn, b.lo());
+      any = 1;
+    }
+    bad |= fin ? 0 : 1;
+  }
+  if (bad) atomicOr(nonfinite, 1);
+  any = __syncthreads_or(any);
+  mx = block_max(mx, s_red, &s_max);
+  mn = -block_max(-mn, s_red, &s_min);
+  const float scale = RotBox::scale(any != 0, mx, mn);
+  for (int t = tid; t < T; t += kThreads) {
+    int l = 0;
+    while (l + 1 < P.L && t >= P.t0[l + 1]) ++l;
+    const size_t o = (size_t)n * T + t;
+    RotBox b = load_box<RotBox>(flat_boxes + o * 5);
+    if (cat_ids[o] >= 0) {
+      b.shift((float)l * scale);
+      if (seg_per_image) cat_ids[o] = n;
+    }
+    store_box(nms_boxes + o * 5, b);
   }
 }
 
@@ -396,10 +573,13 @@ __global__ void __launch_bounds__(kThreads) dense_prepare_kernel(const DenseLeve
 
 }  // namespace
 
-D2B_API int d2b_frcnn_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes, int kreg,
-                              const float* image_hw, float score_thresh, int cap, float* cand_boxes, float* nms_boxes,
-                              float* nms_scores, float* raw_scores, int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand,
-                              int64_t* row_map, void* stream) {
+namespace {
+
+template <class Box>
+int frcnn_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes, int kreg,
+                  const float* image_hw, float score_thresh, int cap, int seg_per_image, float* cand_boxes, float* nms_boxes,
+                  float* nms_scores, float* raw_scores, int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand, int64_t* row_map,
+                  void* stream) {
   if (N < 0 || N > D2B_MAX_IMAGES || num_classes <= 0 || (kreg != 1 && kreg != num_classes) || cap < 0 || !row_start)
     return D2B_EINVAL;
   if (N == 0) return D2B_OK;
@@ -412,11 +592,61 @@ D2B_API int d2b_frcnn_prepare(const float* boxes, const float* scores, const int
   if (!image_hw || !n_cand) return D2B_EINVAL;
   if (row_start[N] > row_start[0] && (!boxes || !scores || !row_map)) return D2B_EINVAL;
   if (cap > 0 && (!cand_boxes || !nms_boxes || !nms_scores || !raw_scores || !cand_flat || !cat_ids)) return D2B_EINVAL;
-  if ((reinterpret_cast<uintptr_t>(cand_boxes) & 15) != 0 || (reinterpret_cast<uintptr_t>(nms_boxes) & 15) != 0) return D2B_EINVAL;
-  frcnn_prepare_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(I, boxes, scores, num_classes, kreg, image_hw, score_thresh, cap,
-                                                                 cand_boxes, nms_boxes, nms_scores, raw_scores,
-                                                                 (long long*)cand_flat, (long long*)cat_ids, (long long*)n_cand,
-                                                                 (long long*)row_map);
+  if (Box::D == 4 &&
+      ((reinterpret_cast<uintptr_t>(cand_boxes) & 15) != 0 || (reinterpret_cast<uintptr_t>(nms_boxes) & 15) != 0))
+    return D2B_EINVAL;
+  frcnn_prepare_kernel<Box><<<N, kThreads, 0, (cudaStream_t)stream>>>(I, boxes, scores, num_classes, kreg, image_hw,
+                                                                      score_thresh, cap, seg_per_image, cand_boxes, nms_boxes,
+                                                                      nms_scores, raw_scores, (long long*)cand_flat,
+                                                                      (long long*)cat_ids, (long long*)n_cand,
+                                                                      (long long*)row_map);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
+}
+
+}  // namespace
+
+D2B_API int d2b_frcnn_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes, int kreg,
+                              const float* image_hw, float score_thresh, int cap, float* cand_boxes, float* nms_boxes,
+                              float* nms_scores, float* raw_scores, int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand,
+                              int64_t* row_map, void* stream) {
+  return frcnn_prepare<XyxyBox>(boxes, scores, row_start, N, num_classes, kreg, image_hw, score_thresh, cap, 0, cand_boxes,
+                                nms_boxes, nms_scores, raw_scores, cand_flat, cat_ids, n_cand, row_map, stream);
+}
+
+D2B_API int d2b_frcnn_rotated_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes,
+                                      int kreg, const float* image_hw, float score_thresh, int cap, int seg_per_image,
+                                      float* cand_boxes, float* nms_boxes, float* nms_scores, float* raw_scores,
+                                      int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand, int64_t* row_map, void* stream) {
+  return frcnn_prepare<RotBox>(boxes, scores, row_start, N, num_classes, kreg, image_hw, score_thresh, cap, seg_per_image,
+                               cand_boxes, nms_boxes, nms_scores, raw_scores, cand_flat, cat_ids, n_cand, row_map, stream);
+}
+
+D2B_API int d2b_rrpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int seg_per_image,
+                             float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
+                             int* nonfinite, void* stream) {
+  if (!lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0 || !nonfinite) return D2B_EINVAL;
+  RpnLevels P = {};
+  P.L = lv->num_levels;
+  long long T = 0;
+  for (int l = 0; l < P.L; ++l) {
+    if (lv->A[l] < 0 || lv->k[l] < 0 || lv->k[l] > lv->A[l]) return D2B_EINVAL;
+    if (N > 0 && lv->k[l] > 0 && (!lv->proposals[l] || !lv->topk_idx[l] || !lv->topk_scores[l])) return D2B_EINVAL;
+    P.proposals[l] = lv->proposals[l];
+    P.topk_idx[l] = lv->topk_idx[l];
+    P.topk_scores[l] = lv->topk_scores[l];
+    P.A[l] = lv->A[l];
+    P.k[l] = lv->k[l];
+    P.t0[l] = (int)T;
+    T += lv->k[l];
+  }
+  if (T > INT_MAX) return D2B_EINVAL;
+  P.t0[P.L] = (int)T;
+  if (N > 0 && T > 0 && (!image_hw || !flat_boxes || !nms_boxes || !nms_scores || !raw_scores || !cat_ids)) return D2B_EINVAL;
+  D2B_CUDA(cudaMemsetAsync(nonfinite, 0, sizeof(int), (cudaStream_t)stream));
+  if (N == 0 || T == 0) return D2B_OK;
+  rrpn_prepare_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(P, (int)T, image_hw, min_box_size, seg_per_image, flat_boxes,
+                                                                nms_boxes, nms_scores, raw_scores, (long long*)cat_ids, nonfinite);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }

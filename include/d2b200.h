@@ -259,6 +259,34 @@ int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const 
                       float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
                       int64_t* cat_ids, void* stream);
 
+/* ---- Rotated RRPN proposal selection and rotated Fast R-CNN inference around the NMS -----------------------------
+ * Replace the per-image Python loops of detectron2/modeling/proposal_generator/rrpn.py:20-127 (find_top_rrpn_proposals)
+ * and modeling/roi_heads/rotated_fast_rcnn.py:46-132 (fast_rcnn_inference_rotated) by
+ *   d2b_rrpn_prepare | d2b_frcnn_rotated_prepare  ->  d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET, category =
+ *   image*L + level | image*(K+1) + class, -1 = removed)  ->  d2b_rpn_select_rotated.
+ * Boxes are (cx, cy, w, h, angle_deg) fp32, 5 floats per box, no alignment requirement.  Both prepares apply
+ * RotatedBoxes.clip(image, clip_angle_threshold = 1): every angle is normalised to (a + 180) % 360 - 180 (torch's float
+ * remainder), boxes with |angle| <= 1 are clipped as xyxy boxes; and batched_nms_rotated's per-image offsets
+ * category * (max - min + 1) on the centre (layers/nms.py:137-146), over the image's surviving boxes.
+ * seg_per_image != 0 (pass it for iou_threshold <= 0, which IoU 0 passes: the reference's single NMS then suppresses
+ * across categories too): every surviving candidate of image n gets category n instead, offsets unchanged; the NMS
+ * max_segment must then bound the image's slot count.
+ * d2b_rrpn_prepare: as d2b_rpn_prepare with lv->proposals[l] [N,A_l,5]; removed = non-finite or w / h not larger than
+ *   min_box_size after clipping (RotatedBoxes.nonempty); flat_boxes / nms_boxes [N*T,5].
+ * d2b_frcnn_rotated_prepare: as d2b_frcnn_prepare with boxes [Rtot, kreg*5]; cand_boxes / nms_boxes [N*cap,5].
+ * d2b_rpn_select_rotated: as d2b_rpn_select with flat_boxes [N*T,5] and out_boxes [N,post_nms_topk,5].
+ * All arguments are checked before the first CUDA call. */
+int d2b_rrpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int seg_per_image,
+                     float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
+                     int* nonfinite, void* stream);
+int d2b_frcnn_rotated_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes,
+                              int kreg, const float* image_hw, float score_thresh, int cap, int seg_per_image,
+                              float* cand_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cand_flat,
+                              int64_t* cat_ids, int64_t* n_cand, int64_t* row_map, void* stream);
+int d2b_rpn_select_rotated(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
+                           const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
+                           float* out_scores, int64_t* out_index, int64_t* counts, void* stream);
+
 /* ---- Mask-head training targets + loss (SURVEY 8f-4) ------------------------------------------------------
  * Replaces, for one image, BitMasks.crop_and_resize (detectron2/structures/masks.py:193-224) + the class gather and
  * binary_cross_entropy_with_logits of mask_rcnn_loss (modeling/roi_heads/mask_head.py:60-112).

@@ -84,10 +84,106 @@ def bench_rotated_pooler(add, refgpu):
     add(name % "bwd" + " former loop", t, refgpu.get(name % "bwd"), "autograd of the per-level loop over our ROIAlignRotated")
 
 
+def _clip_rotated_ref(b, h, w):
+    """RotatedBoxes.clip as the reference writes it (structures/rotated_boxes.py:279-303): torch.where(...)[0] + indexing."""
+    b = b.clone()
+    b[:, 4] = (b[:, 4] + 180.0) % 360.0 - 180.0
+    idx = torch.where(torch.abs(b[:, 4]) <= 1.0)[0]
+    x1, y1 = (b[idx, 0] - b[idx, 2] / 2.0).clamp(0, w), (b[idx, 1] - b[idx, 3] / 2.0).clamp(0, h)
+    x2, y2 = (b[idx, 0] + b[idx, 2] / 2.0).clamp(0, w), (b[idx, 1] + b[idx, 3] / 2.0).clamp(0, h)
+    b[idx, 0], b[idx, 1] = (x1 + x2) / 2.0, (y1 + y2) / 2.0
+    b[idx, 2], b[idx, 3] = torch.min(b[idx, 2], x2 - x1), torch.min(b[idx, 3], y2 - y1)
+    return b
+
+
+def bench_rotated_inference(add):
+    """find_top_rrpn_proposals and fast_rcnn_inference_rotated against the reference's per-image loops (rrpn.py:90-126,
+    rotated_fast_rcnn.py:98-132) on the same GPU over this library's batched_nms_rotated."""
+    from detectron2_b200.rotated_fast_rcnn import fast_rcnn_inference_rotated
+    from detectron2_b200.rrpn import find_top_rrpn_proposals
+
+    gb = torch.Generator().manual_seed(13)
+    # p2..p6 of an 800 x 1344 input, 9 anchors per location (3 ratios x 3 angles)
+    per_level = [9 * h * w for h, w in ((200, 336), (100, 168), (50, 84), (25, 42), (13, 21))]
+    pp, ll = [], []
+    for a in per_level:
+        ctr = torch.rand(2, a, 2, generator=gb) * torch.tensor([1400.0, 850.0]) - 20
+        wh = torch.exp(torch.rand(2, a, 2, generator=gb) * 5.0) + 0.5
+        ang = (torch.randint(0, 3, (2, a, 1), generator=gb).float() - 1) * 60 + torch.randn(2, a, 1, generator=gb) * 5
+        pp.append(torch.cat([ctr, wh, ang], 2).to(DEV))
+        ll.append(torch.randn(2, a, generator=gb).to(DEV))
+    szs = [(800, 1344), (800, 1344)]
+
+    def ref_rrpn(pre, post):
+        bi = torch.arange(2, device=DEV)
+        ts, tp, lv = [], [], []
+        for lid, (p_i, l_i) in enumerate(zip(pp, ll)):
+            k = min(l_i.shape[1], pre)
+            s_i, idx = l_i.topk(k, dim=1)
+            tp.append(p_i[bi[:, None], idx]); ts.append(s_i); lv.append(torch.full((k,), lid, dtype=torch.int64, device=DEV))
+        ts, tp, lv = torch.cat(ts, 1), torch.cat(tp, 1), torch.cat(lv, 0)
+        outs = []
+        for n_, (h_, w_) in enumerate(szs):
+            b_, s_, l_ = tp[n_], ts[n_], lv
+            v_ = torch.isfinite(b_).all(1) & torch.isfinite(s_)
+            if not v_.all():
+                b_, s_, l_ = b_[v_], s_[v_], l_[v_]
+            b_ = _clip_rotated_ref(b_, h_, w_)
+            kp = (b_[:, 2] > 0) & (b_[:, 3] > 0)
+            if kp.sum().item() != len(b_):
+                b_, s_, l_ = b_[kp], s_[kp], l_[kp]
+            kk_ = L.batched_nms_rotated(b_, s_, l_, 0.7)[:post]
+            outs.append((b_[kk_], s_[kk_]))
+        return outs
+
+    for pre, post, tag in ((2000, 2000, "train"), (1000, 1000, "test")):
+        t = timeit(lambda: find_top_rrpn_proposals(pp, ll, szs, 0.7, pre, post, 0.0, tag == "train"), rep=10)
+        tr = timeit(lambda: ref_rrpn(pre, post), rep=10)
+        add("find_top_rrpn_proposals 2 img x p2-p6 800x1344 x 9 anchors, top %d/%d (%s)" % (pre, post, tag), t, tr,
+            "ref = reference per-image loop over our batched_nms_rotated")
+    k_cls, r = 15, 1000
+    boxes, scores = [], []
+    for _ in range(2):
+        base = torch.cat([torch.rand(80, 2, generator=gb) * torch.tensor([1300.0, 780.0]),
+                          8 + torch.rand(80, 2, generator=gb) * 250, (torch.rand(80, 1, generator=gb) - 0.5) * 180], 1)
+        b = base[torch.randint(0, 80, (r,), generator=gb)][:, None, :] + torch.randn(r, k_cls, 5, generator=gb) * torch.tensor(
+            [6.0, 6.0, 4.0, 4.0, 3.0])
+        boxes.append(b.reshape(r, k_cls * 5).to(DEV))
+        scores.append(torch.softmax(torch.randn(r, k_cls + 1, generator=gb) * 2.0, dim=1).to(DEV))
+    shapes = [(800, 1344), (800, 1344)]
+
+    def ref_frcnn():
+        res = []
+        for b_, s_, (h_, w_) in zip(boxes, scores, shapes):
+            v_ = torch.isfinite(b_).all(1) & torch.isfinite(s_).all(1)
+            if not v_.all():
+                b_, s_ = b_[v_], s_[v_]
+            s_ = s_[:, :-1]
+            bb = _clip_rotated_ref(b_.reshape(-1, 5), h_, w_).view(-1, k_cls, 5)
+            fm = s_ > 0.05
+            fi = fm.nonzero()
+            bb, sc = bb[fm], s_[fm]
+            kk_ = L.batched_nms_rotated(bb, sc, fi[:, 1], 0.5)[:100]
+            res.append((bb[kk_], sc[kk_], fi[kk_, 1], fi[kk_, 0]))
+        return res
+
+    t = timeit(lambda: fast_rcnn_inference_rotated(boxes, scores, shapes, 0.05, 0.5, 100), rep=10)
+    tr = timeit(ref_frcnn, rep=10)
+    add("fast_rcnn_inference_rotated 2 img x 1000 rows x 15 classes", t, tr,
+        "ref = reference per-image loop over our batched_nms_rotated")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "r2_ops.md"))
+    ap.add_argument("--rotated-inference-only", action="store_true", help="only the rotated RRPN / Fast R-CNN inference rows")
     args = ap.parse_args()
+    if args.rotated_inference_only:
+        def show(name, ours_us, ref_us, note=""):
+            print("%-58s ours %9.1f us   ref-gpu %9.1f us   %s" % (name, ours_us, ref_us, note), flush=True)
+
+        bench_rotated_inference(show)
+        return
     try:
         import torchvision
         tv = torchvision.ops
@@ -229,6 +325,7 @@ def main():
     t = timeit(lambda: torch.autograd.grad(yr, xrg, gor, retain_graph=True))
     add("roi_align_rotated bwd 512 boxes, 2x256x50x84", t, refgpu.get("roi_align_rotated bwd 512 boxes, 2x256x50x84"), "ref = reference csrc CUDA")
     bench_rotated_pooler(add, refgpu)
+    bench_rotated_inference(add)
     # ---- paste
     masks, det = d["masks"].to(DEV), d["det_boxes"][:100].to(DEV)
     t = timeit(lambda: L.paste_masks_in_image(masks, det, (800, 1333), 0.5))
