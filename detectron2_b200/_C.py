@@ -27,6 +27,8 @@ MAX_IMAGES = 64  # D2B_MAX_IMAGES
 ABI_VERSION = 4  # include/d2b200.h D2B_ABI_VERSION
 DCN_X_NHWC = 1   # D2B_DCN_X_NHWC
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}  # D2B_F32 / D2B_F16 / D2B_BF16
+MATCH_ROTATED, MATCH_LOW_QUALITY, MATCH_APPEND_GT = 1, 2, 4  # D2B_MATCH_*
+MATCH_MAX_THRESHOLDS = 8  # D2B_MATCH_MAX_THRESHOLDS
 
 
 class Pyramid(C.Structure):
@@ -91,6 +93,9 @@ def _declare(lib):
         "d2b_mask_loss_forward": (i, [f32p, i, i, i, u8p, i, i, i, f32p, i64p, i64p, f32p, u8p, vp]),
         "d2b_mask_loss_backward": (i, [f32p, i, i, i, u8p, i64p, f32p, f32p, vp]),
         "d2b_box_iou_rotated": (i, [f32p, i64, f32p, i64, f32p, vp]),
+        "d2b_match_workspace_bytes": (sz, [i, i, i]),
+        "d2b_match_boxes": (i, [f32p, i64p, i, i, f32p, i64, i64p, i, C.POINTER(C.c_double), i, C.POINTER(C.c_int), i, f32p, d,
+                                i64p, i64, i64p, vp, f32p, i64p, vp, vp, sz, vp]),
         "d2b_deform_conv_tc_shape_supported": (i, [C.POINTER(DcnParams), i]),
         "d2b_deform_conv_forward_workspace_bytes": (sz, [C.POINTER(DcnParams), i, i]),
         "d2b_deform_conv_cols_bytes": (sz, [C.POINTER(DcnParams), i]),

@@ -287,6 +287,39 @@ int d2b_rpn_select_rotated(const int64_t* keep, const int64_t* num_keep, int N, 
                            const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
                            float* out_scores, int64_t* out_index, int64_t* counts, void* stream);
 
+/* ---- Anchor / proposal matching for the training targets -------------------------------------------------------
+ * Replaces the per-image pairwise_iou + Matcher loops of RPN / RRPN.label_and_sample_anchors, RetinaNet.label_anchors,
+ * (R)ROIHeads.label_and_sample_proposals and CascadeROIHeads._match_and_label_boxes up to their sampling step, for all
+ * images at once and without the G x A IoU matrix (structures/boxes.py:312-358, modeling/matcher.py:61-127).
+ *   gt_boxes [N,Gmax,D] fp32 with gt_count [N] (device, int64; clamped to [0, Gmax]); D = 4 xyxy, or 5 (cx,cy,w,h,angle_deg)
+ *   with D2B_MATCH_ROTATED.  pred_boxes [A,D] shared by every image (pred_image_stride 0, anchors) or [N,stride,D] per image
+ *   (pred_image_stride >= Pmax rows); pred_count [N] (device, int64, clamped to [0, Pmax]) or NULL for Pmax.
+ *   D2B_MATCH_APPEND_GT: the image's GT boxes follow its pred_count predictions (add_ground_truth_to_proposals); output row
+ *   p >= pred_count[n] is GT p - pred_count[n].  Output rows per image P = Pmax (+ Gmax with D2B_MATCH_APPEND_GT).
+ *   thresholds[num_thresholds] (HOST, compared in fp32) and labels[num_thresholds + 1] (HOST) as Matcher(thresholds, labels):
+ *   thresholds[0] > 0, ascending, labels in {-1, 0, 1}, 1 <= num_thresholds <= D2B_MATCH_MAX_THRESHOLDS.
+ *   D2B_MATCH_LOW_QUALITY = allow_low_quality_matches.  boundary_thresh >= 0 (axis-aligned only): after the matcher, rows
+ *   whose box is not Boxes.inside_box(image_hw[n], boundary_thresh) get label -1; image_hw [N,2] (h, w) fp32 device.
+ * Outputs [N,P]: matches (int64, first GT on ties), match_labels (int8), matched_gt_boxes [N,P,D] (NULL-able; zeros for an
+ *   image without GT), classes (NULL-able; needs gt_classes [N,Gmax] int64: label 1 -> gt_classes[match], 0 -> num_classes,
+ *   -1 -> -1, an image without GT -> num_classes).  Rows past pred_count (+ gt_count) are padding: match 0, label -1, zero
+ *   box, class -1.  An image without GT gets matches 0 and label labels[0], as the reference.  status [N] int32:
+ *   D2B_MATCH_STATUS_INVALID_IOU when an IoU of the image is negative or NaN (the reference's assertion; the image's other
+ *   outputs are then unspecified).  workspace: d2b_match_workspace_bytes(N, Gmax, P) bytes, no initialisation needed.
+ * No host synchronisation, static shapes: capturable in a CUDA graph.  All arguments are checked before the first CUDA call. */
+#define D2B_MATCH_ROTATED 1
+#define D2B_MATCH_LOW_QUALITY 2
+#define D2B_MATCH_APPEND_GT 4
+#define D2B_MATCH_MAX_THRESHOLDS 8
+#define D2B_MATCH_STATUS_INVALID_IOU 1
+size_t d2b_match_workspace_bytes(int N, int Gmax, int P);
+int d2b_match_boxes(const float* gt_boxes, const int64_t* gt_count, int N, int Gmax, const float* pred_boxes,
+                    int64_t pred_image_stride, const int64_t* pred_count, int Pmax, const double* thresholds,
+                    int num_thresholds, const int* labels, int flags, const float* image_hw, double boundary_thresh,
+                    const int64_t* gt_classes, int64_t num_classes, int64_t* matches, int8_t* match_labels,
+                    float* matched_gt_boxes, int64_t* classes, int* status, void* workspace, size_t workspace_bytes,
+                    void* stream);
+
 /* ---- Mask-head training targets + loss (SURVEY 8f-4) ------------------------------------------------------
  * Replaces, for one image, BitMasks.crop_and_resize (detectron2/structures/masks.py:193-224) + the class gather and
  * binary_cross_entropy_with_logits of mask_rcnn_loss (modeling/roi_heads/mask_head.py:60-112).

@@ -173,16 +173,88 @@ def bench_rotated_inference(add):
         "ref = reference per-image loop over our batched_nms_rotated")
 
 
+def bench_matching(add):
+    """Fused matching (d2b_match_boxes through detectron2_b200.matching) against the reference's per-image loop of torch
+    ops on the same GPU (pairwise_iou + Matcher + inside_box + the box / class gathers; the rotated IoU of that loop is
+    this library's d2b_box_iou_rotated).  Both sides stop before the sampling, which is the same torch code on both."""
+    from detectron2_b200 import matching as mt
+
+    g = torch.Generator(device=DEV).manual_seed(0)
+
+    def xyxy(n, smax):
+        c = torch.rand(n, 2, generator=g, device=DEV) * torch.tensor([1344.0, 800.0], device=DEV)
+        wh = torch.rand(n, 2, generator=g, device=DEV) * smax + 4
+        return torch.cat([c - wh / 2, c + wh / 2], 1)
+
+    def rot(n, smax):
+        c = torch.rand(n, 2, generator=g, device=DEV) * torch.tensor([1344.0, 800.0], device=DEV)
+        wh = torch.rand(n, 2, generator=g, device=DEV) * smax + 4
+        return torch.cat([c, wh, (torch.rand(n, 1, generator=g, device=DEV) - 0.5) * 180], 1)
+
+    def ref_loop(preds, gts, matcher, sizes=None, bt=-1, cls=None, num_classes=80):
+        out = []
+        for i, gt in enumerate(gts):
+            p = preds[i] if isinstance(preds, list) else preds
+            m, lab = matcher(mt._iou(gt, p))
+            if bt >= 0:
+                lab[~mt.inside_box(p, sizes[i], bt)] = -1
+            c = mt._class_targets(m, lab, cls[i], num_classes) if cls is not None else None
+            out.append((m, lab, gt[m], c))
+        return out
+
+    def fused(preds, gts, matcher, **kw):
+        gt, cnt = mt._pad(gts, gts[0].shape[-1], DEV)
+        if isinstance(preds, list):
+            pr, pc = mt._pad(preds, preds[0].shape[-1], DEV)
+            return mt.match_boxes_fixed(gt, cnt, pr, matcher, pred_count=pc, **kw)
+        return mt.match_boxes_fixed(gt, cnt, preds, matcher, **kw)
+
+    sizes = [(800, 1344), (800, 1344)]
+    anchors = xyxy(268569, 600.0)
+    for G in (7, 100):
+        gts = [xyxy(G, 400.0), xyxy(G, 400.0)]
+        m = mt.Matcher([0.3, 0.7], [0, -1, 1], True)
+        t = timeit(lambda: fused(anchors, gts, m, image_hw=sizes, boundary_thresh=0), rep=10)
+        tr = timeit(lambda: ref_loop(anchors, gts, m, sizes, 0), rep=10)
+        add("match RPN 2 img x 268569 anchors, G = %d" % G, t, tr, "labels + boxes, boundary 0")
+    ret_anchors = xyxy(201600, 500.0)
+    gts = [xyxy(40, 400.0), xyxy(40, 400.0)]
+    cls = [torch.randint(0, 80, (40,), generator=g, device=DEV) for _ in gts]
+    m = mt.Matcher([0.4, 0.5], [0, -1, 1], True)
+    gcls = mt._pad_classes(cls, DEV)
+    t = timeit(lambda: fused(ret_anchors, gts, m, gt_classes=gcls, num_classes=80), rep=10)
+    tr = timeit(lambda: ref_loop(ret_anchors, gts, m, cls=cls), rep=10)
+    add("match RetinaNet 2 img x 201600 anchors, G = 40", t, tr, "labels + boxes + classes")
+    props = [xyxy(2000, 400.0), xyxy(2000, 400.0)]
+    m = mt.Matcher([0.5], [0, 1], False)
+    t = timeit(lambda: fused(props, gts, m, append_gt=True, gt_classes=gcls, num_classes=80), rep=10)
+    tr = timeit(lambda: ref_loop([torch.cat([p, x]) for p, x in zip(props, gts)], gts, m, cls=cls), rep=10)
+    add("match ROI heads 2 img x (2000 + 40) proposals", t, tr, "proposal_append_gt, classes")
+    ms = [mt.Matcher([th], [0, 1], False) for th in (0.5, 0.6, 0.7)]
+    t = timeit(lambda: [fused(props, gts, mm, gt_classes=gcls, num_classes=80) for mm in ms], rep=10)
+    tr = timeit(lambda: [ref_loop(props, gts, mm, cls=cls) for mm in ms], rep=10)
+    add("match cascade 3 stages x 2 img x 2000 proposals", t, tr, "classes + boxes")
+    ranchors = rot(805707, 500.0)
+    rgts = [rot(20, 300.0), rot(20, 300.0)]
+    m = mt.Matcher([0.3, 0.7], [0, -1, 1], True)
+    t = timeit(lambda: fused(ranchors, rgts, m), rep=5, warm=1)
+    tr = timeit(lambda: ref_loop(ranchors, rgts, m), rep=5, warm=1)
+    add("match RRPN 2 img x 805707 anchors, G = 20", t, tr,
+        "%.2f G rotated IoU pairs/s (fused)" % (2 * 805707 * 20 / t * 1e-3))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "r2_ops.md"))
     ap.add_argument("--rotated-inference-only", action="store_true", help="only the rotated RRPN / Fast R-CNN inference rows")
+    ap.add_argument("--matching-only", action="store_true", help="only the anchor / proposal matching rows")
     args = ap.parse_args()
-    if args.rotated_inference_only:
+    if args.rotated_inference_only or args.matching_only:
         def show(name, ours_us, ref_us, note=""):
             print("%-58s ours %9.1f us   ref-gpu %9.1f us   %s" % (name, ours_us, ref_us, note), flush=True)
 
-        bench_rotated_inference(show)
+        print(torch.cuda.get_device_name(0), flush=True)
+        (bench_matching if args.matching_only else bench_rotated_inference)(show)
         return
     try:
         import torchvision
