@@ -76,7 +76,9 @@ struct Epi {
   int relu;
 };
 
-struct K1P { int BN, noct, nkp, ksplit, S, tap_bytes, stage_bytes, red; };  // red: k-split partial sums meet through red.add
+// noct: output-channel tiles of a super-group; goct: those of them the launch computes (noct, or 1 when the column-fed K1c
+// computes the others); red: k-split partial sums meet through red.add
+struct K1P { int BN, noct, goct, nkp, ksplit, S, tap_bytes, stage_bytes, red; };
 struct K2P { int mper, msplit, tap_bytes; };
 struct K3P { int BN, noct, sper, nsplit, S, stage_bytes; };
 
@@ -152,11 +154,13 @@ int best_split(long long base, int work, int max_split, int overhead) {
   return best;
 }
 
-bool plan_k1(const TC& d, K1P& k) {
+// colfed: the gathering K1 runs output-channel tile 0 only and K1c the others (plan_k1c)
+bool plan_k1(const TC& d, K1P& k, bool colfed = false) {
   k.BN = largest_tile(d.ops);
   if (k.BN < 16) return false;
   k.noct = d.ops / k.BN;
-  const int base = d.N * d.tiles_img * d.SG * k.noct;
+  k.goct = colfed ? 1 : k.noct;
+  const int base = d.N * d.tiles_img * d.SG * k.goct;
   k.ksplit = best_split(base, d.KK, d.KK, 1);
   k.nkp = d2b_cdiv(d.KK, k.ksplit);
   k.ksplit = d2b_cdiv(d.KK, k.nkp);
@@ -167,6 +171,24 @@ bool plan_k1(const TC& d, K1P& k) {
   k.S = 3;
   while (k.S > 1 && k.S * k.stage_bytes + k.tap_bytes + 1024 + 128 > kMaxSmem) --k.S;
   return k.S >= 2;
+}
+
+// K1c: output-channel tiles 1..noct-1 of a column-fed forward, split over kernel points on its own grid.  Both launches
+// write the same output: if either splits, both add their partials (k1.red and kc.red are set together).
+bool plan_k1c(const TC& d, K1P& k1, K1P& kc) {
+  const long long base = (long long)d.N * d.tiles_img * d.SG * (k1.noct - 1);
+  if (k1.goct != 1 || k1.noct < 2 || (long long)d.N * d.tiles_img * (k1.noct - 1) > 0x7fffffffLL) return false;
+  kc = k1;
+  kc.goct = k1.noct - 1;
+  kc.ksplit = best_split(base, d.KK, d.KK, 1);
+  kc.nkp = d2b_cdiv(d.KK, kc.ksplit);
+  kc.ksplit = d2b_cdiv(d.KK, kc.nkp);
+  kc.tap_bytes = 0;
+  kc.S = 3;
+  while (kc.S > 1 && kc.S * kc.stage_bytes + 1024 + 128 > kMaxSmem) --kc.S;
+  if (kc.S < 2) return false;
+  k1.red = kc.red = k1.ksplit > 1 || kc.ksplit > 1;
+  return true;
 }
 
 bool plan_k2(const TC& d, K2P& k) {
@@ -329,8 +351,33 @@ __device__ __forceinline__ int acc_col(int i) {
   return (threadIdx.x >> 8) * (BN / 2) + (i >> 2) * 8 + (threadIdx.x & 3) * 2 + (i & 1);
 }
 
+// Forward epilogue of K1 and K1c: accumulator tile [128 px][BN oc] -> scale / shift / ReLU -> NCHW out.  With a k-split
+// (k.red) the partial sums meet through red.add in the zero-filled output and dcn_epilogue_kernel applies scale / ReLU once
+// all of them are in; the shift is added here by the first split only when nothing else is to be applied after it.
+template <int BN>
+__device__ __forceinline__ void fwd_epilogue(const float (&acc)[BN / 4], const Epi& ep, const TC& d, const K1P& k,
+                                             float* __restrict__ out, int b, int p0, int oc0) {
+  const bool add_shift = ep.shift != nullptr && blockIdx.z == 0;
+#pragma unroll
+  for (int i = 0; i < BN / 4; ++i) {
+    const int p = p0 + acc_row<BN>(i);
+    if (p >= d.HoWo) continue;
+    const int oc = oc0 + acc_col<BN>(i);
+    float* dst = out + ((size_t)b * d.Cout + oc) * d.HoWo + p;
+    float v = acc[i];
+    if (k.red) {
+      red_add(dst, v + ((add_shift && !ep.scale && !ep.relu) ? __ldg(ep.shift + oc) : 0.f));
+    } else {
+      if (ep.scale) v *= __ldg(ep.scale + oc);
+      if (ep.shift) v += __ldg(ep.shift + oc);
+      if (ep.relu) v = fmaxf(v, 0.f);
+      *dst = v;
+    }
+  }
+}
+
 // ================================================================================================ K1: forward
-// grid (N * tiles_img, SG * oc tiles, k splits).  Warp 17 is the SAVER, which (when the caller keeps the
+// grid (N * tiles_img, SG * k.goct, k splits).  Warp 17 is the SAVER, which (when the caller keeps the
 // sampled columns for the weight gradient) copies every finished A stage -- already bf16 hi | lo in the tensor core's
 // swizzled tile layout -- to global memory with one bulk store, so that the backward streams the tiles back instead of
 // sampling x a second time (dcn_bwd_weight_cols_kernel).  Column tile of (image tile, super-group, unit): 16 KB hi [+ 16 KB lo].
@@ -352,7 +399,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.x / d.tiles_img, p0 = (blockIdx.x - b * d.tiles_img) * 128;
-  const int sg = blockIdx.y / k.noct, oct = blockIdx.y - sg * k.noct;
+  const int sg = blockIdx.y / k.goct, oct = blockIdx.y - sg * k.goct;
   const int kp0 = blockIdx.z * k.nkp, nkp = min(d.KK, kp0 + k.nkp) - kp0;
   const int nt = nkp * d.cbs;
   const int dg0 = (sg * d.cps) / d.cpdg;
@@ -427,25 +474,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
       if (lane == 0) mbar_arrive(&empty_bar[(t - 1) % k.S]);
     }
     wgmma_wait<0>();
-    // =============================================================== EPILOGUE: registers -> NCHW global
-    const int oc0 = sg * d.ops + oct * k.BN;
-    const bool add_shift = ep.shift != nullptr && blockIdx.z == 0;
-#pragma unroll
-    for (int i = 0; i < BN / 4; ++i) {
-      const int p = p0 + acc_row<BN>(i);
-      if (p >= d.HoWo) continue;
-      const int oc = oc0 + acc_col<BN>(i);
-      float* dst = out + ((size_t)b * d.Cout + oc) * d.HoWo + p;
-      float v = acc[i];
-      if (k.red) {  // k-split partial sums: scale / relu run in dcn_epilogue_kernel once all partials are in
-        red_add(dst, v + ((add_shift && !ep.scale && !ep.relu) ? __ldg(ep.shift + oc) : 0.f));
-      } else {
-        if (ep.scale) v *= __ldg(ep.scale + oc);
-        if (ep.shift) v += __ldg(ep.shift + oc);
-        if (ep.relu) v = fmaxf(v, 0.f);
-        *dst = v;
-      }
-    }
+    fwd_epilogue<BN>(acc, ep, d, k, out, b, p0, sg * d.ops + oct * k.BN);
   } else if (warp == kWorkerWarps) {
     // =============================================================== TMA producer: weight tile of every chunk
     if (lane == 0) {
@@ -474,6 +503,83 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
         mbar_arrive(&empty_bar[s]);
       }
       bulk_wait0();
+    }
+  }
+}
+
+// ================================================================================================ K1c: forward from saved columns
+// Output-channel tiles 1..noct-1 of a forward that saves its columns: K1 gathers and saves them once (tile 0), and this kernel
+// streams each stage's column tile back with one bulk copy (hi [+ lo], already in K1's swizzled A layout) next to K1's weight
+// tile of its output-channel tile: a pure TMA -> wgmma pipeline like K3c, with K1's epilogue.  grid ((N * tiles_img) *
+// (noct - 1), SG, k splits), the output-channel tile fastest: the CTAs that read one column tile run together and share it in L2.
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1) dcn_fwd_cols_kernel(const uint8_t* __restrict__ cols,
+                                                                   const uint8_t* __restrict__ wt, const Epi ep, const TC d,
+                                                                   const K1P k, const int split, float* __restrict__ out) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + k.S * k.stage_bytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + k.S;
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tile = blockIdx.x / k.goct, oct = 1 + (blockIdx.x - tile * k.goct);
+  const int b = tile / d.tiles_img, p0 = (tile - b * d.tiles_img) * 128;
+  const int sg = blockIdx.y;
+  const int kp0 = blockIdx.z * k.nkp, nkp = min(d.KK, kp0 + k.nkp) - kp0;
+  const int nt = nkp * d.cbs;
+
+  if (tid == 0) {
+    for (int s = 0; s < k.S; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kWorkerWarps);
+    }
+    mbar_init_fence();
+  }
+  __syncthreads();
+  if (warp < kWorkerWarps) reg_alloc<kWorkerRegs>();
+  else reg_dealloc<kSideRegs>();
+
+  if (warp < kWorkerWarps) {
+    float acc[BN / 4];
+#pragma unroll
+    for (int i = 0; i < BN / 4; ++i) acc[i] = 0.f;
+    auto issue = [&](int t) {
+      const int s = t % k.S;
+      mbar_wait(&full_bar[s], (uint32_t)((t / k.S) & 1));
+      const uint32_t sa = smem_u32(smem + s * k.stage_bytes), sb = sa + 2 * kTile;
+      mma_stage<BN, 0>(acc, sa, sa + kTile, sb, sb + (uint32_t)BN * 128u, split);
+    };
+    issue(0);  // as in K1: one wgmma group in flight at every pass through the loop head
+    for (int t = 1; t < nt; ++t) {
+      issue(t);
+      wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[(t - 1) % k.S]);
+    }
+    wgmma_wait<0>();
+    fwd_epilogue<BN>(acc, ep, d, k, out, b, p0, sg * d.ops + oct * k.BN);
+  } else if (warp == kWorkerWarps) {
+    // =============================================================== TMA producer: column tile + weight tile per stage
+    if (lane == 0) {
+      const uint32_t parts = split ? 2u : 1u;
+      // pointers and ring position advance with the stage (this warp runs on kSideRegs registers)
+      const uint32_t abytes = parts * (uint32_t)kTile;
+      const size_t u0 = (size_t)kp0 * d.cbs;
+      const uint8_t* asrc = cols + (((size_t)tile * d.SG + sg) * d.U + u0) * abytes;  // as K1's saver wrote them
+      const uint8_t* bsrc = wt + ((size_t)(sg * k.noct + oct) * d.U + u0) * (size_t)(2 * BN * 128);
+      int s = 0;
+      uint32_t par = 1u;
+      for (int t = nt; t > 0; --t, asrc += abytes, bsrc += 2 * BN * 128) {
+        mbar_wait(&empty_bar[s], par);
+        mbar_arrive_expect_tx(&full_bar[s], abytes / 128u * (128u + BN));
+        bulk_g2s(smem + s * k.stage_bytes, asrc, abytes, &full_bar[s]);
+        bulk_g2s(smem + s * k.stage_bytes + 2 * kTile, bsrc, abytes / 128u * BN, &full_bar[s]);
+        if (++s == k.S) {
+          s = 0;
+          par ^= 1u;
+        }
+      }
     }
   }
 }
@@ -772,7 +878,7 @@ __global__ void __launch_bounds__(256) dcn_gw_reduce_tile_kernel(const float* __
 }
 
 // ================================================================================================ K3: backward weight
-// grid (M blocks = pairs of units, pixel splits, SG * oc tiles).  D[128 k'][BN oc] += col^T[128 k'][64 px] . gout[64 px][BN oc]
+// grid (SG * oc tiles, M blocks = pairs of units, pixel splits).  D[128 k'][BN oc] += col^T[128 k'][64 px] . gout[64 px][BN oc]
 // per 64-pixel stage; the gathered tile is written [unit half][pixel][64 ch] = MN-major for the tensor core.  As in K1 the
 // workers issue the MMAs of a stage after gathering it and release the previous stage once its MMAs are done.
 template <int BN>
@@ -790,10 +896,10 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const fl
   uint64_t* empty_bar = bars + k.S;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int mb = blockIdx.x;
-  const int sg = blockIdx.z / k.noct, oct = blockIdx.z - sg * k.noct;
+  const int mb = blockIdx.y;
+  const int sg = blockIdx.x / k.noct, oct = blockIdx.x - sg * k.noct;
   const int total = d.N * d.stages_img;
-  const int gs0 = blockIdx.y * k.sper, gs1 = min(total, gs0 + k.sper), ns = gs1 - gs0;
+  const int gs0 = blockIdx.z * k.sper, gs1 = min(total, gs0 + k.sper), ns = gs1 - gs0;
 
   if (tid == 0) {
     for (int s = 0; s < k.S; ++s) {
@@ -918,10 +1024,10 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const 
   uint64_t* empty_bar = bars + S;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int mb = blockIdx.x;
-  const int sg = blockIdx.z / k.noct, oct = blockIdx.z - sg * k.noct;
+  const int mb = blockIdx.y;
+  const int sg = blockIdx.x / k.noct, oct = blockIdx.x - sg * k.noct;
   const int total = d.N * d.stages_img;
-  const int gs0 = blockIdx.y * k.sper, gs1 = min(total, gs0 + k.sper), ns = gs1 - gs0;
+  const int gs0 = blockIdx.z * k.sper, gs1 = min(total, gs0 + k.sper), ns = gs1 - gs0;
   const int nu = (2 * mb + 1 < d.U) ? 2 : 1;
 
   if (tid == 0) {
@@ -1259,11 +1365,22 @@ int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float*
     dcn_wtile_fwd_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(weight, d, k.BN, k.noct, wt);
     D2B_CHECK_LAUNCH();
   }
+  // With saved columns, the gathering K1 computes output-channel tile 0 only and K1c the others from its columns, so that x
+  // is sampled once per layer rather than once per output-channel tile.
+  K1P kc;
+  bool colfed = false;
+  if (cols && k.noct > 1) {
+    K1P k1;
+    if (plan_k1(d, k1, true) && plan_k1c(d, k1, kc)) {
+      k = k1;
+      colfed = true;
+    }
+  }
   if (k.red) D2B_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)d.N * d.Cout * d.HoWo, stream));
   const int smem_bytes = k.S * k.stage_bytes + k.tap_bytes + 1024 + 128;
   const int split = precision == 1 ? 1 : 0;
   const Epi ep = {scale, shift, relu};
-  dim3 grid(d.N * d.tiles_img, d.SG * k.noct, k.ksplit);
+  dim3 grid(d.N * d.tiles_img, d.SG * k.goct, k.ksplit);
 #define D2B_LAUNCH_K1(BN)                                                                                              \
   {                                                                                                                    \
     D2B_ALLOW_BIG_SMEM(dcn_fwd_tc_kernel<BN>);                                                                         \
@@ -1276,6 +1393,22 @@ int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float*
   else D2B_LAUNCH_K1(128)
 #undef D2B_LAUNCH_K1
   D2B_CHECK_LAUNCH();
+  if (colfed) {
+    const int smem_c = kc.S * kc.stage_bytes + 1024 + 128;
+    dim3 grid_c(d.N * d.tiles_img * kc.goct, d.SG, kc.ksplit);
+    const uint8_t* cl = reinterpret_cast<const uint8_t*>(cols);
+#define D2B_LAUNCH_K1C(BN)                                                                                             \
+  {                                                                                                                    \
+    D2B_ALLOW_BIG_SMEM(dcn_fwd_cols_kernel<BN>);                                                                       \
+    dcn_fwd_cols_kernel<BN><<<grid_c, kThreads, smem_c, stream>>>(cl, wt, ep, d, kc, split, out);                      \
+  }
+    if (kc.BN == 16) D2B_LAUNCH_K1C(16)
+    else if (kc.BN == 32) D2B_LAUNCH_K1C(32)
+    else if (kc.BN == 64) D2B_LAUNCH_K1C(64)
+    else D2B_LAUNCH_K1C(128)
+#undef D2B_LAUNCH_K1C
+    D2B_CHECK_LAUNCH();
+  }
   if (k.red && (scale || relu)) {
     const long long total = (long long)d.N * d.Cout * d.HoWo;
     dcn_epilogue_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(out, total, d.Cout, d.HoWo, ep);
@@ -1401,7 +1534,9 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
       dcn_gout_oc_tiles_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(grad_out, y_saved, ep, d, k3.BN, k3.noct, gt_oc);
       D2B_CHECK_LAUNCH();
     }
-    dim3 grid(d.MC, k3.nsplit, d.SG * k3.noct);
+    // output-channel tile fastest, then the unit pair: the CTAs that read one column (or gathered) tile and those that read one
+    // grad_out tile run in the same wave and share them in L2
+    dim3 grid(d.SG * k3.noct, d.MC, k3.nsplit);
     if (cols) {  // the forward kept its sampled columns: stream them back (no second pass over x)
       const int S = std::min(6, (kMaxSmem - 2048) / k3.stage_bytes);
       const int smem_bytes = S * k3.stage_bytes + 1024 + 128;
