@@ -1,20 +1,22 @@
 // Batched RPN proposal selection around the NMS (SURVEY.md 8f-2): the two data-dependent stages of
-// detectron2/modeling/proposal_generator/proposal_utils.py:22-135 as fixed-capacity kernels, one CTA per image.
+// detectron2/modeling/proposal_generator/proposal_utils.py:22-135 (find_top_rpn_proposals) and rrpn.py:20-127
+// (find_top_rrpn_proposals) as fixed-capacity kernels, one CTA per image.
 //
-//   d2b_rpn_prepare   gathers the per-level top-k candidates, clips them to the image (Boxes.clip, :112), marks non-finite
-//                     (:104-110) and too-small (:115-119) boxes as IGNORED (category -1) instead of removing them, and
-//                     applies torchvision's batched-NMS coordinate offsets per image -- level * (max coordinate of that
-//                     image's surviving boxes + 1), fp32 -- so that every IoU rounds like the reference's;
-//   d2b_rpn_select    walks the score-ordered keep list of ONE NMS over all images and hands every image its first
+//   d2b_rpn_prepare / d2b_rrpn_prepare   gather the per-level top-k candidates, clip them to the image (Boxes.clip, :112 /
+//                     RotatedBoxes.clip), mark non-finite (:104-110) and too-small (:115-119) boxes as IGNORED (category -1)
+//                     instead of removing them, and apply the batched-NMS coordinate offsets per image -- torchvision's
+//                     level * (max coordinate + 1), or batched_nms_rotated's level * (max - min + 1) on the centres, over
+//                     that image's surviving boxes, fp32 -- so that every IoU rounds like the reference's;
+//   d2b_rpn_select[_rotated]   walks the score-ordered keep list of ONE NMS over all images and hands every image its first
 //                     post_nms_topk survivors (:129) in a fixed [N, post_nms_topk] layout + a count.
 //
 // Together with d2b_nms (category = image * L + level, per-category bound = pre_nms_topk) the whole selection is a
 // sync-free launch sequence with static shapes: capturable in a CUDA graph; the reference loops over images in Python
 // with boolean indexing and one `.item()` per image.  Compiled with -fmad=false like nms.cu (bit-exact clip / offsets).
 //
-// The rotated pipeline has the same shape (rrpn.py:20-127, rotated_fast_rcnn.py:46-132): d2b_rrpn_prepare /
-// d2b_frcnn_rotated_prepare -> d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET) -> d2b_rpn_select_rotated.  The box type is a
-// template policy (XyxyBox / RotBox below) of the shared candidate and selection kernels.
+// The box type is a template policy (XyxyBox / RotBox below) of every candidate and selection kernel in this file:
+// rpn_prepare_kernel, frcnn_prepare_kernel (d2b_frcnn_prepare / d2b_frcnn_rotated_prepare) and rpn_select_kernel; the
+// rotated calls run d2b_nms with D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET.
 #include <climits>
 #include <type_traits>
 
@@ -26,7 +28,7 @@ constexpr int kThreads = 1024;
 
 struct RpnLevels {
   int L;
-  const float* proposals[D2B_MAX_LEVELS];    // [N, A_l, 4]
+  const float* proposals[D2B_MAX_LEVELS];    // [N, A_l, Box::D]
   const int64_t* topk_idx[D2B_MAX_LEVELS];   // [N, k_l]
   const float* topk_scores[D2B_MAX_LEVELS];  // [N, k_l]
   int A[D2B_MAX_LEVELS], k[D2B_MAX_LEVELS], t0[D2B_MAX_LEVELS + 1];  // t0: prefix of k
@@ -48,6 +50,8 @@ struct XyxyBox {
     v[2] = fminf(fmaxf(v[2], 0.f), iw);
     v[3] = fminf(fmaxf(v[3], 0.f), ih);
   }
+  __device__ __forceinline__ float width() const { return v[2] - v[0]; }
+  __device__ __forceinline__ float height() const { return v[3] - v[1]; }
   __device__ __forceinline__ float hi() const { return fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])); }  // boxes.max()
   __device__ __forceinline__ float lo() const { return 0.f; }                                          // not part of the range
   static __device__ __forceinline__ float scale(bool any, float mx, float) { return (any ? mx : 0.f) + 1.0f; }
@@ -77,6 +81,8 @@ struct RotBox {
       v[3] = fminf(v[3], y2 - y1);
     }
   }
+  __device__ __forceinline__ float width() const { return v[2]; }
+  __device__ __forceinline__ float height() const { return v[3]; }
   __device__ __forceinline__ float hi() const { return fmaxf(v[0], v[1]) + fmaxf(v[2], v[3]) / 2; }
   __device__ __forceinline__ float lo() const { return fminf(v[0], v[1]) - fmaxf(v[2], v[3]) / 2; }
   static __device__ __forceinline__ float scale(bool any, float mx, float mn) { return (any ? mx - mn : 0.f) + 1.0f; }
@@ -120,64 +126,6 @@ __device__ __forceinline__ Box zero_box() {
 #pragma unroll
   for (int q = 0; q < Box::D; ++q) b.v[q] = 0.f;
   return b;
-}
-
-__global__ void __launch_bounds__(kThreads) rpn_prepare_kernel(const RpnLevels P, int T, const float* __restrict__ image_hw,
-                                                               float min_box_size, int use_offsets,
-                                                               float* __restrict__ flat_boxes, float* __restrict__ nms_boxes,
-                                                               float* __restrict__ nms_scores, float* __restrict__ raw_scores,
-                                                               long long* __restrict__ cat_ids, int* __restrict__ nonfinite) {
-  __shared__ float s_red[32];
-  __shared__ float s_max;
-  const int n = blockIdx.x, tid = threadIdx.x;
-  const float ih = image_hw[2 * n], iw = image_hw[2 * n + 1];
-  float mx = -INFINITY;
-  int bad = 0;
-  for (int t = tid; t < T; t += kThreads) {
-    int l = 0;
-    while (l + 1 < P.L && t >= P.t0[l + 1]) ++l;
-    const int j = t - P.t0[l];
-    const long long a = P.topk_idx[l][(size_t)n * P.k[l] + j];
-    const float s = P.topk_scores[l][(size_t)n * P.k[l] + j];
-    const float4 b = *reinterpret_cast<const float4*>(P.proposals[l] + ((size_t)n * P.A[l] + a) * 4);
-    const bool fin = finitef(b.x) && finitef(b.y) && finitef(b.z) && finitef(b.w) && finitef(s);
-    // Boxes.clip: x to [0, w], y to [0, h]   (torch.clamp(min=0) then minimum with the size, like the host restatement)
-    const float x1 = fminf(fmaxf(b.x, 0.f), iw), y1 = fminf(fmaxf(b.y, 0.f), ih);
-    const float x2 = fminf(fmaxf(b.z, 0.f), iw), y2 = fminf(fmaxf(b.w, 0.f), ih);
-    const bool valid = fin && (x2 - x1) > min_box_size && (y2 - y1) > min_box_size;
-    const size_t o = (size_t)n * T + t;
-    *reinterpret_cast<float4*>(flat_boxes + o * 4) = valid ? make_float4(x1, y1, x2, y2) : make_float4(0.f, 0.f, 0.f, 0.f);
-    raw_scores[o] = s;
-    nms_scores[o] = valid ? s : -INFINITY;
-    cat_ids[o] = valid ? (long long)n * P.L + l : -1LL;
-    if (valid) mx = fmaxf(mx, fmaxf(fmaxf(x1, y1), fmaxf(x2, y2)));
-    bad |= fin ? 0 : 1;
-  }
-  for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  if ((tid & 31) == 0) s_red[tid >> 5] = mx;
-  if (bad) atomicOr(nonfinite, 1);
-  __syncthreads();
-  if (tid < 32) {
-    mx = s_red[tid];
-    for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if (tid == 0) s_max = mx;
-  }
-  __syncthreads();
-  const float scale = s_max + 1.0f;  // torchvision _batched_nms_coordinate_trick: idxs * (boxes.max() + 1)
-  for (int t = tid; t < T; t += kThreads) {
-    int l = 0;
-    while (l + 1 < P.L && t >= P.t0[l + 1]) ++l;
-    const size_t o = (size_t)n * T + t;
-    float4 b = *reinterpret_cast<const float4*>(flat_boxes + o * 4);
-    if (use_offsets && cat_ids[o] >= 0) {
-      const float off = (float)l * scale;
-      b.x += off;
-      b.y += off;
-      b.z += off;
-      b.w += off;
-    }
-    *reinterpret_cast<float4*>(nms_boxes + o * 4) = b;
-  }
 }
 
 // Exclusive prefix sum of one int per thread over a 1024-thread CTA; `total` = sum.
@@ -247,37 +195,6 @@ __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* _
 }
 
 }  // namespace
-
-D2B_API int d2b_rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int use_offsets,
-                            float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
-                            int* nonfinite, void* stream) {
-  if (!lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0) return D2B_EINVAL;
-  if (!nonfinite) return D2B_EINVAL;
-  D2B_CUDA(cudaMemsetAsync(nonfinite, 0, sizeof(int), (cudaStream_t)stream));
-  if (N == 0) return D2B_OK;
-  if (!image_hw || !flat_boxes || !nms_boxes || !nms_scores || !raw_scores || !cat_ids) return D2B_EINVAL;
-  RpnLevels P = {};
-  P.L = lv->num_levels;
-  int T = 0;
-  for (int l = 0; l < P.L; ++l) {
-    if (!lv->proposals[l] || !lv->topk_idx[l] || !lv->topk_scores[l] || lv->A[l] <= 0 || lv->k[l] < 0 || lv->k[l] > lv->A[l])
-      return D2B_EINVAL;
-    if ((reinterpret_cast<uintptr_t>(lv->proposals[l]) & 15) != 0) return D2B_EINVAL;
-    P.proposals[l] = lv->proposals[l];
-    P.topk_idx[l] = lv->topk_idx[l];
-    P.topk_scores[l] = lv->topk_scores[l];
-    P.A[l] = lv->A[l];
-    P.k[l] = lv->k[l];
-    P.t0[l] = T;
-    T += lv->k[l];
-  }
-  P.t0[P.L] = T;
-  if (T == 0) return D2B_OK;
-  rpn_prepare_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(P, T, image_hw, min_box_size, use_offsets, flat_boxes, nms_boxes,
-                                                               nms_scores, raw_scores, (long long*)cat_ids, nonfinite);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
-}
 
 namespace {
 
@@ -433,14 +350,18 @@ __global__ void __launch_bounds__(kThreads) frcnn_prepare_kernel(const FrcnnImag
   }
 }
 
-// find_top_rrpn_proposals (detectron2/modeling/proposal_generator/rrpn.py:59-113) up to the NMS, one CTA per image: the
-// per-level top-k gather, the finiteness check (:97-105), RotatedBoxes.clip (:106), nonempty (:109) and the per-image
-// offsets of batched_nms_rotated (layers/nms.py:137-146) over the surviving boxes.  Removed boxes get category -1.
-__global__ void __launch_bounds__(kThreads) rrpn_prepare_kernel(const RpnLevels P, int T, const float* __restrict__ image_hw,
-                                                                float min_box_size, int seg_per_image,
-                                                                float* __restrict__ flat_boxes, float* __restrict__ nms_boxes,
-                                                                float* __restrict__ nms_scores, float* __restrict__ raw_scores,
-                                                                long long* __restrict__ cat_ids, int* __restrict__ nonfinite) {
+// find_top_rpn_proposals (proposal_utils.py:60-122) / find_top_rrpn_proposals (rrpn.py:59-113) up to the NMS, one CTA
+// per image: the per-level top-k gather, the finiteness check (:104-110), the box type's clip (:112) and nonempty test
+// (width and height larger than min_box_size, :115-119), and the per-image batched-NMS offsets over the surviving boxes.
+// Removed boxes get category -1.  use_offsets = 0 leaves nms_boxes unshifted (torchvision's batched_nms over more than
+// 25 000 boxes per image); seg_per_image (rotated only) puts every surviving box of image n in NMS category n.
+template <class Box>
+__global__ void __launch_bounds__(kThreads) rpn_prepare_kernel(const RpnLevels P, int T, const float* __restrict__ image_hw,
+                                                               float min_box_size, int use_offsets, int seg_per_image,
+                                                               float* __restrict__ flat_boxes, float* __restrict__ nms_boxes,
+                                                               float* __restrict__ nms_scores, float* __restrict__ raw_scores,
+                                                               long long* __restrict__ cat_ids, int* __restrict__ nonfinite) {
+  constexpr int D = Box::D;
   __shared__ float s_red[32];
   __shared__ float s_max, s_min;
   const int n = blockIdx.x, tid = threadIdx.x;
@@ -453,20 +374,20 @@ __global__ void __launch_bounds__(kThreads) rrpn_prepare_kernel(const RpnLevels 
     const int j = t - P.t0[l];
     const long long a = P.topk_idx[l][(size_t)n * P.k[l] + j];
     const float s = P.topk_scores[l][(size_t)n * P.k[l] + j];
-    RotBox b = load_box<RotBox>(P.proposals[l] + ((size_t)n * P.A[l] + a) * 5);
+    Box b = load_box_aligned<Box>(P.proposals[l] + ((size_t)n * P.A[l] + a) * D);
     bool fin = finitef(s);
 #pragma unroll
-    for (int q = 0; q < 5; ++q) fin = fin && finitef(b.v[q]);
+    for (int q = 0; q < D; ++q) fin = fin && finitef(b.v[q]);
     b.clip(ih, iw);
-    const bool valid = fin && b.v[2] > min_box_size && b.v[3] > min_box_size;
+    const bool valid = fin && b.width() > min_box_size && b.height() > min_box_size;
     const size_t o = (size_t)n * T + t;
-    store_box(flat_boxes + o * 5, valid ? b : zero_box<RotBox>());
+    store_box(flat_boxes + o * D, valid ? b : zero_box<Box>());
     raw_scores[o] = s;
     nms_scores[o] = valid ? s : -INFINITY;
     cat_ids[o] = valid ? (long long)n * P.L + l : -1LL;
     if (valid) {
       mx = fmaxf(mx, b.hi());
-      mn = fminf(mn, b.lo());
+      if constexpr (Box::kRotated) mn = fminf(mn, b.lo());
       any = 1;
     }
     bad |= fin ? 0 : 1;
@@ -474,18 +395,19 @@ __global__ void __launch_bounds__(kThreads) rrpn_prepare_kernel(const RpnLevels 
   if (bad) atomicOr(nonfinite, 1);
   any = __syncthreads_or(any);
   mx = block_max(mx, s_red, &s_max);
-  mn = -block_max(-mn, s_red, &s_min);
-  const float scale = RotBox::scale(any != 0, mx, mn);
+  if constexpr (Box::kRotated) mn = -block_max(-mn, s_red, &s_min);
+  const float scale = Box::scale(any != 0, mx, mn);
   for (int t = tid; t < T; t += kThreads) {
     int l = 0;
     while (l + 1 < P.L && t >= P.t0[l + 1]) ++l;
     const size_t o = (size_t)n * T + t;
-    RotBox b = load_box<RotBox>(flat_boxes + o * 5);
+    Box b = load_box_aligned<Box>(flat_boxes + o * D);
     if (cat_ids[o] >= 0) {
-      b.shift((float)l * scale);
-      if (seg_per_image) cat_ids[o] = n;
+      if (use_offsets) b.shift((float)l * scale);
+      if constexpr (Box::kRotated)
+        if (seg_per_image) cat_ids[o] = n;
     }
-    store_box(nms_boxes + o * 5, b);
+    store_box(nms_boxes + o * D, b);
   }
 }
 
@@ -604,6 +526,41 @@ int frcnn_prepare(const float* boxes, const float* scores, const int* row_start,
   return D2B_OK;
 }
 
+template <class Box>
+int rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int use_offsets, int seg_per_image,
+                float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids, int* nonfinite,
+                void* stream) {
+  if (!lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0 || !nonfinite) return D2B_EINVAL;
+  RpnLevels P = {};
+  P.L = lv->num_levels;
+  long long T = 0;
+  for (int l = 0; l < P.L; ++l) {
+    if (lv->A[l] < 0 || lv->k[l] < 0 || lv->k[l] > lv->A[l]) return D2B_EINVAL;
+    if (N > 0 && lv->k[l] > 0 && (!lv->proposals[l] || !lv->topk_idx[l] || !lv->topk_scores[l])) return D2B_EINVAL;
+    if (Box::D == 4 && (reinterpret_cast<uintptr_t>(lv->proposals[l]) & 15) != 0) return D2B_EINVAL;  // float4 loads
+    P.proposals[l] = lv->proposals[l];
+    P.topk_idx[l] = lv->topk_idx[l];
+    P.topk_scores[l] = lv->topk_scores[l];
+    P.A[l] = lv->A[l];
+    P.k[l] = lv->k[l];
+    P.t0[l] = (int)T;
+    T += lv->k[l];
+  }
+  if (T > INT_MAX) return D2B_EINVAL;
+  P.t0[P.L] = (int)T;
+  if (N > 0 && T > 0 && (!image_hw || !flat_boxes || !nms_boxes || !nms_scores || !raw_scores || !cat_ids)) return D2B_EINVAL;
+  if (Box::D == 4 &&
+      ((reinterpret_cast<uintptr_t>(flat_boxes) & 15) != 0 || (reinterpret_cast<uintptr_t>(nms_boxes) & 15) != 0))
+    return D2B_EINVAL;
+  D2B_CUDA(cudaMemsetAsync(nonfinite, 0, sizeof(int), (cudaStream_t)stream));
+  if (N == 0 || T == 0) return D2B_OK;
+  rpn_prepare_kernel<Box><<<N, kThreads, 0, (cudaStream_t)stream>>>(P, (int)T, image_hw, min_box_size, use_offsets,
+                                                                    seg_per_image, flat_boxes, nms_boxes, nms_scores,
+                                                                    raw_scores, (long long*)cat_ids, nonfinite);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
+}
+
 }  // namespace
 
 D2B_API int d2b_frcnn_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes, int kreg,
@@ -622,33 +579,18 @@ D2B_API int d2b_frcnn_rotated_prepare(const float* boxes, const float* scores, c
                                cand_boxes, nms_boxes, nms_scores, raw_scores, cand_flat, cat_ids, n_cand, row_map, stream);
 }
 
+D2B_API int d2b_rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int use_offsets,
+                            float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
+                            int* nonfinite, void* stream) {
+  return rpn_prepare<XyxyBox>(lv, N, image_hw, min_box_size, use_offsets, 0, flat_boxes, nms_boxes, nms_scores, raw_scores,
+                              cat_ids, nonfinite, stream);
+}
+
 D2B_API int d2b_rrpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int seg_per_image,
                              float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
                              int* nonfinite, void* stream) {
-  if (!lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0 || !nonfinite) return D2B_EINVAL;
-  RpnLevels P = {};
-  P.L = lv->num_levels;
-  long long T = 0;
-  for (int l = 0; l < P.L; ++l) {
-    if (lv->A[l] < 0 || lv->k[l] < 0 || lv->k[l] > lv->A[l]) return D2B_EINVAL;
-    if (N > 0 && lv->k[l] > 0 && (!lv->proposals[l] || !lv->topk_idx[l] || !lv->topk_scores[l])) return D2B_EINVAL;
-    P.proposals[l] = lv->proposals[l];
-    P.topk_idx[l] = lv->topk_idx[l];
-    P.topk_scores[l] = lv->topk_scores[l];
-    P.A[l] = lv->A[l];
-    P.k[l] = lv->k[l];
-    P.t0[l] = (int)T;
-    T += lv->k[l];
-  }
-  if (T > INT_MAX) return D2B_EINVAL;
-  P.t0[P.L] = (int)T;
-  if (N > 0 && T > 0 && (!image_hw || !flat_boxes || !nms_boxes || !nms_scores || !raw_scores || !cat_ids)) return D2B_EINVAL;
-  D2B_CUDA(cudaMemsetAsync(nonfinite, 0, sizeof(int), (cudaStream_t)stream));
-  if (N == 0 || T == 0) return D2B_OK;
-  rrpn_prepare_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(P, (int)T, image_hw, min_box_size, seg_per_image, flat_boxes,
-                                                                nms_boxes, nms_scores, raw_scores, (long long*)cat_ids, nonfinite);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
+  return rpn_prepare<RotBox>(lv, N, image_hw, min_box_size, 1, seg_per_image, flat_boxes, nms_boxes, nms_scores, raw_scores,
+                             cat_ids, nonfinite, stream);
 }
 
 D2B_API int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,

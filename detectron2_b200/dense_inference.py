@@ -25,6 +25,7 @@ from typing import List, Sequence, Tuple
 import torch
 
 from . import ops
+from ._batched_select import first_k_per_image, nms_select
 from .fast_rcnn_inference import Detections
 
 __all__ = ["apply_deltas", "dense_detector_inference", "retinanet_inference"]
@@ -103,21 +104,13 @@ def dense_detector_inference_fixed(anchors: List[torch.Tensor], pred_scores: Lis
     flat_boxes, nms_boxes = torch.empty((m, 4), **f32), torch.empty((m, 4), **f32)
     nms_scores, raw_scores = torch.empty((m,), **f32), torch.empty((m,), **f32)
     classes, cat_ids = torch.empty((m,), **i64), torch.empty((m,), **i64)
-    out_boxes = torch.zeros((n, topk, 4), **f32)
-    out_scores = torch.zeros((n, topk), **f32)
-    out_index = torch.zeros((n, topk), **i64)
-    counts = torch.zeros((n,), **i64)
     w = (C.c_float * 4)(*[float(x) for x in box2box_weights])
     with torch.cuda.device(device):
         check(_C.lib().d2b_dense_prepare(C.byref(lv), n, ncls, w, float(scale_clamp), ptr(flat_boxes), ptr(nms_boxes),
                                          ptr(nms_scores), ptr(raw_scores), ptr(classes), ptr(cat_ids), stream_ptr(device)),
               "dense_prepare")
-        if m and topk:
-            keep, num_keep = ops.nms_fixed(nms_boxes, nms_scores, cat_ids, float(nms_thresh), False, apply_offsets=False,
-                                           max_segment=max(t, 1))
-            check(_C.lib().d2b_rpn_select(ptr(keep), ptr(num_keep), n, t, topk, ptr(flat_boxes), ptr(raw_scores), ptr(cat_ids),
-                                          ptr(out_boxes), ptr(out_scores), ptr(out_index), ptr(counts), stream_ptr(device)),
-                  "det_select")
+    out_boxes, out_scores, out_index, counts = nms_select(nms_boxes, nms_scores, cat_ids, flat_boxes, raw_scores, n, t, topk,
+                                                          nms_thresh, False, max(t, 1))
     out_classes = classes[out_index.reshape(-1)].reshape(n, topk) if m else out_index
     del keepalive
     return out_boxes, out_scores, out_classes, counts
@@ -195,21 +188,9 @@ def _dense_detector_inference_host(anchors: List[torch.Tensor], pred_scores: Lis
                                    max_segment=max(t, 1))
 
     # 5. per-image first max_detections_per_image of the score-ordered keep list (:308), on the device
-    m = keep.shape[0]
-    topk = int(max_detections_per_image) if max_detections_per_image >= 0 else m
-    pos = torch.arange(m, device=device)
-    in_list = pos < num_keep
-    kidx = torch.where(in_list, keep, torch.zeros_like(keep))
-    kok = in_list & live.reshape(-1)[kidx]
-    kimg = torch.div(kidx, max(t, 1), rounding_mode="floor")
-    onehot = (kimg[None, :] == batch_idx[:, None]) & kok[None, :]               # N x M
-    rank = torch.cumsum(onehot.to(torch.int32), dim=1) - 1
-    sel = onehot & (rank < topk)
-    counts = sel.sum(dim=1)
-    out_idx = torch.zeros((num_images, topk + 1), dtype=torch.int64, device=device)
-    col = torch.where(sel, rank.long(), torch.full_like(rank, topk, dtype=torch.int64))
-    out_idx.scatter_(1, col, kidx[None, :].expand(num_images, m))                # unselected entries land in a trash column
-    out_idx = out_idx[:, :topk]
+    topk = int(max_detections_per_image) if max_detections_per_image >= 0 else keep.shape[0]
+    img_of = batch_idx[:, None].expand(n, t).reshape(-1)
+    out_idx, counts = first_k_per_image(keep, num_keep, img_of, live.reshape(-1), num_images, topk)
     flat_boxes, flat_scores, flat_cls = boxes.reshape(-1, 4), scores.reshape(-1), classes.reshape(-1)
 
     counts_host = counts.tolist()  # the one host sync: the reference contract returns exactly-sized results

@@ -3,21 +3,23 @@ detectron2/modeling/proposal_generator/rrpn.py:20-127.
 
 The reference loops over images in Python: per image it filters non-finite boxes with boolean indexing, clips the rotated
 boxes (`RotatedBoxes.clip`, whose `torch.where(...)[0]` is a host sync), drops empty boxes after a `.item()` (:110) and runs
-one `batched_nms_rotated`.  Here all images go through ONE rotated NMS, as in `proposal_utils.find_top_rpn_proposals`:
+one `batched_nms_rotated`.  Here all images go through ONE rotated NMS: the functions below are
+`proposal_utils.find_top_rpn_proposals[_fixed]` with `rotated=True`:
 
   * `d2b_rrpn_prepare` (one CTA per image) gathers the per-level top-k, normalises the angles and clips, and moves removed
     boxes (non-finite, or not larger than `min_box_size` after clipping) to the ignored category -1 instead of removing them;
     it adds batched_nms_rotated's offsets -- level * (max - min + 1) over THAT image's surviving boxes, fp32 -- to the centres;
-  * one `d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET)` with category image * L + level;
+  * one `d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET)` with category image * L + level (image alone for a threshold <= 0,
+    which IoU 0 passes: the reference's one NMS per image then suppresses across levels too);
   * `d2b_rpn_select_rotated` hands every image the first `post_nms_topk` survivors of the score-ordered keep list.
-The only host synchronisation is the final read of the N output lengths.
+The only host synchronisation is the final read of the N output lengths.  `clip_rotated` and `rotated_offset_scale` are
+the torch-op forms of the clip and the offsets that the host restatements use.
 """
 from typing import List, Tuple
 
 import torch
 
-from . import ops
-from .proposal_utils import ProposalBoxes, Proposals
+from .proposal_utils import _find_top_rpn_proposals_host, find_top_rpn_proposals, find_top_rpn_proposals_fixed
 
 __all__ = ["find_top_rrpn_proposals", "find_top_rrpn_proposals_fixed", "clip_rotated"]
 
@@ -54,58 +56,8 @@ def find_top_rrpn_proposals_fixed(proposals: List[torch.Tensor], pred_objectness
     [N, post_nms_topk], counts [N] int64, nonfinite [1] int32) -- rows beyond counts[i] are zero.  `image_sizes` is a list
     of (h, w) or an [N, 2] CUDA tensor.  The launch sequence (torch.topk per level, d2b_rrpn_prepare, d2b_nms,
     d2b_rpn_select_rotated) has static shapes: it can be captured in a CUDA graph."""
-    import ctypes as C
-
-    from . import _C
-    from ._C import check, ptr, stream_ptr
-
-    n = len(image_sizes)
-    device = proposals[0].device
-    _C.require_cuda(*proposals, *pred_objectness_logits)
-    L = len(proposals)
-    if L > _C.MAX_LEVELS:
-        raise RuntimeError("find_top_rrpn_proposals: at most %d feature levels" % _C.MAX_LEVELS)
-    lv = _C.RpnLevels()
-    lv.num_levels = L
-    keepalive = []
-    t = 0
-    for l, (p_l, s_l) in enumerate(zip(proposals, pred_objectness_logits)):
-        k = min(s_l.shape[1], pre_nms_topk)
-        top_s, top_i = s_l.float().topk(k, dim=1)  # rrpn.py:76 (library top-k, one call per level)
-        p_c = p_l.float().contiguous()
-        keepalive += [top_s, top_i, p_c]
-        lv.proposals[l], lv.topk_idx[l], lv.topk_scores[l] = p_c.data_ptr(), top_i.data_ptr(), top_s.data_ptr()
-        lv.A[l], lv.k[l] = p_c.shape[1], k
-        t += k
-    if isinstance(image_sizes, torch.Tensor):
-        hw = image_sizes.to(device=device, dtype=torch.float32).contiguous()
-    else:
-        hw = torch.tensor([[float(h), float(w)] for (h, w) in image_sizes], dtype=torch.float32).to(device)
-    m = n * t
-    f32 = dict(dtype=torch.float32, device=device)
-    flat_boxes, nms_boxes = torch.empty((m, 5), **f32), torch.empty((m, 5), **f32)
-    nms_scores, raw_scores = torch.empty((m,), **f32), torch.empty((m,), **f32)
-    cat_ids = torch.empty((m,), dtype=torch.int64, device=device)
-    nonfinite = torch.empty((1,), dtype=torch.int32, device=device)
-    out_boxes = torch.empty((n, post_nms_topk, 5), **f32)
-    out_scores = torch.empty((n, post_nms_topk), **f32)
-    out_index = torch.empty((n, post_nms_topk), dtype=torch.int64, device=device)
-    counts = torch.zeros((n,), dtype=torch.int64, device=device)
-    # IoU 0 passes a threshold <= 0: the reference's one NMS per image then suppresses across levels as well
-    per_image = float(nms_thresh) <= 0.0
-    with torch.cuda.device(device):
-        check(_C.lib().d2b_rrpn_prepare(C.byref(lv), n, ptr(hw), float(min_box_size), int(per_image), ptr(flat_boxes),
-                                        ptr(nms_boxes), ptr(nms_scores), ptr(raw_scores), ptr(cat_ids), ptr(nonfinite),
-                                        stream_ptr(device)), "rrpn_prepare")
-        if m:
-            max_segment = t if per_image else max(int(lv.k[l]) for l in range(L))
-            keep, num_keep = ops.nms_fixed(nms_boxes, nms_scores, cat_ids, float(nms_thresh), True, apply_offsets=False,
-                                           max_segment=max_segment)
-            check(_C.lib().d2b_rpn_select_rotated(ptr(keep), ptr(num_keep), n, t, int(post_nms_topk), ptr(flat_boxes),
-                                                  ptr(raw_scores), ptr(cat_ids), ptr(out_boxes), ptr(out_scores),
-                                                  ptr(out_index), ptr(counts), stream_ptr(device)), "rrpn_select")
-    del keepalive
-    return out_boxes, out_scores, counts, nonfinite
+    return find_top_rpn_proposals_fixed(proposals, pred_objectness_logits, image_sizes, nms_thresh, pre_nms_topk,
+                                        post_nms_topk, min_box_size, rotated=True)
 
 
 def find_top_rrpn_proposals(proposals: List[torch.Tensor], pred_objectness_logits: List[torch.Tensor],
@@ -113,81 +65,13 @@ def find_top_rrpn_proposals(proposals: List[torch.Tensor], pred_objectness_logit
                             min_box_size: float, training: bool):
     """proposals[l]: [N, Hi*Wi*A, 5] rotated boxes, pred_objectness_logits[l]: [N, Hi*Wi*A].  Returns N `Proposals` with
     [k, 5] `proposal_boxes.tensor` and [k] `objectness_logits`, exactly like the reference."""
-    if proposals[0].is_cuda:  # fused, fixed-capacity kernels + ONE host read of the output lengths
-        out_boxes, out_scores, counts, nonfinite = find_top_rrpn_proposals_fixed(
-            proposals, pred_objectness_logits, image_sizes, nms_thresh, pre_nms_topk, post_nms_topk, min_box_size)
-        host = torch.cat([counts, nonfinite.to(torch.int64)]).tolist()  # the one host sync: exactly-sized results
-        if training and host[-1]:  # same failure mode as the reference (:98-102); training only
-            raise FloatingPointError("Predicted boxes or scores contain Inf/NaN. Training has diverged.")
-        dt = pred_objectness_logits[0].dtype
-        return [Proposals(sz, ProposalBoxes(out_boxes[i, :host[i]]), out_scores[i, :host[i]].to(dt))
-                for i, sz in enumerate(image_sizes)]
-    return _find_top_rrpn_proposals_host(proposals, pred_objectness_logits, image_sizes, nms_thresh, pre_nms_topk,
-                                         post_nms_topk, min_box_size, training)
+    return find_top_rpn_proposals(proposals, pred_objectness_logits, image_sizes, nms_thresh, pre_nms_topk, post_nms_topk,
+                                  min_box_size, training, rotated=True)
 
 
 def _find_top_rrpn_proposals_host(proposals, pred_objectness_logits, image_sizes, nms_thresh, pre_nms_topk, post_nms_topk,
                                   min_box_size, training):
-    """The same selection written with torch ops (the host-logic restatement that tests/test_rotated_inference_host.py pins
-    to the real reference function with the NMS call replaced by the oracle; the CUDA path above is the product)."""
-    num_images = len(image_sizes)
-    device = proposals[0].device
-    num_levels = len(proposals)
-    # 1. top-k per level and image (rrpn.py:62-88)
-    batch_idx = torch.arange(num_images, device=device)
-    boxes_l, scores_l, level_l = [], [], []
-    for level_id, (proposals_i, logits_i) in enumerate(zip(proposals, pred_objectness_logits)):
-        k = min(logits_i.shape[1], pre_nms_topk)
-        topk_scores_i, topk_idx = logits_i.topk(k, dim=1)
-        boxes_l.append(proposals_i[batch_idx[:, None], topk_idx])
-        scores_l.append(topk_scores_i)
-        level_l.append(torch.full((k,), level_id, dtype=torch.int64, device=device))
-    boxes = torch.cat(boxes_l, dim=1).float()   # N x T x 5
-    scores = torch.cat(scores_l, dim=1)         # N x T
-    levels = torch.cat(level_l, dim=0)          # T
-    n, t = scores.shape
-
-    # 2. validity, clip, empty-box filter -- as masks, not as shape changes (:97-111)
-    finite = torch.isfinite(boxes).all(dim=2) & torch.isfinite(scores)
-    if training and not bool(finite.all()):  # same failure mode as the reference (:98-102); training only
-        raise FloatingPointError("Predicted boxes or scores contain Inf/NaN. Training has diverged.")
-    hw = torch.tensor([[float(h), float(w)] for (h, w) in image_sizes], device=device)  # N x 2
-    clipped = clip_rotated(boxes, hw[:, 0:1], hw[:, 1:2])
-    valid = finite & (clipped[..., 2] > min_box_size) & (clipped[..., 3] > min_box_size)
-
-    # 3. one rotated NMS over all images: category = image * L + level (image alone for a threshold IoU 0 passes),
-    #    removed boxes get category -1; centres carry batched_nms_rotated's per-image offsets
-    per_image = float(nms_thresh) <= 0.0
-    img_of = batch_idx[:, None].expand(n, t)
-    cat_ids = img_of if per_image else img_of * num_levels + levels[None, :]
-    cat_ids = torch.where(valid, cat_ids, torch.full_like(cat_ids, -1)).reshape(-1)
-    max_segment = t if per_image else max(x.shape[1] for x in scores_l)
-    zeros = torch.zeros_like(clipped)
-    flat_boxes = torch.where(valid[..., None], clipped, zeros).reshape(-1, 5)
-    flat_scores = torch.where(valid, scores.float(), torch.full_like(scores, float("-inf"), dtype=torch.float32)).reshape(-1)
-    offs = levels[None, :].to(torch.float32) * rotated_offset_scale(clipped, valid)[:, None]  # N x T
-    nms_boxes = torch.cat([clipped[..., :2] + offs[..., None], clipped[..., 2:]], dim=2)
-    nms_boxes = torch.where(valid[..., None], nms_boxes, zeros).reshape(-1, 5)
-    keep, num_keep = ops.nms_fixed(nms_boxes, flat_scores, cat_ids, float(nms_thresh), True, apply_offsets=False,
-                                   max_segment=max_segment)
-
-    # 4. per-image top post_nms_topk of the score-ordered keep list (:121)
-    m = keep.shape[0]
-    live = torch.arange(m, device=device) < num_keep          # keep[] beyond num_keep is padding
-    kidx = torch.where(live, keep, torch.zeros_like(keep))
-    kimg = torch.div(kidx, t, rounding_mode="floor")
-    kvalid = live & valid.reshape(-1)[kidx]
-    onehot = (kimg[None, :] == batch_idx[:, None]) & kvalid[None, :]          # N x M
-    rank = torch.cumsum(onehot.to(torch.int32), dim=1) - 1
-    sel = onehot & (rank < post_nms_topk)
-    counts = sel.sum(dim=1)
-    out_idx = torch.zeros((num_images, post_nms_topk + 1), dtype=torch.int64, device=device)
-    col = torch.where(sel, rank.long(), torch.full_like(rank, post_nms_topk, dtype=torch.int64))
-    out_idx.scatter_(1, col, kidx[None, :].expand(n, m))
-    out_idx = out_idx[:, :post_nms_topk].contiguous()
-    out_boxes = flat_boxes[out_idx.reshape(-1)].reshape(num_images, post_nms_topk, 5)
-    out_scores = scores.reshape(-1)[out_idx.reshape(-1)].reshape(num_images, post_nms_topk)
-
-    counts_host = counts.tolist()  # the one host sync: the reference contract returns exactly-sized results
-    return [Proposals(image_size, ProposalBoxes(out_boxes[i, :counts_host[i]]), out_scores[i, :counts_host[i]])
-            for i, image_size in enumerate(image_sizes)]
+    """The torch-op restatement of the same selection (also for CUDA tensors, with the GPU NMS): the kernels are tested
+    against it."""
+    return _find_top_rpn_proposals_host(proposals, pred_objectness_logits, image_sizes, nms_thresh, pre_nms_topk,
+                                        post_nms_topk, min_box_size, training, rotated=True)

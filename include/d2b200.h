@@ -208,6 +208,10 @@ int d2b_nms(const float* boxes, const float* scores, const int64_t* idxs, int64_
  *   candidates: flat_boxes (clipped to the image; zeros for removed ones), nms_boxes (+ torchvision's per-image
  *   level offsets when use_offsets), nms_scores (-inf for removed), raw_scores, cat_ids (image*L + level, or -1 = removed:
  *   non-finite or not larger than min_box_size after clipping), nonfinite[1] (1 if any candidate was non-finite).
+ *   Arguments (the same rules for d2b_rrpn_prepare, checked before the first CUDA call): 1 <= num_levels <= D2B_MAX_LEVELS,
+ *   N >= 0, nonfinite non-NULL; per level 0 <= k_l <= A_l, and the level's three pointers non-NULL when N > 0 and k_l > 0;
+ *   T <= INT_MAX; image_hw and the five output arrays non-NULL when N > 0 and T > 0.  proposals[l], flat_boxes and
+ *   nms_boxes must be 16-byte aligned (float4 access).  nonfinite is zeroed even when there is no candidate.
  * d2b_rpn_select: keep / num_keep as returned by d2b_nms over the N*T candidates; out_boxes [N,post_nms_topk,4],
  *   out_scores / out_index [N,post_nms_topk] (0-padded), counts [N] int64. */
 typedef struct {
@@ -271,8 +275,9 @@ int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const 
  * seg_per_image != 0 (pass it for iou_threshold <= 0, which IoU 0 passes: the reference's single NMS then suppresses
  * across categories too): every surviving candidate of image n gets category n instead, offsets unchanged; the NMS
  * max_segment must then bound the image's slot count.
- * d2b_rrpn_prepare: as d2b_rpn_prepare with lv->proposals[l] [N,A_l,5]; removed = non-finite or w / h not larger than
- *   min_box_size after clipping (RotatedBoxes.nonempty); flat_boxes / nms_boxes [N*T,5].
+ * d2b_rrpn_prepare: as d2b_rpn_prepare (same argument rules, no alignment requirement) with lv->proposals[l] [N,A_l,5];
+ *   removed = non-finite or w / h not larger than min_box_size after clipping (RotatedBoxes.nonempty); flat_boxes /
+ *   nms_boxes [N*T,5]; the offsets are always applied.
  * d2b_frcnn_rotated_prepare: as d2b_frcnn_prepare with boxes [Rtot, kreg*5]; cand_boxes / nms_boxes [N*cap,5].
  * d2b_rpn_select_rotated: as d2b_rpn_select with flat_boxes [N*T,5] and out_boxes [N,post_nms_topk,5].
  * All arguments are checked before the first CUDA call. */

@@ -1059,6 +1059,26 @@ def test_find_top_rpn_proposals_fixed_in_cuda_graph(golden):
     assert int(bad.item()) in (0, 1)  # the fixture contains non-finite candidates (flagged, and dropped like the reference does)
 
 
+@pytest.mark.parametrize("rotated", [False, True])
+def test_find_top_rpn_proposals_fixed_zero_rows_without_candidates(rotated):
+    # pre_nms_topk = 0 leaves no candidate (every level's top-k is empty), so the selection kernel does not run: the outputs
+    # must still be zero, not what the caching allocator hands back.  A freed NaN-filled block of the boxes' size (> 1 MB:
+    # large pool) is that block.
+    from detectron2_b200.proposal_utils import find_top_rpn_proposals_fixed
+    from detectron2_b200.rrpn import find_top_rrpn_proposals_fixed
+
+    n, post, d = 2, 50000, (5 if rotated else 4)  # [2, 50000, d] fp32 >= 1.6 MB
+    g = torch.Generator().manual_seed(4)
+    props = [(torch.rand(n, a, d, generator=g) * 50).cumsum(2).to(DEV) for a in (300, 120)]
+    logits = [torch.randn(n, a, generator=g).to(DEV) for a in (300, 120)]
+    dirty = torch.full((n, post, d), float("nan"), device=DEV)
+    del dirty
+    fixed = find_top_rrpn_proposals_fixed if rotated else find_top_rpn_proposals_fixed
+    boxes, scores, counts, _ = fixed(props, logits, [(400, 600)] * n, 0.7, 0, post, 0.0)
+    torch.cuda.synchronize()
+    assert boxes.shape == (n, post, d) and (boxes == 0).all() and (scores == 0).all() and (counts == 0).all()
+
+
 def test_find_top_rpn_proposals_fpn_size_vs_oracle():
     # BASELINE config-2 shape: 5 levels, pre-NMS top 1000 per level, 2 images; oracle = per-image reference loop on CPU
     from detectron2_b200.proposal_utils import find_top_rpn_proposals
@@ -1159,15 +1179,28 @@ def test_fast_rcnn_inference_kernels_vs_host_restatement_coco_size():
     for a, b, ra, rb in zip(res, ref, rows, ref_rows):
         assert torch.equal(a.pred_boxes, b.pred_boxes) and torch.equal(a.scores, b.scores)
         assert torch.equal(a.pred_classes, b.pred_classes) and torch.equal(ra, rb)
-    # CUDA graph of the fixed-capacity sequence
+    # CUDA graph of the fixed-capacity sequence, together with the dense-head form on RetinaNet-shaped levels
+    from detectron2_b200 import dense_inference as di
+
+    gd = torch.Generator().manual_seed(22)
+    anchors, dscores, deltas = [], [], []
+    for stride in (32, 64, 128):
+        r = math.ceil(800 / stride) * math.ceil(1333 / stride) * 9
+        ctr = torch.rand(r, 2, generator=gd) * torch.tensor([1333.0, 800.0])
+        wh = stride * (2 + 6 * torch.rand(r, 2, generator=gd))
+        anchors.append(torch.cat([ctr - wh / 2, ctr + wh / 2], 1).to(DEV))
+        dscores.append((torch.randn(2, r, k, generator=gd) * 1.2 - 3.0).sigmoid().to(DEV))
+        deltas.append((torch.randn(2, r, 4, generator=gd) * 0.2).to(DEV))
     hw = torch.tensor([[float(h), float(w)] for (h, w) in shapes], device=DEV)
     fri.fast_rcnn_inference_fixed(boxes[:3], scores[:3], hw[:3], 0.05, 0.5, 100)  # warm-up outside the capture
+    di.dense_detector_inference_fixed(anchors, dscores, deltas, 2, 0.05, 1000, 0.5, 100)
     torch.cuda.synchronize()
     graph = torch.cuda.CUDAGraph()
     st = torch.cuda.Stream()
     with torch.cuda.stream(st):
         with torch.cuda.graph(graph, stream=st):
             out = fri.fast_rcnn_inference_fixed(boxes[:3], scores[:3], hw[:3], 0.05, 0.5, 100)
+            dout = di.dense_detector_inference_fixed(anchors, dscores, deltas, 2, 0.05, 1000, 0.5, 100)
     graph.replay()
     torch.cuda.synchronize()
     res, rows = fri.fast_rcnn_inference(boxes[:3], scores[:3], shapes[:3], 0.05, 0.5, 100)
@@ -1176,6 +1209,13 @@ def test_fast_rcnn_inference_kernels_vs_host_restatement_coco_size():
         assert c == len(res[i])
         assert torch.equal(out["boxes"][i, :c], res[i].pred_boxes) and torch.equal(out["classes"][i, :c], res[i].pred_classes)
         assert torch.equal(out["rows"][i, :c], rows[i])
+    dres = di.dense_detector_inference(anchors, dscores, deltas, shapes[:2], 0.05, 1000, 0.5, 100)
+    ob, osc, ocl, cnt = dout
+    for i in range(2):
+        c = int(cnt[i])
+        assert c == len(dres[i]) > 0 and (ob[i, c:] == 0).all()
+        assert torch.equal(ob[i, :c], dres[i].pred_boxes) and torch.equal(osc[i, :c], dres[i].scores)
+        assert torch.equal(ocl[i, :c], dres[i].pred_classes)
 
 
 # ------------------------------------------------------------------------------- batched RetinaNet inference (8f-2)

@@ -163,31 +163,45 @@ def _lib():
     return _C, _C.lib()
 
 
-def test_rotated_entry_points_reject_bad_arguments():
-    """Every argument is checked before the first CUDA call: these return D2B_EINVAL without a GPU."""
+def _check_rpn_prepare_rejects_bad_arguments(prepare):
+    """The argument checks that d2b_rpn_prepare and d2b_rrpn_prepare share: D2B_EINVAL before the first CUDA call."""
     _C, lib = _lib()
     EINVAL = -1
+    fn = getattr(lib, prepare)
     p = C.c_void_p(16)  # never dereferenced: the checks fail first
     lv = _C.RpnLevels()
     lv.num_levels = 1
     lv.proposals[0], lv.topk_idx[0], lv.topk_scores[0] = 16, 16, 16
     lv.A[0], lv.k[0] = 10, 5
     args = lambda lv_, n=2, nf=p: (C.byref(lv_), n, p, 0.0, 0, p, p, p, p, p, nf, None)  # noqa: E731
-    assert lib.d2b_rrpn_prepare(None, 2, p, 0.0, 0, p, p, p, p, p, p, None) == EINVAL
-    assert lib.d2b_rrpn_prepare(*args(lv, nf=None)) == EINVAL
-    assert lib.d2b_rrpn_prepare(*args(lv, n=-1)) == EINVAL
+    assert fn(None, 2, p, 0.0, 0, p, p, p, p, p, p, None) == EINVAL
+    assert fn(*args(lv, nf=None)) == EINVAL
+    assert fn(*args(lv, n=-1)) == EINVAL
     for field, value in (("num_levels", 0), ("num_levels", 9)):
         bad = _C.RpnLevels.from_buffer_copy(lv)
         setattr(bad, field, value)
-        assert lib.d2b_rrpn_prepare(*args(bad)) == EINVAL, (field, value)
+        assert fn(*args(bad)) == EINVAL, (field, value)
     bad = _C.RpnLevels.from_buffer_copy(lv)
     bad.k[0] = 11  # k > A
-    assert lib.d2b_rrpn_prepare(*args(bad)) == EINVAL
+    assert fn(*args(bad)) == EINVAL
     bad = _C.RpnLevels.from_buffer_copy(lv)
     bad.topk_idx[0] = None
-    assert lib.d2b_rrpn_prepare(*args(bad)) == EINVAL
-    assert lib.d2b_rrpn_prepare(C.byref(lv), 2, None, 0.0, 0, p, p, p, p, p, p, None) == EINVAL
-    assert lib.d2b_rrpn_prepare(C.byref(lv), 2, p, 0.0, 0, p, None, p, p, p, p, None) == EINVAL
+    assert fn(*args(bad)) == EINVAL
+    assert fn(C.byref(lv), 2, None, 0.0, 0, p, p, p, p, p, p, None) == EINVAL
+    assert fn(C.byref(lv), 2, p, 0.0, 0, p, None, p, p, p, p, None) == EINVAL
+
+
+def test_rpn_prepare_rejects_bad_arguments():
+    """d2b_rpn_prepare checks its arguments by the same rules as d2b_rrpn_prepare (one shared host check)."""
+    _check_rpn_prepare_rejects_bad_arguments("d2b_rpn_prepare")
+
+
+def test_rotated_entry_points_reject_bad_arguments():
+    """Every argument is checked before the first CUDA call: these return D2B_EINVAL without a GPU."""
+    _check_rpn_prepare_rejects_bad_arguments("d2b_rrpn_prepare")
+    _C, lib = _lib()
+    EINVAL = -1
+    p = C.c_void_p(16)  # never dereferenced: the checks fail first
 
     rs = (C.c_int * 3)(0, 4, 9)
     good = [p, p, rs, 2, 3, 3, p, 0.05, 16, 0, p, p, p, p, p, p, p, p, None]
