@@ -92,6 +92,10 @@ def _declare(lib):
         "d2b_rpn_select_rotated": (i, [i64p, i64p, i, i, i, f32p, f32p, i64p, f32p, f32p, i64p, i64p, vp]),
         "d2b_mask_loss_forward": (i, [f32p, i, i, i, u8p, i, i, i, f32p, i64p, i64p, f32p, u8p, vp]),
         "d2b_mask_loss_backward": (i, [f32p, i, i, i, u8p, i64p, f32p, f32p, vp]),
+        "d2b_keypoints_workspace_bytes": (sz, [i, i]),
+        "d2b_keypoints_from_heatmaps": (i, [f32p, i, i, i, f32p, f32p, vp, sz, vp]),
+        "d2b_keypoint_loss_forward": (i, [vp, i, i, i, i, f32p, f32p, i64p, u8p, f32p, i64p, vp]),
+        "d2b_keypoint_loss_backward": (i, [vp, i, i, i, i, i64p, u8p, f32p, vp, vp]),
         "d2b_box_iou_rotated": (i, [f32p, i64, f32p, i64, f32p, vp]),
         "d2b_match_workspace_bytes": (sz, [i, i, i]),
         "d2b_match_boxes": (i, [f32p, i64p, i, i, f32p, i64, i64p, i, C.POINTER(C.c_double), i, C.POINTER(C.c_int), i, f32p, d,

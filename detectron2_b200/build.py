@@ -25,6 +25,7 @@ SOURCES = {
     "nms.cu": ["-fmad=false"],
     "postproc.cu": ["-fmad=false"],
     "match.cu": ["-fmad=false"],
+    "keypoints.cu": ["-fmad=false"],
     "deform_conv.cu": [],
     "deform_conv_tc.cu": [],
 }

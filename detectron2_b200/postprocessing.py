@@ -30,20 +30,24 @@ def crop_and_resize(bit_masks: torch.Tensor, boxes: torch.Tensor, mask_size: int
 
 
 class PostprocessedDetections(Detections):
-    """`Detections` plus the optional full-resolution masks `detector_postprocess` produces."""
+    """`Detections` plus the optional full-resolution masks and rescaled keypoints `detector_postprocess` produces."""
 
-    def __init__(self, image_size, pred_boxes, scores, pred_classes, pred_masks: Optional[torch.Tensor] = None):
+    def __init__(self, image_size, pred_boxes, scores, pred_classes, pred_masks: Optional[torch.Tensor] = None,
+                 pred_keypoints: Optional[torch.Tensor] = None):
         super().__init__(image_size, pred_boxes, scores, pred_classes)
         self.pred_masks = pred_masks
+        self.pred_keypoints = pred_keypoints
 
 
 def detector_postprocess(results: Detections, output_height: int, output_width: int, mask_threshold: float = 0.5,
-                         pred_masks: Optional[torch.Tensor] = None) -> PostprocessedDetections:
+                         pred_masks: Optional[torch.Tensor] = None,
+                         pred_keypoints: Optional[torch.Tensor] = None) -> PostprocessedDetections:
     """results: detections at the resolution the detector saw (`results.image_size`); pred_masks: optional
-    (N, 1, M, M) or (N, M, M) soft masks of the mask head.  Returns the detections at (output_height, output_width):
+    (N, 1, M, M) or (N, M, M) soft masks of the mask head; pred_keypoints: optional (N, K, 3) keypoints (x, y, score) of the
+    keypoint head.  Returns the detections at (output_height, output_width):
     boxes scaled (Boxes.scale, boxes.py:271-276), clipped (Boxes.clip, :183-197), empty boxes removed
-    (Boxes.nonempty, :199-213; the one data-dependent shape, as in the reference) and masks pasted
-    (ROIMasks.to_bitmasks -> paste_masks_in_image, masks.py:522-539)."""
+    (Boxes.nonempty, :199-213; the one data-dependent shape, as in the reference), masks pasted
+    (ROIMasks.to_bitmasks -> paste_masks_in_image, masks.py:522-539) and keypoint x / y scaled (postprocessing.py:70-72)."""
     scale_x, scale_y = output_width / results.image_size[1], output_height / results.image_size[0]
     boxes = results.pred_boxes.clone()
     boxes[:, 0::2] *= scale_x
@@ -60,5 +64,10 @@ def detector_postprocess(results: Detections, output_height: int, output_width: 
     if pred_masks is not None:
         soft = pred_masks[:, 0, :, :] if pred_masks.dim() == 4 else pred_masks
         masks = paste_masks_in_image(soft[keep], boxes, (output_height, output_width), threshold=mask_threshold)
+    keypoints = None
+    if pred_keypoints is not None:
+        keypoints = pred_keypoints[keep]
+        keypoints[:, :, 0] *= scale_x
+        keypoints[:, :, 1] *= scale_y
     return PostprocessedDetections((output_height, output_width), boxes, results.scores[keep], results.pred_classes[keep],
-                                   masks)
+                                   masks, keypoints)

@@ -341,6 +341,44 @@ int d2b_mask_loss_forward(const float* logits, int K, int C, int S, const uint8_
 int d2b_mask_loss_backward(const float* logits, int K, int C, int S, const uint8_t* targets, const int64_t* classes,
                            const float* grad_scale, float* grad_logits, void* stream);
 
+/* ---- Keypoint head: heatmap decoding (inference) ----------------------------------------------------------------
+ * Replaces the per-detection loop of heatmaps_to_keypoints (detectron2/structures/keypoints.py:164-235), reached from
+ * keypoint_rcnn_inference (modeling/roi_heads/keypoint_head.py:99-132).
+ *   maps [R,K,S,S] fp32 logits, rois [R,4] xyxy fp32 -> out [R,K,4] fp32 (x, y, logit, score), 16-byte aligned.
+ * Per ROI: w = max(x2 - x1, 1), h = max(y2 - y1, 1), Wo = ceil(w), Ho = ceil(h); the (Ho, Wo) bicubic resize of each map with
+ * PyTorch's CUDA upsample_bicubic2d arithmetic (align_corners = False, A = -0.75, source indices clamped to [0, S-1]) is
+ * evaluated on the fly, never stored.  x = (x_int + 0.5) * (w / Wo) + x1, y likewise, logit = the resized map at the argmax,
+ * score = 1 / sum_{S x S} exp(maps - logit).
+ * Argmax rule (torch.argmax / max on CUDA): ties go to the smallest linear index y * Wo + x; a NaN beats every number and the
+ * first NaN wins (logit NaN); -0.0 and +0.0 are equal.
+ * A ROI with a non-finite coordinate difference, or more than 2^32 output pixels, gets a NaN row (the reference raises
+ * in int(); the condition is detected on the device, without a host synchronisation).
+ * 1 <= S <= D2B_KEYPOINTS_MAX_S (the map is staged in shared memory), K >= 1.  workspace: d2b_keypoints_workspace_bytes(R, K)
+ * bytes, 8-byte aligned, no initialisation needed.  Three launches, no host synchronisation: capturable in a CUDA graph. */
+#define D2B_KEYPOINTS_MAX_S 241
+size_t d2b_keypoints_workspace_bytes(int R, int K);
+int d2b_keypoints_from_heatmaps(const float* maps, int R, int K, int S, const float* rois, float* out, void* workspace,
+                                size_t workspace_bytes, void* stream);
+
+/* ---- Keypoint head: training targets + loss --------------------------------------------------------------------
+ * Replaces keypoint_rcnn_loss (modeling/roi_heads/keypoint_head.py:40-96): the per-image Keypoints.to_heatmap
+ * (_keypoints_to_heatmap, structures/keypoints.py:105-161), the nonzero() host sync, the gather of the valid logit rows and
+ * F.cross_entropy, for all images of the batch in one launch.
+ *   logits [N,K,S,S] of `dtype` (D2B_F32 / D2B_F16 / D2B_BF16, read in place, fp32 arithmetic); keypoints [N,K,3] fp32
+ *   (x, y, v) matched ground truth of every proposal; boxes [N,4] fp32 proposal boxes.
+ *   target [N,K] int64 = y * S + x of the keypoint's heatmap cell, 0 when not valid; valid [N,K] uint8: the cell is inside
+ *   the S x S map and v > 0.  Cell: floor((c - x1) * (S / (x2 - x1))) with S / t evaluated as reciprocal(t) * S, each
+ *   operation rounded on its own; c == x2 gives S - 1 (y likewise).
+ *   loss_per_kp [N,K] fp32: logsumexp(row) - row[target] on valid rows, 0 elsewhere; num_valid [1] int64 (zeroed inside).
+ *   logits and loss_per_kp may both be NULL: the targets alone (Keypoints.to_heatmap).
+ * Backward: grad_scale [N,K] fp32 = d loss / d loss_per_kp; grad_logits [N,K,S,S] of `dtype`, fully written:
+ * (softmax(row) - onehot(target)) * grad_scale on valid rows, 0 elsewhere. */
+int d2b_keypoint_loss_forward(const void* logits, int dtype, int N, int K, int S, const float* keypoints,
+                              const float* boxes, int64_t* target, uint8_t* valid, float* loss_per_kp, int64_t* num_valid,
+                              void* stream);
+int d2b_keypoint_loss_backward(const void* logits, int dtype, int N, int K, int S, const int64_t* target,
+                               const uint8_t* valid, const float* grad_scale, void* grad_logits, void* stream);
+
 /* ---- Rotated-box IoU --------------------------------------------------------------------
  * Replaces torch.ops.detectron2.box_iou_rotated (csrc/vision.cpp:117,
  * csrc/box_iou_rotated/box_iou_rotated.h:20-33).  boxes1 [N,5], boxes2 [M,5] fp32 -> ious [N,M] fp32. */
