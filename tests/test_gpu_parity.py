@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from oracle import oracle as orc
+from test_oracle_pins import deform_golden_cases
 
 pytestmark = pytest.mark.gpu
 T = torch.from_numpy
@@ -393,26 +394,26 @@ def _dcn_run(L, x, off, mask, wt, bias, s, p, dil, grp, dg):
 
 
 def test_deform_conv_golden(L, golden):
-    d = golden("deform_conv")
-    for i, (n, cin, h, w, cout, k, s, p, dil, grp, dg, mod, hb) in enumerate(d["cases"]):
+    # the fixtures' channel counts are below 64 per group: the FFMA kernels
+    for tag, d, i, s, p, dil, grp, dg, mod, hb in deform_golden_cases(golden):
         x = T(d[f"x{i}"]).to(DEV).requires_grad_(True)
         off = T(d[f"off{i}"]).to(DEV).requires_grad_(True)
         wt = T(d[f"w{i}"]).to(DEV).requires_grad_(True)
         mask = T(d[f"mask{i}"]).to(DEV).requires_grad_(True) if mod else None
         bias = T(d[f"bias{i}"]).to(DEV).requires_grad_(True) if hb else None
-        y = _dcn_run(L, x, off, mask, wt, bias, int(s), int(p), int(dil), int(grp), int(dg))
+        y = _dcn_run(L, x, off, mask, wt, bias, s, p, dil, grp, dg)
         ok, err = rel_close(y, T(d[f"y{i}"]), atol=1e-4)
-        assert ok, (i, err)
+        assert ok, (tag, err)
         y.backward(T(d[f"go{i}"]).to(DEV))
         for name, t in (("gx", x), ("goff", off), ("gw", wt)):
             ok, err = rel_close(t.grad, T(d[f"{name}{i}"]), atol=2e-4)
-            assert ok, (i, name, err)
+            assert ok, (tag, name, err)
         if mod:
             ok, err = rel_close(mask.grad, T(d[f"gmask{i}"]), atol=2e-4)
-            assert ok, (i, "gmask", err)
+            assert ok, (tag, "gmask", err)
         if hb:
             ok, err = rel_close(bias.grad, T(d[f"gbias{i}"]), atol=2e-4)
-            assert ok, (i, "gbias", err)
+            assert ok, (tag, "gbias", err)
 
 
 def test_deform_conv_reference_kats(L):

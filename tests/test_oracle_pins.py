@@ -170,23 +170,39 @@ def test_golden_rotated_bit_exact(golden):
         assert torch.equal(orc.nms_rotated(T(d["dets"]), T(d["scores"]), float(t)), T(d[f"keep{i}"]))
 
 
+def deform_golden_cases(golden):
+    """Every case of both deform-conv fixtures: ((fixture, i) tag, fixture arrays, i, stride, padding, dilation, groups,
+    deformable_groups, modulated, bias), stride / padding / dilation as (h, w) pairs.  deform_conv.npz rows hold one kernel
+    size, stride, padding and dilation for both axes (n, cin, h, w, cout, k, s, p, dil, groups, dg, mod, bias);
+    deform_conv_geometry.npz rows hold them per axis (n, cin, h, w, cout, kh, kw, sh, sw, ph, pw, dh, dw, groups, dg, mod,
+    bias).  The kernel size is the weight's."""
+    for fixture in ("deform_conv", "deform_conv_geometry"):
+        d = golden(fixture)
+        for i, row in enumerate(d["cases"]):
+            row = [int(v) for v in row]
+            if len(row) == 13:
+                s, p, dil = [(v, v) for v in row[6:9]]
+            else:
+                s, p, dil = tuple(row[7:9]), tuple(row[9:11]), tuple(row[11:13])
+            grp, dg, mod, hb = row[-4:]
+            yield (fixture, i), d, i, s, p, dil, grp, dg, bool(mod), bool(hb)
+
+
 def test_golden_deform_conv(golden):
-    d = golden("deform_conv")
-    for i, (n, cin, h, w, cout, k, s, p, dil, grp, dg, mod, hb) in enumerate(d["cases"]):
+    for tag, d, i, s, p, dil, grp, dg, mod, hb in deform_golden_cases(golden):
         x, off, wt = T(d[f"x{i}"]), T(d[f"off{i}"]), T(d[f"w{i}"])
         mask = T(d[f"mask{i}"]) if mod else None
         bias = T(d[f"bias{i}"]) if hb else None
-        y = orc.deform_conv_forward(x, off, mask, wt, bias, int(s), int(p), int(dil), int(grp), int(dg))
-        assert torch.allclose(y, T(d[f"y{i}"]), rtol=1e-4, atol=1e-4), i
-        gx, goff, gmask, gw, gb = orc.deform_conv_backward(x, off, mask, wt, T(d[f"go{i}"]), int(s), int(p), int(dil),
-                                                           int(grp), int(dg), bool(hb))
-        assert torch.allclose(gx, T(d[f"gx{i}"]), rtol=1e-4, atol=1e-4), i
-        assert torch.allclose(goff, T(d[f"goff{i}"]), rtol=1e-4, atol=1e-4), i
-        assert torch.allclose(gw, T(d[f"gw{i}"]), rtol=1e-4, atol=1e-4), i
+        y = orc.deform_conv_forward(x, off, mask, wt, bias, s, p, dil, grp, dg)
+        assert torch.allclose(y, T(d[f"y{i}"]), rtol=1e-4, atol=1e-4), tag
+        gx, goff, gmask, gw, gb = orc.deform_conv_backward(x, off, mask, wt, T(d[f"go{i}"]), s, p, dil, grp, dg, hb)
+        assert torch.allclose(gx, T(d[f"gx{i}"]), rtol=1e-4, atol=1e-4), tag
+        assert torch.allclose(goff, T(d[f"goff{i}"]), rtol=1e-4, atol=1e-4), tag
+        assert torch.allclose(gw, T(d[f"gw{i}"]), rtol=1e-4, atol=1e-4), tag
         if mod:
-            assert torch.allclose(gmask, T(d[f"gmask{i}"]), rtol=1e-4, atol=1e-4), i
+            assert torch.allclose(gmask, T(d[f"gmask{i}"]), rtol=1e-4, atol=1e-4), tag
         if hb:
-            assert torch.allclose(gb, T(d[f"gbias{i}"]), rtol=1e-4, atol=1e-4), i
+            assert torch.allclose(gb, T(d[f"gbias{i}"]), rtol=1e-4, atol=1e-4), tag
 
 
 def test_golden_paste_masks(golden):
