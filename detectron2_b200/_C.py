@@ -49,6 +49,17 @@ class DenseLevels(C.Structure):
                 ("R", C.c_int * MAX_LEVELS), ("k", C.c_int * MAX_LEVELS)]
 
 
+LABELS_I8, LABELS_I64 = 0, 1  # D2B_LABELS_*
+LOSS_STATUS_INVALID_BOX, LOSS_STATUS_INVALID_CLASS, LOSS_STATUS_INVALID_BOX_ORDER = 1, 2, 4  # D2B_LOSS_STATUS_*
+LOSS_TYPES = {"smooth_l1": 0, "giou": 1}  # D2B_LOSS_SMOOTH_L1 / D2B_LOSS_GIOU
+
+
+class DenseLossLevels(C.Structure):
+    _fields_ = [("num_levels", C.c_int), ("logits", C.c_void_p * MAX_LEVELS), ("deltas", C.c_void_p * MAX_LEVELS),
+                ("grad_logits", C.c_void_p * MAX_LEVELS), ("grad_deltas", C.c_void_p * MAX_LEVELS),
+                ("R", C.c_int * MAX_LEVELS)]
+
+
 def _declare(lib):
     vp, f32p, i64p, u8p = C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p
     i, f, d, sz, i64 = C.c_int, C.c_float, C.c_double, C.c_size_t, C.c_int64
@@ -96,6 +107,16 @@ def _declare(lib):
         "d2b_keypoints_from_heatmaps": (i, [f32p, i, i, i, f32p, f32p, vp, sz, vp]),
         "d2b_keypoint_loss_forward": (i, [vp, i, i, i, i, f32p, f32p, i64p, u8p, f32p, i64p, vp]),
         "d2b_keypoint_loss_backward": (i, [vp, i, i, i, i, i64p, u8p, f32p, vp, vp]),
+        "d2b_dense_loss_workspace_bytes": (sz, [C.POINTER(DenseLossLevels), i, i, i]),
+        "d2b_dense_loss_forward": (i, [C.POINTER(DenseLossLevels), i, i, i, i, f32p, f32p, vp, i, f, f, f, i, f,
+                                       C.POINTER(C.c_float), f32p, f32p, i64p, i64p, vp, vp, sz, vp]),
+        "d2b_dense_loss_backward": (i, [C.POINTER(DenseLossLevels), i, i, i, i, f32p, f32p, vp, i, f, f, f, i, f,
+                                        C.POINTER(C.c_float), f32p, f32p, vp]),
+        "d2b_frcnn_loss_workspace_bytes": (sz, [i]),
+        "d2b_frcnn_loss_forward": (i, [vp, vp, i, i, i, i, i, f32p, f32p, i64p, f, i, f, C.POINTER(C.c_float), f32p, f32p, i64p,
+                                       i64p, i64p, i64p, vp, vp, sz, vp]),
+        "d2b_frcnn_loss_backward": (i, [vp, vp, i, i, i, i, i, f32p, f32p, i64p, f, i, f, C.POINTER(C.c_float), f32p, f32p, vp,
+                                        vp, vp]),
         "d2b_box_iou_rotated": (i, [f32p, i64, f32p, i64, f32p, vp]),
         "d2b_match_workspace_bytes": (sz, [i, i, i]),
         "d2b_match_boxes": (i, [f32p, i64p, i, i, f32p, i64, i64p, i, C.POINTER(C.c_double), i, C.POINTER(C.c_int), i, f32p, d,

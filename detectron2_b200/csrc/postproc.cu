@@ -20,6 +20,7 @@
 #include <climits>
 #include <type_traits>
 
+#include "box_decode.cuh"
 #include "common.cuh"
 
 namespace {
@@ -443,16 +444,8 @@ __global__ void __launch_bounds__(kThreads) dense_prepare_kernel(const DenseLeve
     const long long cls = f - a * K;
     const float4 an = *reinterpret_cast<const float4*>(P.anchors[l] + (size_t)a * 4);
     const float4 d = *reinterpret_cast<const float4*>(P.deltas[l] + ((size_t)n * P.R[l] + a) * 4);
-    // Box2BoxTransform.apply_deltas, op for op (this file is compiled with -fmad=false)
-    const float widths = an.z - an.x, heights = an.w - an.y;
-    const float ctr_x = an.x + 0.5f * widths, ctr_y = an.y + 0.5f * heights;
-    const float dx = d.x / wx, dy = d.y / wy;
-    float dw = d.z / ww, dh = d.w / wh;
-    dw = dw > scale_clamp ? scale_clamp : dw;  // torch.clamp(max=): NaN stays NaN
-    dh = dh > scale_clamp ? scale_clamp : dh;
-    const float pcx = dx * widths + ctr_x, pcy = dy * heights + ctr_y;
-    const float pw = expf(dw) * widths, ph = expf(dh) * heights;
-    const float x1 = pcx - 0.5f * pw, y1 = pcy - 0.5f * ph, x2 = pcx + 0.5f * pw, y2 = pcy + 0.5f * ph;
+    const DecodedBox db = apply_deltas(an, d, wx, wy, ww, wh, scale_clamp);
+    const float x1 = db.x1, y1 = db.y1, x2 = db.x2, y2 = db.y2;
     const size_t o = (size_t)n * T + t;
     *reinterpret_cast<float4*>(flat_boxes + o * 4) = make_float4(x1, y1, x2, y2);
     raw_scores[o] = s;

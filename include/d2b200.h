@@ -379,6 +379,73 @@ int d2b_keypoint_loss_forward(const void* logits, int dtype, int N, int K, int S
 int d2b_keypoint_loss_backward(const void* logits, int dtype, int N, int K, int S, const int64_t* target,
                                const uint8_t* valid, const float* grad_scale, void* grad_logits, void* stream);
 
+/* ---- Box-branch training losses: RPN / RRPN, RetinaNet, Fast R-CNN ------------------------------------------------
+ * Replace RPN.losses (proposal_generator/rpn.py:366-429), RetinaNet.losses (meta_arch/retinanet.py:160-210) and
+ * FastRCNNOutputLayers.losses / box_reg_loss / _log_classification_stats (roi_heads/fast_rcnn.py:88-115, 307-352, 424-463)
+ * for all images at once, without the reference's host reads (.item(), nonzero, get_deltas' assertion).
+ * Box targets: Box2BoxTransform.get_deltas (modeling/box_regression.py:43-76) for box_dim 4 (x1, y1, x2, y2), and
+ * Box2BoxTransformRotated.get_deltas (:145-180) for box_dim 5 (cx, cy, w, h, angle_deg); weights[box_dim] (HOST).
+ * Regression, summed: loss_type D2B_LOSS_SMOOTH_L1 = fvcore smooth_l1_loss with `beta` (|d| for beta < 1e-5) of the deltas
+ * against the get_deltas targets; D2B_LOSS_GIOU (box_dim 4 only) = fvcore giou_loss (eps 1e-7) of the boxes decoded by
+ * Box2BoxTransform.apply_deltas (:78-116, dw / dh clamped at scale_clamp; the gradient passes the clamp at equality, is 0
+ * above it) against the GT boxes.  Predictions (logits, scores, deltas) are
+ * elements of `dtype` (D2B_F32 / D2B_F16 / D2B_BF16) read in place, fp32 arithmetic; boxes are fp32.
+ * Reductions are per-CTA partials added in a fixed order by a second launch (no float atomics): bitwise reproducible.
+ * status [1] int32, OR of D2B_LOSS_STATUS_*: INVALID_BOX when a source box width is not > 0 (the reference's assertion in
+ * get_deltas: every anchor for the dense losses, the foreground proposals for Fast R-CNN); INVALID_CLASS when a Fast R-CNN
+ * gt class is outside [0, K] or a dense int64 label outside [-1, K] (int8: outside {-1, 0, 1}); INVALID_BOX_ORDER (GIoU)
+ * when a decoded or GT box of a regressed row fails fvcore's x2 >= x1 and y2 >= y1 (NaN included); with GIoU the
+ * get_deltas assertion does not apply, as in the reference.  No host synchronisation, static shapes: capturable in a CUDA graph.  All arguments are checked
+ * before the first CUDA call.
+ *
+ * Dense: lv->logits[l] [N,R_l,K] (16-byte aligned), lv->deltas[l] [N,R_l,box_dim] -- the reference's per-level lists, no cat;
+ *   anchors [R,box_dim] shared by the images (R = sum R_l), gt_boxes [N,R,box_dim] matched GT boxes, labels [N,R]:
+ *     D2B_LABELS_I8   int8 {-1, 0, 1} (RPN gt_labels), K must be 1: target = label;
+ *     D2B_LABELS_I64  int64 {-1, 0..K-1, K = background} (RetinaNet gt_labels): target = one_hot(label)[:K].
+ *   Classification: fvcore sigmoid_focal_loss(gamma, alpha; alpha < 0 = no weighting) summed over the rows with label >= 0;
+ *   gamma = 0 and alpha < 0 is binary_cross_entropy_with_logits.  Rows with label -1 are not read.  Regression over the
+ *   positive rows (I8: label 1, I64: 0 <= label < K).  Outputs (device): cls_sum, reg_sum, num_pos, num_neg (I8: label 0,
+ *   I64: label K).  workspace: d2b_dense_loss_workspace_bytes(lv, N, K, dtype) bytes, 16-byte aligned.
+ *   Backward: grad_cls / grad_reg (device scalars) = d loss / d cls_sum, d loss / d reg_sum; lv->grad_logits[l] (16-byte
+ *   aligned) and lv->grad_deltas[l] are fully written in `dtype` (0 on ignored / non-positive rows).
+ * Fast R-CNN: scores [R,K+1], deltas [R,kreg*box_dim] (kreg = K class-specific, gathered at the gt class, or 1), proposals
+ *   and gt_boxes [R,box_dim] fp32, gt_classes [R] int64.  cls_sum = sum of cross_entropy over all rows; reg_sum over the
+ *   foreground rows (0 <= class < K); the counts of _log_classification_stats (argmax: first index on ties, NaN wins).
+ *   workspace: d2b_frcnn_loss_workspace_bytes(R) bytes, 16-byte aligned.  Backward: grad_scores / grad_deltas fully written. */
+#define D2B_LABELS_I8 0
+#define D2B_LABELS_I64 1
+#define D2B_LOSS_STATUS_INVALID_BOX 1
+#define D2B_LOSS_STATUS_INVALID_CLASS 2
+#define D2B_LOSS_STATUS_INVALID_BOX_ORDER 4
+#define D2B_LOSS_SMOOTH_L1 0
+#define D2B_LOSS_GIOU 1
+typedef struct {
+  int num_levels;
+  const void* logits[D2B_MAX_LEVELS];
+  const void* deltas[D2B_MAX_LEVELS];
+  void* grad_logits[D2B_MAX_LEVELS];
+  void* grad_deltas[D2B_MAX_LEVELS];
+  int R[D2B_MAX_LEVELS];
+} d2b_dense_loss_levels;
+size_t d2b_dense_loss_workspace_bytes(const d2b_dense_loss_levels* lv, int N, int K, int dtype);
+int d2b_dense_loss_forward(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int dtype, const float* anchors,
+                           const float* gt_boxes, const void* labels, int label_kind, float gamma, float alpha, float beta,
+                           int loss_type, float scale_clamp, const float* weights, float* cls_sum, float* reg_sum, int64_t* num_pos, int64_t* num_neg,
+                           int* status, void* workspace, size_t workspace_bytes, void* stream);
+int d2b_dense_loss_backward(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int dtype, const float* anchors,
+                            const float* gt_boxes, const void* labels, int label_kind, float gamma, float alpha, float beta,
+                            int loss_type, float scale_clamp, const float* weights, const float* grad_cls, const float* grad_reg, void* stream);
+size_t d2b_frcnn_loss_workspace_bytes(int R);
+int d2b_frcnn_loss_forward(const void* scores, const void* deltas, int R, int K, int kreg, int box_dim, int dtype,
+                           const float* proposals, const float* gt_boxes, const int64_t* gt_classes, float beta,
+                           int loss_type, float scale_clamp, const float* weights, float* cls_sum, float* reg_sum, int64_t* num_fg, int64_t* num_accurate,
+                           int64_t* fg_num_accurate, int64_t* num_false_negative, int* status, void* workspace,
+                           size_t workspace_bytes, void* stream);
+int d2b_frcnn_loss_backward(const void* scores, const void* deltas, int R, int K, int kreg, int box_dim, int dtype,
+                            const float* proposals, const float* gt_boxes, const int64_t* gt_classes, float beta,
+                            int loss_type, float scale_clamp, const float* weights, const float* grad_cls, const float* grad_reg, void* grad_scores,
+                            void* grad_deltas, void* stream);
+
 /* ---- Rotated-box IoU --------------------------------------------------------------------
  * Replaces torch.ops.detectron2.box_iou_rotated (csrc/vision.cpp:117,
  * csrc/box_iou_rotated/box_iou_rotated.h:20-33).  boxes1 [N,5], boxes2 [M,5] fp32 -> ious [N,M] fp32. */
