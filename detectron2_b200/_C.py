@@ -26,6 +26,7 @@ MAX_LEVELS = 8
 MAX_IMAGES = 64  # D2B_MAX_IMAGES
 ABI_VERSION = 4  # include/d2b200.h D2B_ABI_VERSION
 DCN_X_NHWC = 1   # D2B_DCN_X_NHWC
+ROI_ROTATED, ROI_BACKWARD = 1, 2  # D2B_ROI_ROTATED / D2B_ROI_BACKWARD
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}  # D2B_F32 / D2B_F16 / D2B_BF16
 MATCH_ROTATED, MATCH_LOW_QUALITY, MATCH_APPEND_GT = 1, 2, 4  # D2B_MATCH_*
 MATCH_MAX_THRESHOLDS = 8  # D2B_MATCH_MAX_THRESHOLDS
@@ -89,6 +90,7 @@ def _declare(lib):
         "d2b_roi_pooler_rotated_backward": (i, [C.POINTER(Pyramid), i, i, f32p, f32p, i, i, i, i, vp]),
         "d2b_roi_pooler_rotated_forward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, vp, i, vp]),
         "d2b_roi_pooler_rotated_backward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, vp, i, f32p, i, i, i, i, vp]),
+        "d2b_roi_pooler_nhwc_supported": (i, [C.POINTER(Pyramid), i, i, i, i]),
         "d2b_nms_workspace_bytes": (sz, [i64, i, i64]),
         "d2b_nms": (i, [f32p, f32p, i64p, i64, d, i, i64, i64p, i64p, vp, sz, vp]),
         "d2b_rpn_prepare": (i, [C.POINTER(RpnLevels), i, f32p, f, i, f32p, f32p, f32p, f32p, i64p, vp, vp]),

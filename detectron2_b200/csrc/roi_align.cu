@@ -1123,13 +1123,13 @@ __global__ void __launch_bounds__(kNhwcThreads, 4) roi_align_nhwc_kernel(const P
   }
 }
 
+static int nhwc_supported(int num_levels, const int* H, const int* W, int C, int PH, int PW, int flags);
+
 static int launch_fwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C, int PH, int PW, int sr, int aligned,
                            void* out, cudaStream_t stream, int out_dt = D2B_F32) {
-  if (C % 4 != 0) return D2B_EUNSUPPORTED;
-  for (int l = 0; l < P.num_levels; ++l) {
-    if ((long long)P.H[l] * P.W[l] * (C / 4) >= (1LL << 28)) return D2B_EUNSUPPORTED;  // 32-bit byte offsets inside an image
+  if (int rc = nhwc_supported(P.num_levels, P.H, P.W, C, PH, PW, 0)) return rc;
+  for (int l = 0; l < P.num_levels; ++l)
     if ((reinterpret_cast<uintptr_t>(P.feat[l]) & 15) != 0) return D2B_EINVAL;
-  }
   (void)N;
   const int bins = PH * PW;
   const int slabs = d2b_cdiv(C, kNhwcCh);
@@ -1142,8 +1142,7 @@ static int launch_fwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C,
   nchunks = d2b_cdiv(bins, chunk);
   const int chunk_pad = chunk | 1;
   const size_t smem = sizeof(float) * 128 * (size_t)chunk_pad;
-  if (nchunks > 65535) return D2B_EUNSUPPORTED;
-  dim3 grid(K, slabs, nchunks);
+  dim3 grid(K, slabs, nchunks);  // nchunks <= 65535: chunks hold >= 7 bins (nhwc_supported)
   // (the per-bin loop alone and a 3-CTA / wider-batch variant were measured against this: profiles/r2_pooler_fwd_ab.md)
   D2B_DISPATCH_DTYPE(out_dt, (roi_align_nhwc_kernel<DT><<<grid, kNhwcThreads, smem, stream>>>(P, rois, C, PH, PW, sr, aligned, chunk,
                                                                                             chunk_pad, out)));
@@ -1404,22 +1403,25 @@ __global__ void __launch_bounds__(kBwdThreads) roi_align_bwd_nhwc_kernel(const P
   }
 }
 
+// gradient tile [rows * PW][128] + per-warp row-collapsed tile [8 warps][PW][128]
+static size_t bwd_nhwc_smem(int rows, int PW) {
+  return sizeof(float) * kNhwcCh * ((size_t)rows * PW + (size_t)(kBwdThreads / 32) * PW);
+}
+
 static int launch_bwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C, int PH, int PW, int sr, int aligned,
                            const void* gout, cudaStream_t stream, int g_dt = D2B_F32) {
-  if (C % 4 != 0) return D2B_EUNSUPPORTED;
+  if (int rc = nhwc_supported(P.num_levels, P.H, P.W, C, PH, PW, D2B_ROI_BACKWARD)) return rc;
   for (int l = 0; l < P.num_levels; ++l)
     if ((reinterpret_cast<uintptr_t>(P.grad[l]) & 15) != 0) return D2B_EINVAL;
   (void)N;
   // bin rows per CTA: all of them, unless that leaves fewer than ~2 CTAs per SM resident (shared memory) AND in the grid
   const int slabs = d2b_cdiv(C, kNhwcCh);
   int rows = PH;
-  auto smem_of = [&](int r) { return sizeof(float) * kNhwcCh * ((size_t)r * PW + (size_t)(kBwdThreads / 32) * PW); };
-  while (rows > 4 && (smem_of(rows) > 100 * 1024 || (long long)K * slabs * d2b_cdiv(PH, rows) < 4LL * d2b_num_sms()) &&
-         smem_of(rows) > 56 * 1024)
+  while (rows > 4 &&
+         (bwd_nhwc_smem(rows, PW) > 100 * 1024 || (long long)K * slabs * d2b_cdiv(PH, rows) < 4LL * d2b_num_sms()) &&
+         bwd_nhwc_smem(rows, PW) > 56 * 1024)
     rows = (rows + 1) / 2;
-  // gradient tile [rows * PW][128] + per-warp row-collapsed tile [8 warps][PW][128]
-  const size_t smem = smem_of(rows);
-  if (smem > 180 * 1024) return D2B_EUNSUPPORTED;
+  const size_t smem = bwd_nhwc_smem(rows, PW);  // <= 180 KB (nhwc_supported)
   dim3 grid(K, slabs, d2b_cdiv(PH, rows));
   D2B_DISPATCH_DTYPE(g_dt, {
     D2B_ALLOW_BIG_SMEM(roi_align_bwd_nhwc_kernel<DT>);
@@ -1540,20 +1542,32 @@ static size_t rot_nhwc_smem(int PH, int PW) {
   return sizeof(float) * 128 * (size_t)(BWD ? PH * PW : ((PH * PW) | 1));
 }
 
-// Shapes the channels-last rotated kernel takes (D2B_OK) or not (D2B_EUNSUPPORTED); host-only, launches nothing.
-template <bool BWD>
-static int rot_nhwc_supported(const Pyr& P, int C, int PH, int PW) {
-  if (C % 4 != 0) return D2B_EUNSUPPORTED;
-  for (int l = 0; l < P.num_levels; ++l)
-    if ((long long)P.H[l] * P.W[l] * (C / 4) >= (1LL << 28)) return D2B_EUNSUPPORTED;
-  if (rot_nhwc_smem<BWD>(PH, PW) > 150 * 1024) return D2B_EUNSUPPORTED;
+// The shape limits of every channels-last kernel (D2B_OK or D2B_EUNSUPPORTED), stated once: the channels-last launchers and
+// d2b_roi_pooler_nhwc_supported all ask this.  Host-only, no CUDA call.
+static int nhwc_supported(int num_levels, const int* H, const int* W, int C, int PH, int PW, int flags) {
+  if (C % 4 != 0) return D2B_EUNSUPPORTED;  // lane = 4 channels
+  for (int l = 0; l < num_levels; ++l)
+    if ((long long)H[l] * W[l] * (C / 4) >= (1LL << 28)) return D2B_EUNSUPPORTED;  // 32-bit byte offsets inside an image
+  const long long bins = (long long)PH * PW;
+  if (flags & D2B_ROI_ROTATED) {
+    // [128 ch][bins] fp32 tile in shared memory; the forward's pitch is bins | 1, and the backward is held to the same bound
+    if (sizeof(float) * 128 * (bins | 1) > 150 * 1024) return D2B_EUNSUPPORTED;
+  } else if (flags & D2B_ROI_BACKWARD) {
+    // launch_bwd_nhwc halves the bin rows per CTA at least this far, and further only while the tile stays above 56 KB:
+    // its tile exceeds 180 KB exactly when this one does, whatever K
+    int rows = PH;
+    while (rows > 4 && bwd_nhwc_smem(rows, PW) > 100 * 1024) rows = (rows + 1) / 2;
+    if (bwd_nhwc_smem(rows, PW) > 180 * 1024) return D2B_EUNSUPPORTED;
+  } else {
+    if ((bins + 6) / 7 > 65535) return D2B_EUNSUPPORTED;  // launch_fwd_nhwc's output chunks hold >= 7 bins: grid.z
+  }
   return D2B_OK;
 }
 
 template <bool BWD>
 static int launch_rot_nhwc(const Pyr& P, const float* rois, int K, int C, int PH, int PW, int sr, const void* gout, void* out,
                            cudaStream_t stream, int dt = D2B_F32) {
-  if (int rc = rot_nhwc_supported<BWD>(P, C, PH, PW)) return rc;
+  if (int rc = nhwc_supported(P.num_levels, P.H, P.W, C, PH, PW, D2B_ROI_ROTATED | (BWD ? D2B_ROI_BACKWARD : 0))) return rc;
   const size_t smem = rot_nhwc_smem<BWD>(PH, PW);
   dim3 grid(K, d2b_cdiv(C, kNhwcCh));
   D2B_DISPATCH_DTYPE(dt, {
@@ -1650,39 +1664,6 @@ __global__ void __launch_bounds__(256) nhwc_to_nchw_kernel(const XposeLevels L, 
 
 }  // namespace
 
-static bool make_pyr(const d2b_pyramid* pyr, Pyr& P);
-
-D2B_API int d2b_roi_align_forward_nhwc(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                       float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
-                                       int aligned, float* out, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;
-  if (!input || !rois || !out || N <= 0 || H <= 0 || W <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0)
-    return D2B_EINVAL;
-  Pyr P = {};
-  P.num_levels = 1;
-  P.feat[0] = input;
-  P.H[0] = H;
-  P.W[0] = W;
-  P.scale[0] = spatial_scale;
-  return launch_fwd_nhwc(P, N, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, out, (cudaStream_t)stream);
-}
-
-
-D2B_API int d2b_roi_align_forward(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                  float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio, int aligned,
-                                  float* out, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;
-  if (!input || !rois || !out || N <= 0 || H <= 0 || W <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0)
-    return D2B_EINVAL;
-  Pyr P = {};
-  P.num_levels = 1;
-  P.feat[0] = input;
-  P.H[0] = H;
-  P.W[0] = W;
-  P.scale[0] = spatial_scale;
-  return launch_fwd(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, out, (cudaStream_t)stream);
-}
-
 static bool make_pyr(const d2b_pyramid* pyr, Pyr& P) {
   if (!pyr || pyr->num_levels < 1 || pyr->num_levels > D2B_MAX_LEVELS) return false;
   P = Pyr{};
@@ -1702,6 +1683,102 @@ static bool make_pyr(const d2b_pyramid* pyr, Pyr& P) {
   P.level_rois = pyr->level_rois;
   if (P.num_levels > 1 && P.max_level - P.min_level + 1 != P.num_levels) return false;
   return true;
+}
+
+// A single-level entry point is a one-level pyramid (pick_level returns 0 for it): same kernels, same launches.
+static d2b_pyramid one_level(const float* feat, float* grad, int H, int W, float scale) {
+  d2b_pyramid p = {};
+  p.num_levels = 1;
+  p.feat[0] = feat;
+  p.grad[0] = grad;
+  p.H[0] = H;
+  p.W[0] = W;
+  p.scale[0] = scale;
+  return p;
+}
+
+// Every backward zero-fills the gradient maps of all levels with one launch before it accumulates into them.
+static int zero_grads(const Pyr& P, int N, int C, cudaStream_t stream) {
+  void* zp[D2B_MAX_LEVELS];
+  size_t zb[D2B_MAX_LEVELS];
+  for (int l = 0; l < P.num_levels; ++l) {
+    zp[l] = P.grad[l];
+    zb[l] = sizeof(float) * (size_t)N * C * P.H[l] * P.W[l];
+  }
+  return d2b_zero_buffers(zp, zb, P.num_levels, stream);
+}
+
+D2B_API int d2b_roi_pooler_nhwc_supported(const d2b_pyramid* pyr, int C, int pooled_h, int pooled_w, int flags) {
+  if (!pyr || pyr->num_levels < 1 || pyr->num_levels > D2B_MAX_LEVELS || C < 0 || pooled_h <= 0 || pooled_w <= 0)
+    return D2B_EINVAL;
+  return nhwc_supported(pyr->num_levels, pyr->H, pyr->W, C, pooled_h, pooled_w, flags);
+}
+
+D2B_API int d2b_roi_align_forward(const float* input, int N, int C, int H, int W, const float* rois, int K,
+                                  float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio, int aligned,
+                                  float* out, void* stream) {
+  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
+  return d2b_roi_pooler_forward(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, out, stream);
+}
+
+D2B_API int d2b_roi_align_forward_nhwc(const float* input, int N, int C, int H, int W, const float* rois, int K,
+                                       float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
+                                       int aligned, float* out, void* stream) {
+  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
+  return d2b_roi_pooler_forward_nhwc(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, out, stream);
+}
+
+D2B_API int d2b_roi_align_backward(const float* grad_out, const float* rois, int K, float spatial_scale, int pooled_h,
+                                   int pooled_w, int N, int C, int H, int W, int sampling_ratio, int aligned,
+                                   float* grad_in, void* stream) {
+  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
+  if ((size_t)N * C * H * W == 0) return D2B_OK;  // no gradient element to write
+  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
+  return d2b_roi_pooler_backward(&p, N, C, grad_out, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, stream);
+}
+
+D2B_API int d2b_roi_align_backward_nhwc(const float* grad_out, const float* rois, int K, float spatial_scale,
+                                        int pooled_h, int pooled_w, int N, int C, int H, int W, int sampling_ratio,
+                                        int aligned, float* grad_in, void* stream) {
+  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
+  if ((size_t)N * C * H * W == 0) return D2B_OK;
+  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
+  return d2b_roi_pooler_backward_nhwc(&p, N, C, grad_out, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, stream);
+}
+
+D2B_API int d2b_roi_align_rotated_forward(const float* input, int N, int C, int H, int W, const float* rois, int K,
+                                          float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
+                                          float* out, void* stream) {
+  if (K == 0 || C == 0) return D2B_OK;  // before the pooler's argument checks
+  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
+  return d2b_roi_pooler_rotated_forward(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, out, stream);
+}
+
+D2B_API int d2b_roi_align_rotated_forward_nhwc(const float* input, int N, int C, int H, int W, const float* rois, int K,
+                                               float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
+                                               float* out, void* stream) {
+  if (K == 0 || C == 0) return D2B_OK;
+  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
+  return d2b_roi_pooler_rotated_forward_nhwc_t(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, out, D2B_F32, stream);
+}
+
+D2B_API int d2b_roi_align_rotated_backward(const float* grad_out, const float* rois, int K, float spatial_scale,
+                                           int pooled_h, int pooled_w, int N, int C, int H, int W, int sampling_ratio,
+                                           float* grad_in, void* stream) {
+  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
+  if ((size_t)N * C * H * W == 0) return D2B_OK;
+  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
+  return d2b_roi_pooler_rotated_backward(&p, N, C, grad_out, rois, K, pooled_h, pooled_w, sampling_ratio, stream);
+}
+
+D2B_API int d2b_roi_align_rotated_backward_nhwc(const float* grad_out, const float* rois, int K, float spatial_scale,
+                                                int pooled_h, int pooled_w, int N, int C, int H, int W,
+                                                int sampling_ratio, float* grad_in, void* stream) {
+  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0 || (reinterpret_cast<uintptr_t>(grad_in) & 15) != 0) return D2B_EINVAL;
+  if ((size_t)N * C * H * W == 0) return D2B_OK;
+  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
+  return d2b_roi_pooler_rotated_backward_nhwc_t(&p, N, C, grad_out, D2B_F32, rois, K, pooled_h, pooled_w, sampling_ratio,
+                                                stream);
 }
 
 D2B_API int d2b_roi_pooler_forward(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
@@ -1788,55 +1865,14 @@ D2B_API int d2b_pyramid_nhwc_to_nchw(const d2b_pyramid* pyr, int N, int C, float
   return d2b_pyramid_nhwc_to_nchw_t(pyr, N, C, reinterpret_cast<void* const*>(dst), D2B_F32, stream);
 }
 
-D2B_API int d2b_roi_align_rotated_forward_nhwc(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                               float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
-                                               float* out, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;
-  if (!input || !rois || !out || N <= 0 || H <= 0 || W <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0) return D2B_EINVAL;
-  if ((reinterpret_cast<uintptr_t>(input) & 15) != 0) return D2B_EINVAL;
-  Pyr P = {};
-  P.num_levels = 1;
-  P.feat[0] = input;
-  P.H[0] = H;
-  P.W[0] = W;
-  P.scale[0] = spatial_scale;
-  return launch_rot_nhwc<false>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, nullptr, out, (cudaStream_t)stream);
-}
-
-D2B_API int d2b_roi_align_rotated_backward_nhwc(const float* grad_out, const float* rois, int K, float spatial_scale,
-                                                int pooled_h, int pooled_w, int N, int C, int H, int W,
-                                                int sampling_ratio, float* grad_in, void* stream) {
-  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
-  if ((reinterpret_cast<uintptr_t>(grad_in) & 15) != 0) return D2B_EINVAL;
-  size_t bytes = sizeof(float) * (size_t)N * C * H * W;
-  if (bytes) D2B_CUDA(cudaMemsetAsync(grad_in, 0, bytes, (cudaStream_t)stream));
-  if (K == 0 || bytes == 0) return D2B_OK;
-  if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  Pyr P = {};
-  P.num_levels = 1;
-  P.grad[0] = grad_in;
-  P.H[0] = H;
-  P.W[0] = W;
-  P.scale[0] = spatial_scale;
-  return launch_rot_nhwc<true>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, grad_out, nullptr, (cudaStream_t)stream);
-}
-
 D2B_API int d2b_roi_pooler_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
                                            const float* rois, int K, int pooled_h, int pooled_w, int sampling_ratio, int aligned,
                                            void* stream) {
   Pyr P;
   if (!make_pyr(pyr, P) || N < 0 || C < 0 || !dtype_ok(grad_dtype)) return D2B_EINVAL;
-  {
-    void* zp[D2B_MAX_LEVELS];
-    size_t zb[D2B_MAX_LEVELS];
-    for (int l = 0; l < P.num_levels; ++l) {
-      if (!P.grad[l]) return D2B_EINVAL;
-      zp[l] = P.grad[l];
-      zb[l] = sizeof(float) * (size_t)N * C * P.H[l] * P.W[l];
-    }
-    int rc = d2b_zero_buffers(zp, zb, P.num_levels, (cudaStream_t)stream);  // all levels zero-filled by one launch
-    if (rc) return rc;
-  }
+  for (int l = 0; l < P.num_levels; ++l)
+    if (!P.grad[l]) return D2B_EINVAL;
+  if (int rc = zero_grads(P, N, C, (cudaStream_t)stream)) return rc;
   if (K == 0 || C == 0 || N == 0) return D2B_OK;
   if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
   return launch_bwd_nhwc(P, N, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, grad_out, (cudaStream_t)stream, grad_dtype);
@@ -1847,100 +1883,16 @@ D2B_API int d2b_roi_pooler_backward_nhwc(const d2b_pyramid* pyr, int N, int C, c
   return d2b_roi_pooler_backward_nhwc_t(pyr, N, C, grad_out, D2B_F32, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, stream);
 }
 
-D2B_API int d2b_roi_align_backward_nhwc(const float* grad_out, const float* rois, int K, float spatial_scale,
-                                        int pooled_h, int pooled_w, int N, int C, int H, int W, int sampling_ratio,
-                                        int aligned, float* grad_in, void* stream) {
-  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
-  size_t bytes = sizeof(float) * (size_t)N * C * H * W;
-  if (bytes) D2B_CUDA(cudaMemsetAsync(grad_in, 0, bytes, (cudaStream_t)stream));
-  if (K == 0 || bytes == 0) return D2B_OK;
-  if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  Pyr P = {};
-  P.num_levels = 1;
-  P.grad[0] = grad_in;
-  P.H[0] = H;
-  P.W[0] = W;
-  P.scale[0] = spatial_scale;
-  return launch_bwd_nhwc(P, N, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, grad_out, (cudaStream_t)stream);
-}
-
 D2B_API int d2b_roi_pooler_backward(const d2b_pyramid* pyr, int N, int C, const float* grad_out, const float* rois,
                                     int K, int pooled_h, int pooled_w, int sampling_ratio, int aligned, void* stream) {
   Pyr P;
   if (!make_pyr(pyr, P) || N < 0 || C < 0) return D2B_EINVAL;
-  {
-    void* zp[D2B_MAX_LEVELS];
-    size_t zb[D2B_MAX_LEVELS];
-    for (int l = 0; l < P.num_levels; ++l) {
-      if (!P.grad[l]) return D2B_EINVAL;
-      zp[l] = P.grad[l];
-      zb[l] = sizeof(float) * (size_t)N * C * P.H[l] * P.W[l];
-    }
-    int rc = d2b_zero_buffers(zp, zb, P.num_levels, (cudaStream_t)stream);  // all levels zero-filled by one launch
-    if (rc) return rc;
-  }
+  for (int l = 0; l < P.num_levels; ++l)
+    if (!P.grad[l]) return D2B_EINVAL;
+  if (int rc = zero_grads(P, N, C, (cudaStream_t)stream)) return rc;
   if (K == 0 || C == 0 || N == 0) return D2B_OK;
   if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
   return launch_fwd(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, nullptr, (cudaStream_t)stream, grad_out);
-}
-
-D2B_API int d2b_roi_align_rotated_forward(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                          float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
-                                          float* out, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;
-  if (!input || !rois || !out || N <= 0 || H <= 0 || W <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0)
-    return D2B_EINVAL;
-  Pyr P = {};
-  P.num_levels = 1;
-  P.feat[0] = input;
-  P.H[0] = H;
-  P.W[0] = W;
-  P.scale[0] = spatial_scale;
-  int cpc = pick_c_per_cta(K, C);
-  dim3 grid(K, d2b_cdiv(C, cpc));
-  roi_align_rot_fwd_kernel<1024><<<grid, kThreads, 0, (cudaStream_t)stream>>>(P, rois, C, pooled_h, pooled_w, sampling_ratio,
-                                                                               cpc, out);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
-}
-
-template <bool ROT>
-static int roi_bwd_launch(const float* grad_out, const float* rois, int K, float spatial_scale, int pooled_h,
-                          int pooled_w, int N, int C, int H, int W, int sampling_ratio, int aligned, float* grad_in,
-                          void* stream) {
-  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
-  size_t bytes = sizeof(float) * (size_t)N * C * H * W;
-  if (bytes) D2B_CUDA(cudaMemsetAsync(grad_in, 0, bytes, (cudaStream_t)stream));
-  if (K == 0 || bytes == 0) return D2B_OK;
-  if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  Pyr P = {};
-  P.num_levels = 1;
-  P.grad[0] = grad_in;
-  P.H[0] = H;
-  P.W[0] = W;
-  P.scale[0] = spatial_scale;
-  if (!ROT)
-    return launch_fwd(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, nullptr, (cudaStream_t)stream, grad_out);
-  int cpc = pick_c_per_cta(K, C);
-  dim3 grid(K, d2b_cdiv(C, cpc));
-  roi_align_bwd_kernel<ROT><<<grid, kThreads, 0, (cudaStream_t)stream>>>(P, grad_out, rois, C, pooled_h, pooled_w,
-                                                                         sampling_ratio, aligned, cpc);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
-}
-
-D2B_API int d2b_roi_align_backward(const float* grad_out, const float* rois, int K, float spatial_scale, int pooled_h,
-                                   int pooled_w, int N, int C, int H, int W, int sampling_ratio, int aligned,
-                                   float* grad_in, void* stream) {
-  return roi_bwd_launch<false>(grad_out, rois, K, spatial_scale, pooled_h, pooled_w, N, C, H, W, sampling_ratio,
-                               aligned, grad_in, stream);
-}
-
-D2B_API int d2b_roi_align_rotated_backward(const float* grad_out, const float* rois, int K, float spatial_scale,
-                                           int pooled_h, int pooled_w, int N, int C, int H, int W, int sampling_ratio,
-                                           float* grad_in, void* stream) {
-  return roi_bwd_launch<true>(grad_out, rois, K, spatial_scale, pooled_h, pooled_w, N, C, H, W, sampling_ratio, 1,
-                              grad_in, stream);
 }
 
 // ------------------------------------------------------------------ multi-level rotated pooler
@@ -1952,16 +1904,6 @@ static int rot_pooler_args(const d2b_pyramid* pyr, int N, int C, int K, int dtyp
   if (!make_pyr(pyr, P) || P.level_rois || N < 0 || C < 0 || K < 0 || !dtype_ok(dtype)) return D2B_EINVAL;
   if (N == 0 && K > 0) return D2B_EINVAL;  // RoIs of images that do not exist
   return D2B_OK;
-}
-
-static int rot_pooler_zero_grads(const Pyr& P, int N, int C, cudaStream_t stream) {
-  void* zp[D2B_MAX_LEVELS];
-  size_t zb[D2B_MAX_LEVELS];
-  for (int l = 0; l < P.num_levels; ++l) {
-    zp[l] = P.grad[l];
-    zb[l] = sizeof(float) * (size_t)N * C * P.H[l] * P.W[l];
-  }
-  return d2b_zero_buffers(zp, zb, P.num_levels, stream);  // all levels zero-filled by one launch
 }
 
 D2B_API int d2b_roi_pooler_rotated_forward(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
@@ -2000,7 +1942,7 @@ D2B_API int d2b_roi_pooler_rotated_backward(const d2b_pyramid* pyr, int N, int C
   for (int l = 0; l < P.num_levels; ++l)
     if (!P.grad[l]) return D2B_EINVAL;
   if (K > 0 && (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0)) return D2B_EINVAL;
-  int rc = rot_pooler_zero_grads(P, N, C, (cudaStream_t)stream);
+  int rc = zero_grads(P, N, C, (cudaStream_t)stream);
   if (rc || K == 0) return rc;
   int cpc = pick_c_per_cta(K, C);
   dim3 grid(K, d2b_cdiv(C, cpc));
@@ -2019,8 +1961,10 @@ D2B_API int d2b_roi_pooler_rotated_backward_nhwc_t(const d2b_pyramid* pyr, int N
   for (int l = 0; l < P.num_levels; ++l)
     if (!P.grad[l] || (reinterpret_cast<uintptr_t>(P.grad[l]) & 15) != 0) return D2B_EINVAL;
   if (K > 0 && (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0)) return D2B_EINVAL;
-  if (int rc = K > 0 ? rot_nhwc_supported<true>(P, C, pooled_h, pooled_w) : D2B_OK) return rc;  // before the zero-fill
-  int rc = rot_pooler_zero_grads(P, N, C, (cudaStream_t)stream);
+  if (int rc = K > 0 ? nhwc_supported(P.num_levels, P.H, P.W, C, pooled_h, pooled_w, D2B_ROI_ROTATED | D2B_ROI_BACKWARD)
+                     : D2B_OK)
+    return rc;  // before the zero-fill
+  int rc = zero_grads(P, N, C, (cudaStream_t)stream);
   if (rc || K == 0) return rc;
   return launch_rot_nhwc<true>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, grad_out, nullptr, (cudaStream_t)stream,
                                grad_dtype);

@@ -11,6 +11,7 @@ Two op namespaces are served:
 PyTorch is plumbing here: allocation, streams, autograd graph.  All arithmetic happens in the hand-written kernels.
 """
 import ctypes as C
+import functools
 import os
 from typing import List, Optional, Tuple
 
@@ -29,37 +30,61 @@ def _f32c(t: Optional[Tensor]) -> Optional[Tensor]:
 
 
 # =================================================================================== RoIAlign
-# Feature-map layout policy of the axis-aligned forward (D2B_POOLER_LAYOUT = auto | nchw | nhwc):
-#   * channels_last inputs are consumed in place by the NHWC kernel (torchvision would .contiguous() them first);
-#   * NCHW inputs go to the NCHW kernel, unless the call is large enough that "one layout-change launch + NHWC
-#     pooling" is cheaper.  Cost model fitted to tools/bench_pooler_layouts.py on an H100 80GB HBM3 SXM at 700 W
-#     (bench.py's 800x1333 pyramid, 256 channels; 1 000 / 512 / 2 000 RoIs at 7x7 and 100 at 14x14); it picks the faster
-#     path on all four.
+# One host path serves the eight RoIAlign ops: axis-aligned or rotated, each as a single-level op (a one-level pyramid) or
+# a multi-level pooler op, forward and backward.  Feature-map layout policy (D2B_POOLER_LAYOUT = auto | nchw | nhwc):
+#   * shapes the channels-last kernels do not take (d2b_roi_pooler_nhwc_supported) go to the NCHW kernels;
+#   * channels_last inputs are consumed in place by the channels-last kernels (torchvision would .contiguous() them first);
+#   * NCHW inputs go to the NCHW kernels, unless the call is large enough that "one layout-change launch + channels-last
+#     kernel" is cheaper.  Cost model of the axis-aligned forward fitted to tools/bench_pooler_layouts.py on an H100 80GB
+#     HBM3 SXM at 700 W (bench.py's 800x1333 pyramid, 256 channels; 1 000 / 512 / 2 000 RoIs at 7x7 and 100 at 14x14); it
+#     picks the faster path on all four.  The backward and rotated per-element costs are carried over from the kernels'
+#     first tuning and have not been re-measured on an H100 (the layout-change cost per byte has); the choice only changes
+#     speed, every path computes the same result.
 POOLER_LAYOUT = os.environ.get("D2B_POOLER_LAYOUT", "auto")
-_NCHW_PS_PER_OUT = 21.0      # NCHW kernel: picoseconds per output element (13.9 mask head .. 27.5 box head, 512 RoIs)
-_NHWC_PS_PER_OUT = 9.0       # NHWC kernel (7.8 .. 16.8)
+# picoseconds per output element (forward) / grad_out element (backward): (NCHW kernel, channels-last kernel)
+_PS_PER_OUT = {  # (rotated, backward)
+    (False, False): (21.0, 9.0),  # NCHW 13.9 mask head .. 27.5 box head (512 RoIs); channels-last 7.8 .. 16.8
+    (False, True): (40.0, 8.0),   # channels-last: one red.v4 per footprint pixel
+    (True, False): (30.0, 10.0),
+    (True, True): (64.0, 16.0),
+}
 _XPOSE_PS_PER_BYTE = 0.72    # layout change: 91.4 MB of fp32 features in 65-68 us (reads + writes each byte once)
+_HALF = (torch.float16, torch.bfloat16)
+_ONE_LEVEL = (0, 0, 0, 1.0)  # min_level, max_level, canonical_level, canonical_box_size of a single-level call
 
 
 def _is_channels_last(t: Tensor) -> bool:
     return t.dim() == 4 and not t.is_contiguous() and t.is_contiguous(memory_format=torch.channels_last)
 
 
-def _nhwc_ok(feats, c: int) -> bool:
-    return c % 4 == 0 and all(t.shape[2] * t.shape[3] * (c // 4) < 2 ** 28 for t in feats)
+@functools.lru_cache(maxsize=256)
+def _nhwc_supported(c: int, hw: Tuple[Tuple[int, int], ...], pooled_h: int, pooled_w: int, flags: int) -> bool:
+    """d2b_roi_pooler_nhwc_supported: the channels-last kernels take `c` channels over levels of (h, w) sizes `hw`."""
+    P = _C.Pyramid()
+    P.num_levels = len(hw)
+    for l, (h, w) in enumerate(hw):
+        P.H[l], P.W[l] = h, w
+    return _C.lib().d2b_roi_pooler_nhwc_supported(C.byref(P), c, pooled_h, pooled_w, flags) == 0
 
 
-def _pick_layout(feats, n_out: int) -> str:
-    """'cl' = channels_last inputs used in place, 'xpose' = layout change + NHWC kernel, 'nchw' = NCHW kernel."""
-    c = feats[0].shape[1]
-    if POOLER_LAYOUT == "nchw" or not _nhwc_ok(feats, c):
+def _pick_layout(feats, n_out: int, pooled: Tuple[int, int] = (1, 1), rotated: bool = False, backward: bool = False,
+                 channels_last: Optional[bool] = None) -> str:
+    """'cl' = channels-last levels used in place (forward) / gradients produced channels-last (backward), 'xpose' = layout
+    change + channels-last kernel, 'nchw' = NCHW kernel.  feats: the levels as tensors or as (n, c, h, w) sizes;
+    channels_last defaults to "every level is a 16-byte aligned channels_last tensor"."""
+    shapes = [tuple(t.shape) if isinstance(t, Tensor) else tuple(t) for t in feats]
+    flags = (_C.ROI_ROTATED if rotated else 0) | (_C.ROI_BACKWARD if backward else 0)
+    if POOLER_LAYOUT == "nchw" or not _nhwc_supported(shapes[0][1], tuple(s[2:] for s in shapes), *pooled, flags):
         return "nchw"
-    if all(_is_channels_last(t) and t.data_ptr() % 16 == 0 for t in feats):
+    if channels_last is None:
+        channels_last = all(_is_channels_last(t) and t.data_ptr() % 16 == 0 for t in feats)
+    if channels_last:
         return "cl"
     if POOLER_LAYOUT == "nhwc":
         return "xpose"
-    feat_bytes = 4 * sum(t.numel() for t in feats)
-    return "xpose" if (n_out * _NHWC_PS_PER_OUT + feat_bytes * _XPOSE_PS_PER_BYTE < n_out * _NCHW_PS_PER_OUT) else "nchw"
+    nchw_ps, nhwc_ps = _PS_PER_OUT[(rotated, backward)]
+    feat_bytes = 4 * sum(n * c * h * w for (n, c, h, w) in shapes)
+    return "xpose" if n_out * nhwc_ps + feat_bytes * _XPOSE_PS_PER_BYTE < n_out * nchw_ps else "nchw"
 
 
 def _to_nhwc(fs, P, n: int, c: int, device):
@@ -72,8 +97,37 @@ def _to_nhwc(fs, P, n: int, c: int, device):
     return bufs
 
 
+def _from_nhwc(bufs, n: int, c: int, device, dtype=torch.float32):
+    """One launch: fp32 NHWC buffers -> freshly allocated NCHW tensors of `dtype` (fp32, or fp16 / bf16: the layout change
+    is also the down-cast of the gradients of half-precision features)."""
+    outs = [torch.empty((b.shape[0], b.shape[3], b.shape[1], b.shape[2]), dtype=dtype, device=device) for b in bufs]
+    P = _C.Pyramid()
+    P.num_levels = len(bufs)
+    for l, b in enumerate(bufs):
+        P.feat[l] = b.data_ptr()
+        P.H[l], P.W[l] = b.shape[1], b.shape[2]
+    dst = (C.c_void_p * len(outs))(*[o.data_ptr() for o in outs])
+    check(_C.lib().d2b_pyramid_nhwc_to_nchw_t(C.byref(P), n, c, dst, _C.DTYPE_CODE[dtype], stream_ptr(device)),
+          "pyramid_nhwc_to_nchw")
+    return outs
+
+
 def _same_half_dtype(ts) -> bool:
     return ts[0].dtype in _HALF and all(t.dtype == ts[0].dtype for t in ts)
+
+
+def _pyramid(feats, grads, scales, min_level, max_level, canonical_level, canonical_box_size, level_rois=None):
+    P = _C.Pyramid()
+    P.level_rois = level_rois.data_ptr() if level_rois is not None else None
+    P.num_levels = len(feats)
+    for l, t in enumerate(feats):
+        P.feat[l] = t.data_ptr()
+        P.grad[l] = grads[l].data_ptr() if grads is not None else None
+        P.H[l], P.W[l] = t.shape[2], t.shape[3]
+        P.scale[l] = scales[l]
+    P.min_level, P.max_level, P.canonical_level = min_level, max_level, canonical_level
+    P.canonical_box_size = canonical_box_size
+    return P
 
 
 def pyramid_to_channels_last(feats: List[Tensor]) -> List[Tensor]:
@@ -81,12 +135,13 @@ def pyramid_to_channels_last(feats: List[Tensor]) -> List[Tensor]:
     with ONE kernel launch.  A caller that pools the same features more than once per image (box head + mask head,
     roi_heads.py:798,843 in the reference) converts once and hands the result to every ROIPooler / ROIAlign call, which
     then run the channels-last kernel in place.  Inputs that are already channels_last, need autograd, are not fp32 or
-    do not fit the NHWC kernel's limits are returned through torch's own (autograd-aware) conversion / unchanged."""
+    do not fit the channels-last kernels' limits are returned through torch's own (autograd-aware) conversion / unchanged."""
     _C.require_cuda(*feats)
     if len(feats) == 0 or len(feats) > _C.MAX_LEVELS:
         raise RuntimeError("pyramid_to_channels_last: need 1..%d levels" % _C.MAX_LEVELS)
     c = feats[0].shape[1]
-    if not _nhwc_ok(feats, c) or any(t.shape[:2] != feats[0].shape[:2] for t in feats):
+    if (not _nhwc_supported(c, tuple((t.shape[2], t.shape[3]) for t in feats), 1, 1, 0)
+            or any(t.shape[:2] != feats[0].shape[:2] for t in feats)):
         return list(feats)
     if any(t.dtype != torch.float32 for t in feats) or (torch.is_grad_enabled() and any(t.requires_grad for t in feats)):
         return [t.contiguous(memory_format=torch.channels_last) for t in feats]
@@ -110,31 +165,132 @@ def _roi_common(input: Tensor, rois: Tensor, cols: int):
         raise RuntimeError("roi_align: rois must be K x %d" % cols)
 
 
+def _check_levels(what: str, feats, scales):
+    if len(feats) < 1 or len(feats) > _C.MAX_LEVELS or len(feats) != len(scales):
+        raise RuntimeError("%s: need 1..%d feature levels with one scale each" % (what, _C.MAX_LEVELS))
+
+
+def _roi_forward(feats, rois, scales, pooled_h: int, pooled_w: int, sampling_ratio: int, levels, rotated: bool,
+                 aligned: bool = True, level_rois: Optional[Tensor] = None) -> Tensor:
+    """The forward of every RoIAlign op.  feats: the levels (one for a single-level op); levels: (min_level, max_level,
+    canonical_level, canonical_box_size); rois: the boxes sampled with, level_rois: the ones the FPN level is assigned
+    from when they differ.  The output has the dtype of the features."""
+    r, lr = _f32c(rois), _f32c(level_rois)
+    n, c = feats[0].shape[:2]
+    k = r.shape[0]
+    numel = k * c * pooled_h * pooled_w
+    layout = _pick_layout(feats, numel, (pooled_h, pooled_w), rotated) if numel else "nchw"
+    # half-precision NCHW levels: the layout-change launch reads them as they are (it is also the up-cast) and the pooling
+    # kernel writes the result in their dtype -- no cast passes; every other combination computes on fp32 copies
+    fused_half = layout == "xpose" and _same_half_dtype(feats)
+    fs = list(feats) if fused_half else [t.to(dtype=torch.float32) for t in feats]
+    out_dt = feats[0].dtype if (layout != "nchw" and feats[0].dtype in _C.DTYPE_CODE) else torch.float32
+    out = torch.empty((k, c, pooled_h, pooled_w), dtype=out_dt, device=r.device)
+    if numel:
+        lib = _C.lib()
+        what = "roi_pooler_rotated_forward" if rotated else "roi_pooler_forward"
+        with torch.cuda.device(r.device):
+            if layout != "cl":
+                fs = [t.contiguous() for t in fs]
+            # channels_last tensors: same logical shape, NHWC storage -- _pyramid only takes pointers and H, W
+            P = _pyramid(fs, None, scales, *levels, lr)
+            args = (C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w, sampling_ratio) + (() if rotated else (int(aligned),))
+            if layout == "nchw":
+                fn = lib.d2b_roi_pooler_rotated_forward if rotated else lib.d2b_roi_pooler_forward
+                check(fn(*args, ptr(out), stream_ptr(r.device)), what)
+            else:
+                if layout == "xpose":
+                    bufs = _to_nhwc(fs, P, n, c, r.device)
+                    for l, b in enumerate(bufs):
+                        P.feat[l] = b.data_ptr()
+                fn = lib.d2b_roi_pooler_rotated_forward_nhwc_t if rotated else lib.d2b_roi_pooler_forward_nhwc_t
+                check(fn(*args, ptr(out), _C.DTYPE_CODE[out_dt], stream_ptr(r.device)), what + "_nhwc")
+    return out if out.dtype == feats[0].dtype else out.to(feats[0].dtype)
+
+
+def _roi_backward(grad, rois, shapes, scales, pooled_h: int, pooled_w: int, sampling_ratio: int, levels, rotated: bool,
+                  channels_last: bool, aligned: bool = True, level_rois: Optional[Tensor] = None,
+                  half_grads: bool = False) -> List[Tensor]:
+    """The backward of every RoIAlign op: the gradient of each level, shapes = [n, c, h0, w0, h1, w1, ...].  fp32 NCHW
+    tensors, or channels-last ones when `channels_last` and the channels-last kernel ran; `half_grads`: NCHW gradients in
+    `grad`'s fp16 / bf16 dtype (written by the layout-change launch) instead of fp32."""
+    r, lr = _f32c(rois), _f32c(level_rois)
+    n, c = shapes[0], shapes[1]
+    hw = [(shapes[2 + 2 * l], shapes[3 + 2 * l]) for l in range(len(scales))]
+    layout = (_pick_layout([(n, c, h, w) for (h, w) in hw], grad.numel(), (pooled_h, pooled_w), rotated, True,
+                           channels_last) if n * c else "nchw")
+    # the channels-last kernels read fp16 / bf16 gradients in place; the NCHW kernels take fp32
+    g = grad.contiguous() if (layout != "nchw" and grad.dtype in _C.DTYPE_CODE) else _f32c(grad)
+    lib = _C.lib()
+    what = "roi_pooler_rotated_backward" if rotated else "roi_pooler_backward"
+    args = (ptr(r), r.shape[0], pooled_h, pooled_w, sampling_ratio) + (() if rotated else (int(aligned),))
+    with torch.cuda.device(g.device):
+        if layout == "nchw":
+            grads = [torch.empty((n, c, h, w), dtype=torch.float32, device=g.device) for (h, w) in hw]
+            P = _pyramid(grads, grads, scales, *levels, lr)
+            fn = lib.d2b_roi_pooler_rotated_backward if rotated else lib.d2b_roi_pooler_backward
+            check(fn(C.byref(P), n, c, ptr(g), *args, stream_ptr(g.device)), what)
+        else:
+            bufs = [torch.empty((n, h, w, c), dtype=torch.float32, device=g.device) for (h, w) in hw]
+            views = [b.permute(0, 3, 1, 2) for b in bufs]  # logical NCHW shape: _pyramid reads H, W from dims 2, 3
+            P = _pyramid(views, views, scales, *levels, lr)
+            fn = lib.d2b_roi_pooler_rotated_backward_nhwc_t if rotated else lib.d2b_roi_pooler_backward_nhwc_t
+            check(fn(C.byref(P), n, c, ptr(g), _C.DTYPE_CODE[g.dtype], *args, stream_ptr(g.device)), what + "_nhwc")
+            if layout == "cl":
+                grads = views
+            else:
+                grads = _from_nhwc(bufs, n, c, g.device, grad.dtype if (half_grads and grad.dtype in _HALF) else torch.float32)
+    if half_grads and grad.dtype in _HALF:
+        grads = [t if t.dtype == grad.dtype else t.to(grad.dtype) for t in grads]
+    return grads
+
+
+def _one_level_backward(grad, rois, spatial_scale, pooled_h, pooled_w, n, c, h, w, sampling_ratio, rotated, channels_last,
+                        aligned=True) -> Tensor:
+    _C.require_cuda(grad, rois)
+    if n * c * h * w == 0:  # nothing to write (and a pyramid level needs h, w > 0)
+        return torch.empty((n, c, h, w), dtype=grad.dtype, device=grad.device)
+    return _roi_backward(grad, rois, [n, c, h, w], [spatial_scale], pooled_h, pooled_w, sampling_ratio, _ONE_LEVEL, rotated,
+                         channels_last, aligned)[0].to(grad.dtype)
+
+
+def _register_roi_autograd(op, backward_op, rotated: bool):
+    """The autograd pair of the four RoIAlign ops.  Their inputs are (input or feats, rois, *args); the backward op takes
+    args with the feature shapes and the channels-last flag added, and for the axis-aligned pooler the level boxes."""
+
+    def setup_context(ctx, inputs, output):
+        feats, rois, *args = inputs
+        ctx.pyramid = isinstance(feats, (list, tuple))
+        fs = list(feats) if ctx.pyramid else [feats]
+        ctx.save_for_backward(rois)
+        ctx.args = args
+        ctx.shapes = [fs[0].shape[0], fs[0].shape[1]] + [s for t in fs for s in t.shape[2:]]
+        ctx.dtypes = [t.dtype for t in fs]
+        ctx.channels_last = all(_is_channels_last(t) for t in fs)
+
+    def backward(ctx, grad):
+        (rois,) = ctx.saved_tensors
+        a, dts, cl = ctx.args, ctx.dtypes, ctx.channels_last
+        nones = (None,) * (len(a) + 1)
+        if not ctx.pyramid:  # args (scale, ph, pw, sr[, aligned]) -> (scale, ph, pw, n, c, h, w, sr[, aligned], channels_last)
+            return (backward_op(grad, rois, *a[:3], *ctx.shapes, *a[3:], cl).to(dts[0]),) + nones
+        half = dts[0] in _HALF
+        half_grads = half and grad.dtype == dts[0] and all(d == dts[0] for d in dts)
+        if rotated:
+            grads = backward_op(grad, rois, ctx.shapes, *a, cl, half_grads)
+        else:  # same rois as the forward: rounded to the feature dtype for sampling, fp32 for the level
+            grads = backward_op(grad, rois.to(dts[0]).to(torch.float32) if half else rois, ctx.shapes, *a, cl,
+                                rois if half else None, half_grads)
+        return ([g.to(dt) for g, dt in zip(grads, dts)],) + nones
+
+    op.register_autograd(backward, setup_context=setup_context)
+
+
 @torch.library.custom_op("d2b200::roi_align", mutates_args=(), device_types="cuda")
 def roi_align_op(input: Tensor, rois: Tensor, spatial_scale: float, pooled_h: int, pooled_w: int,
                  sampling_ratio: int, aligned: bool) -> Tensor:
     _roi_common(input, rois, 5)
-    r = _f32c(rois)
-    n, c, h, w = input.shape
-    k = r.shape[0]
-    out = torch.empty((k, c, pooled_h, pooled_w), dtype=torch.float32, device=input.device)
-    if out.numel():
-        x = input.to(dtype=torch.float32)
-        layout = _pick_layout([x], out.numel())
-        with torch.cuda.device(x.device):
-            if layout == "nchw":
-                x = x.contiguous()
-                check(_C.lib().d2b_roi_align_forward(ptr(x), n, c, h, w, ptr(r), k, spatial_scale, pooled_h, pooled_w,
-                                                     sampling_ratio, int(aligned), ptr(out), stream_ptr(x.device)),
-                      "roi_align_forward")
-            else:
-                if layout == "xpose":
-                    x = x.contiguous()
-                    x = _to_nhwc([x], _pyramid([x], None, [spatial_scale], 0, 0, 0, 1.0), n, c, x.device)[0]
-                check(_C.lib().d2b_roi_align_forward_nhwc(ptr(x), n, c, h, w, ptr(r), k, spatial_scale, pooled_h,
-                                                          pooled_w, sampling_ratio, int(aligned), ptr(out),
-                                                          stream_ptr(x.device)), "roi_align_forward_nhwc")
-    return out.to(input.dtype)
+    return _roi_forward([input], rois, [spatial_scale], pooled_h, pooled_w, sampling_ratio, _ONE_LEVEL, False, aligned)
 
 
 @roi_align_op.register_fake
@@ -142,62 +298,12 @@ def _(input, rois, spatial_scale, pooled_h, pooled_w, sampling_ratio, aligned):
     return input.new_empty((rois.shape[0], input.shape[1], pooled_h, pooled_w))
 
 
-# Backward and rotated per-element costs are carried over from the kernels' first tuning and have not been re-measured on an
-# H100 (the layout-change cost per byte above has); the choice only changes speed, every path computes the same result.
-_NCHW_BWD_PS_PER_OUT = 40.0  # NCHW backward kernel: picoseconds per grad_out element
-_NHWC_BWD_PS_PER_OUT = 8.0   # channels-last backward (one red.v4 per footprint pixel)
-
-
-def _bwd_layout(shapes_nchw, n_out: int, channels_last: bool) -> str:
-    """'cl': gradients produced channels-last in place; 'xpose': channels-last kernel into scratch + one layout-change
-    launch back to NCHW; 'nchw': the NCHW kernel.  shapes_nchw: [(n, c, h, w)] per level."""
-    c = shapes_nchw[0][1]
-    ok = c % 4 == 0 and POOLER_LAYOUT != "nchw" and all(h * w * (c // 4) < 2 ** 28 for (_, _, h, w) in shapes_nchw)
-    if not ok:
-        return "nchw"
-    if channels_last:
-        return "cl"
-    if POOLER_LAYOUT == "nhwc":
-        return "xpose"
-    feat_bytes = 4 * sum(n * c * h * w for (n, c, h, w) in shapes_nchw)
-    return "xpose" if n_out * _NHWC_BWD_PS_PER_OUT + feat_bytes * _XPOSE_PS_PER_BYTE < n_out * _NCHW_BWD_PS_PER_OUT else "nchw"
-
-
-def _from_nhwc(bufs, n: int, c: int, device, dtype=torch.float32):
-    """One launch: fp32 NHWC buffers -> freshly allocated NCHW tensors of `dtype` (fp32, or fp16 / bf16: the layout change
-    is also the down-cast of the gradients of half-precision features)."""
-    outs = [torch.empty((b.shape[0], b.shape[3], b.shape[1], b.shape[2]), dtype=dtype, device=device) for b in bufs]
-    P = _C.Pyramid()
-    P.num_levels = len(bufs)
-    for l, b in enumerate(bufs):
-        P.feat[l] = b.data_ptr()
-        P.H[l], P.W[l] = b.shape[1], b.shape[2]
-    dst = (C.c_void_p * len(outs))(*[o.data_ptr() for o in outs])
-    check(_C.lib().d2b_pyramid_nhwc_to_nchw_t(C.byref(P), n, c, dst, _C.DTYPE_CODE[dtype], stream_ptr(device)),
-          "pyramid_nhwc_to_nchw")
-    return outs
-
-
 @torch.library.custom_op("d2b200::roi_align_backward", mutates_args=(), device_types="cuda")
 def roi_align_backward_op(grad: Tensor, rois: Tensor, spatial_scale: float, pooled_h: int, pooled_w: int, n: int,
                           c: int, h: int, w: int, sampling_ratio: int, aligned: bool,
                           channels_last: bool = False) -> Tensor:
-    _C.require_cuda(grad, rois)
-    g, r = _f32c(grad), _f32c(rois)
-    layout = _bwd_layout([(n, c, h, w)], g.numel(), channels_last) if n * c * h * w else "nchw"
-    with torch.cuda.device(g.device):
-        if layout == "nchw":
-            gin = torch.empty((n, c, h, w), dtype=torch.float32, device=g.device)
-            check(_C.lib().d2b_roi_align_backward(ptr(g), ptr(r), r.shape[0], spatial_scale, pooled_h, pooled_w, n, c, h,
-                                                  w, sampling_ratio, int(aligned), ptr(gin), stream_ptr(g.device)),
-                  "roi_align_backward")
-        else:
-            buf = torch.empty((n, h, w, c), dtype=torch.float32, device=g.device)
-            check(_C.lib().d2b_roi_align_backward_nhwc(ptr(g), ptr(r), r.shape[0], spatial_scale, pooled_h, pooled_w, n, c,
-                                                       h, w, sampling_ratio, int(aligned), ptr(buf),
-                                                       stream_ptr(g.device)), "roi_align_backward_nhwc")
-            gin = buf.permute(0, 3, 1, 2) if layout == "cl" else _from_nhwc([buf], n, c, g.device)[0]
-    return gin.to(grad.dtype)
+    return _one_level_backward(grad, rois, spatial_scale, pooled_h, pooled_w, n, c, h, w, sampling_ratio, False,
+                               channels_last, aligned)
 
 
 @roi_align_backward_op.register_fake
@@ -206,80 +312,20 @@ def _(grad, rois, spatial_scale, pooled_h, pooled_w, n, c, h, w, sampling_ratio,
     return out.contiguous(memory_format=torch.channels_last) if channels_last else out
 
 
-def _roi_align_setup(ctx, inputs, output):
-    input, rois, spatial_scale, ph, pw, sr, aligned = inputs
-    ctx.save_for_backward(rois)
-    ctx.args = (spatial_scale, ph, pw, tuple(input.shape), sr, aligned, _is_channels_last(input))
-
-
-def _roi_align_bwd(ctx, grad):
-    (rois,) = ctx.saved_tensors
-    scale, ph, pw, (n, c, h, w), sr, aligned, cl = ctx.args
-    gin = roi_align_backward_op(grad, rois, scale, ph, pw, n, c, h, w, sr, aligned, cl)
-    return gin, None, None, None, None, None, None
-
-
-roi_align_op.register_autograd(_roi_align_bwd, setup_context=_roi_align_setup)
-
-
 # ----------------------------------------------------------------------------------- fused multi-level pooler
-_HALF = (torch.float16, torch.bfloat16)
-
-
-def _pyramid(feats, grads, scales, min_level, max_level, canonical_level, canonical_box_size, level_rois=None):
-    P = _C.Pyramid()
-    P.level_rois = level_rois.data_ptr() if level_rois is not None else None
-    P.num_levels = len(feats)
-    for l, t in enumerate(feats):
-        P.feat[l] = t.data_ptr()
-        P.grad[l] = grads[l].data_ptr() if grads is not None else None
-        P.H[l], P.W[l] = t.shape[2], t.shape[3]
-        P.scale[l] = scales[l]
-    P.min_level, P.max_level, P.canonical_level = min_level, max_level, canonical_level
-    P.canonical_box_size = canonical_box_size
-    return P
-
-
 @torch.library.custom_op("d2b200::roi_pooler", mutates_args=(), device_types="cuda")
 def roi_pooler_op(feats: List[Tensor], rois: Tensor, scales: List[float], pooled_h: int, pooled_w: int,
                   sampling_ratio: int, aligned: bool, min_level: int, max_level: int, canonical_level: int,
                   canonical_box_size: float) -> Tensor:
     _C.require_cuda(rois, *feats)
-    if len(feats) < 1 or len(feats) > _C.MAX_LEVELS or len(feats) != len(scales):
-        raise RuntimeError("roi_pooler: need 1..%d feature levels with one scale each" % _C.MAX_LEVELS)
-    r_lvl = _f32c(rois)
+    _check_levels("roi_pooler", feats, scales)
+    r = _f32c(rois)
     # half-precision feature maps: the reference samples with the rois cast to the feature dtype (layers/roi_align.py:60,
     # then torchvision's autocast wrapper upcasts both) while the FPN level comes from the fp32 boxes (poolers.py:245)
     half = feats[0].dtype in _HALF
-    r = r_lvl.to(feats[0].dtype).to(torch.float32) if half else r_lvl
-    n, c = feats[0].shape[:2]
-    k = r.shape[0]
-    numel = k * c * pooled_h * pooled_w
-    layout = _pick_layout(feats, numel) if numel else "nchw"
-    # half-precision NCHW levels: the layout-change launch reads them as they are (it is also the up-cast) and the pooling
-    # kernel writes the result in their dtype -- no cast passes; every other combination computes on fp32 copies
-    fused_half = layout == "xpose" and _same_half_dtype(feats)
-    fs = list(feats) if fused_half else [t.to(dtype=torch.float32) for t in feats]
-    out_dt = feats[0].dtype if (layout != "nchw" and feats[0].dtype in _C.DTYPE_CODE) else torch.float32
-    out = torch.empty((k, c, pooled_h, pooled_w), dtype=out_dt, device=r.device)
-    if numel:
-        with torch.cuda.device(r.device):
-            if layout != "cl":
-                fs = [t.contiguous() for t in fs]
-            # channels_last tensors: same logical shape, NHWC storage -- _pyramid only takes pointers and H, W
-            P = _pyramid(fs, None, scales, min_level, max_level, canonical_level, canonical_box_size, r_lvl if half else None)
-            if layout == "nchw":
-                check(_C.lib().d2b_roi_pooler_forward(C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w, sampling_ratio,
-                                                      int(aligned), ptr(out), stream_ptr(r.device)), "roi_pooler_forward")
-            else:
-                if layout == "xpose":
-                    bufs = _to_nhwc(fs, P, n, c, r.device)
-                    for l, b in enumerate(bufs):
-                        P.feat[l] = b.data_ptr()
-                check(_C.lib().d2b_roi_pooler_forward_nhwc_t(C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w, sampling_ratio,
-                                                             int(aligned), ptr(out), _C.DTYPE_CODE[out_dt],
-                                                             stream_ptr(r.device)), "roi_pooler_forward_nhwc")
-    return out if out.dtype == feats[0].dtype else out.to(feats[0].dtype)
+    return _roi_forward(feats, r.to(feats[0].dtype).to(torch.float32) if half else r, scales, pooled_h, pooled_w,
+                        sampling_ratio, (min_level, max_level, canonical_level, canonical_box_size), False, aligned,
+                        r if half else None)
 
 
 @roi_pooler_op.register_fake
@@ -298,34 +344,9 @@ def roi_pooler_backward_op(grad: Tensor, rois: Tensor, shapes: List[int], scales
     sampled with (half-precision features, see roi_pooler_op).  `half_grads`: return NCHW gradients in `grad`'s fp16 / bf16
     dtype (written by the layout-change launch) instead of fp32."""
     _C.require_cuda(grad, rois, level_rois)
-    r = _f32c(rois)
-    lr = _f32c(level_rois)
-    nl = len(scales)
-    n, c = shapes[0], shapes[1]
-    hw = [(shapes[2 + 2 * l], shapes[3 + 2 * l]) for l in range(nl)]
-    layout = _bwd_layout([(n, c, h, w) for (h, w) in hw], grad.numel(), channels_last) if n * c else "nchw"
-    # the channels-last kernel reads fp16 / bf16 gradients in place; the NCHW kernel takes fp32
-    g = grad.contiguous() if (layout != "nchw" and grad.dtype in _C.DTYPE_CODE) else _f32c(grad)
-    with torch.cuda.device(g.device):
-        if layout == "nchw":
-            grads = [torch.empty((n, c, h, w), dtype=torch.float32, device=g.device) for (h, w) in hw]
-            P = _pyramid(grads, grads, scales, min_level, max_level, canonical_level, canonical_box_size, lr)
-            check(_C.lib().d2b_roi_pooler_backward(C.byref(P), n, c, ptr(g), ptr(r), r.shape[0], pooled_h, pooled_w,
-                                                   sampling_ratio, int(aligned), stream_ptr(g.device)), "roi_pooler_backward")
-        else:
-            bufs = [torch.empty((n, h, w, c), dtype=torch.float32, device=g.device) for (h, w) in hw]
-            views = [b.permute(0, 3, 1, 2) for b in bufs]  # logical NCHW shape: _pyramid reads H, W from dims 2, 3
-            P = _pyramid(views, views, scales, min_level, max_level, canonical_level, canonical_box_size, lr)
-            check(_C.lib().d2b_roi_pooler_backward_nhwc_t(C.byref(P), n, c, ptr(g), _C.DTYPE_CODE[g.dtype], ptr(r), r.shape[0],
-                                                          pooled_h, pooled_w, sampling_ratio, int(aligned),
-                                                          stream_ptr(g.device)), "roi_pooler_backward_nhwc")
-            if layout == "cl":
-                grads = views
-            else:
-                grads = _from_nhwc(bufs, n, c, g.device, grad.dtype if (half_grads and grad.dtype in _HALF) else torch.float32)
-    if half_grads and grad.dtype in _HALF:
-        grads = [t if t.dtype == grad.dtype else t.to(grad.dtype) for t in grads]
-    return grads
+    return _roi_backward(grad, rois, shapes, scales, pooled_h, pooled_w, sampling_ratio,
+                         (min_level, max_level, canonical_level, canonical_box_size), False, channels_last, aligned,
+                         level_rois, half_grads)
 
 
 @roi_pooler_backward_op.register_fake
@@ -337,78 +358,12 @@ def _(grad, rois, shapes, scales, pooled_h, pooled_w, sampling_ratio, aligned, m
     return [o.contiguous(memory_format=torch.channels_last) for o in outs] if channels_last else outs
 
 
-def _pooler_setup(ctx, inputs, output):
-    feats, rois, scales, ph, pw, sr, aligned, lo, hi, cl, cs = inputs
-    ctx.save_for_backward(rois)
-    shapes = [feats[0].shape[0], feats[0].shape[1]]
-    for t in feats:
-        shapes += [t.shape[2], t.shape[3]]
-    ctx.args = (shapes, scales, ph, pw, sr, aligned, lo, hi, cl, cs, [t.dtype for t in feats],
-                all(_is_channels_last(t) for t in feats))
-
-
-def _pooler_bwd(ctx, grad):
-    (rois,) = ctx.saved_tensors
-    shapes, scales, ph, pw, sr, aligned, lo, hi, cl, cs, dts, chl = ctx.args
-    half = dts[0] in _HALF  # same rois as the forward: rounded to the feature dtype for sampling, fp32 for the level
-    grads = roi_pooler_backward_op(grad, rois.to(dts[0]).to(torch.float32) if half else rois, shapes, scales, ph, pw, sr,
-                                   aligned, lo, hi, cl, cs, chl, rois if half else None,
-                                   half and grad.dtype == dts[0] and all(d == dts[0] for d in dts))
-    return [g.to(dt) for g, dt in zip(grads, dts)], None, None, None, None, None, None, None, None, None, None
-
-
-roi_pooler_op.register_autograd(_pooler_bwd, setup_context=_pooler_setup)
-
-
-_ROT_NCHW_PS = (30.0, 64.0)  # rotated NCHW kernels: picoseconds per output element (forward, backward); not re-measured, above
-_ROT_NHWC_PS = (10.0, 16.0)  # rotated channels-last kernels
-
-
-def _rot_layout(n: int, c: int, h: int, w: int, n_out: int, channels_last: bool, bwd: bool) -> str:
-    return _rot_pyramid_layout([(n, c, h, w)], n_out, channels_last, bwd)
-
-
-def _rot_pyramid_layout(shapes_nchw, n_out: int, channels_last: bool, bwd: bool, bins: int = 0) -> str:
-    """Rotated kernels: 'cl', 'xpose' or 'nchw' as in _bwd_layout, for a pyramid of (n, c, h, w) levels.  bins: pooled
-    h * w when known; the channels-last kernel keeps a [128 channels][bins] fp32 tile in shared memory (<= 150 KB)."""
-    c = shapes_nchw[0][1]
-    if c % 4 != 0 or POOLER_LAYOUT == "nchw" or any(h * w * (c // 4) >= 2 ** 28 for (_, _, h, w) in shapes_nchw):
-        return "nchw"
-    if 4 * 128 * (bins | 1) > 150 * 1024:
-        return "nchw"
-    if channels_last:
-        return "cl"
-    if POOLER_LAYOUT == "nhwc":
-        return "xpose"
-    i = 1 if bwd else 0
-    feat_bytes = 4 * sum(n * c * h * w for (n, c, h, w) in shapes_nchw)
-    return "xpose" if n_out * _ROT_NHWC_PS[i] + feat_bytes * _XPOSE_PS_PER_BYTE < n_out * _ROT_NCHW_PS[i] else "nchw"
-
-
+# ----------------------------------------------------------------------------------- rotated
 @torch.library.custom_op("d2b200::roi_align_rotated", mutates_args=(), device_types="cuda")
 def roi_align_rotated_op(input: Tensor, rois: Tensor, spatial_scale: float, pooled_h: int, pooled_w: int,
                          sampling_ratio: int) -> Tensor:
     _roi_common(input, rois, 6)
-    x, r = input.to(dtype=torch.float32), _f32c(rois)
-    n, c, h, w = x.shape
-    k = r.shape[0]
-    out = torch.empty((k, c, pooled_h, pooled_w), dtype=torch.float32, device=x.device)
-    if out.numel():
-        layout = _rot_layout(n, c, h, w, out.numel(), _is_channels_last(x) and x.data_ptr() % 16 == 0, False)
-        with torch.cuda.device(x.device):
-            if layout == "nchw":
-                x = x.contiguous()
-                check(_C.lib().d2b_roi_align_rotated_forward(ptr(x), n, c, h, w, ptr(r), k, spatial_scale, pooled_h,
-                                                             pooled_w, sampling_ratio, ptr(out), stream_ptr(x.device)),
-                      "roi_align_rotated_forward")
-            else:
-                if layout == "xpose":
-                    x = x.contiguous()
-                    x = _to_nhwc([x], _pyramid([x], None, [spatial_scale], 0, 0, 0, 1.0), n, c, x.device)[0]
-                check(_C.lib().d2b_roi_align_rotated_forward_nhwc(ptr(x), n, c, h, w, ptr(r), k, spatial_scale, pooled_h,
-                                                                  pooled_w, sampling_ratio, ptr(out),
-                                                                  stream_ptr(x.device)), "roi_align_rotated_forward_nhwc")
-    return out.to(input.dtype)
+    return _roi_forward([input], rois, [spatial_scale], pooled_h, pooled_w, sampling_ratio, _ONE_LEVEL, True)
 
 
 @roi_align_rotated_op.register_fake
@@ -420,22 +375,8 @@ def _(input, rois, spatial_scale, pooled_h, pooled_w, sampling_ratio):
 def roi_align_rotated_backward_op(grad: Tensor, rois: Tensor, spatial_scale: float, pooled_h: int, pooled_w: int,
                                   n: int, c: int, h: int, w: int, sampling_ratio: int,
                                   channels_last: bool = False) -> Tensor:
-    _C.require_cuda(grad, rois)
-    g, r = _f32c(grad), _f32c(rois)
-    layout = _rot_layout(n, c, h, w, g.numel(), channels_last, True) if n * c * h * w else "nchw"
-    with torch.cuda.device(g.device):
-        if layout == "nchw":
-            gin = torch.empty((n, c, h, w), dtype=torch.float32, device=g.device)
-            check(_C.lib().d2b_roi_align_rotated_backward(ptr(g), ptr(r), r.shape[0], spatial_scale, pooled_h, pooled_w,
-                                                          n, c, h, w, sampling_ratio, ptr(gin), stream_ptr(g.device)),
-                  "roi_align_rotated_backward")
-        else:
-            buf = torch.empty((n, h, w, c), dtype=torch.float32, device=g.device)
-            check(_C.lib().d2b_roi_align_rotated_backward_nhwc(ptr(g), ptr(r), r.shape[0], spatial_scale, pooled_h,
-                                                               pooled_w, n, c, h, w, sampling_ratio, ptr(buf),
-                                                               stream_ptr(g.device)), "roi_align_rotated_backward_nhwc")
-            gin = buf.permute(0, 3, 1, 2) if layout == "cl" else _from_nhwc([buf], n, c, g.device)[0]
-    return gin.to(grad.dtype)
+    return _one_level_backward(grad, rois, spatial_scale, pooled_h, pooled_w, n, c, h, w, sampling_ratio, True,
+                               channels_last)
 
 
 @roi_align_rotated_backward_op.register_fake
@@ -444,22 +385,6 @@ def _(grad, rois, spatial_scale, pooled_h, pooled_w, n, c, h, w, sampling_ratio,
     return out.contiguous(memory_format=torch.channels_last) if channels_last else out
 
 
-def _roi_rot_setup(ctx, inputs, output):
-    input, rois, spatial_scale, ph, pw, sr = inputs
-    ctx.save_for_backward(rois)
-    ctx.args = (spatial_scale, ph, pw, tuple(input.shape), sr, _is_channels_last(input))
-
-
-def _roi_rot_bwd(ctx, grad):
-    (rois,) = ctx.saved_tensors
-    scale, ph, pw, (n, c, h, w), sr, cl = ctx.args
-    return roi_align_rotated_backward_op(grad, rois, scale, ph, pw, n, c, h, w, sr, cl), None, None, None, None, None
-
-
-roi_align_rotated_op.register_autograd(_roi_rot_bwd, setup_context=_roi_rot_setup)
-
-
-# ----------------------------------------------------------------------------------- fused multi-level rotated pooler
 @torch.library.custom_op("d2b200::roi_pooler_rotated", mutates_args=(), device_types="cuda")
 def roi_pooler_rotated_op(feats: List[Tensor], rois: Tensor, scales: List[float], pooled_h: int, pooled_w: int,
                           sampling_ratio: int, min_level: int, max_level: int, canonical_level: int,
@@ -467,39 +392,10 @@ def roi_pooler_rotated_op(feats: List[Tensor], rois: Tensor, scales: List[float]
     """ROIPooler(pooler_type="ROIAlignRotated") over several levels in one launch: rois [K,6] = (batch, cx, cy, w, h, angle),
     the level of each from w*h.  The rois are used in fp32 whatever the feature dtype (layers/roi_align_rotated.py:81-83)."""
     _C.require_cuda(rois, *feats)
-    if len(feats) < 1 or len(feats) > _C.MAX_LEVELS or len(feats) != len(scales):
-        raise RuntimeError("roi_pooler_rotated: need 1..%d feature levels with one scale each" % _C.MAX_LEVELS)
+    _check_levels("roi_pooler_rotated", feats, scales)
     _roi_common(feats[0], rois, 6)
-    r = _f32c(rois)
-    n, c = feats[0].shape[:2]
-    k = r.shape[0]
-    numel = k * c * pooled_h * pooled_w
-    cl = all(_is_channels_last(t) and t.data_ptr() % 16 == 0 for t in feats)
-    layout = (_rot_pyramid_layout([(n, c, t.shape[2], t.shape[3]) for t in feats], numel, cl, False, pooled_h * pooled_w)
-              if numel else "nchw")
-    # half-precision NCHW levels: the layout-change launch reads them as they are (it is also the up-cast) and the pooling
-    # kernel writes the result in their dtype; every other combination computes on fp32 copies
-    fused_half = layout == "xpose" and _same_half_dtype(feats)
-    fs = list(feats) if fused_half else [t.to(dtype=torch.float32) for t in feats]
-    out_dt = feats[0].dtype if (layout != "nchw" and feats[0].dtype in _C.DTYPE_CODE) else torch.float32
-    out = torch.empty((k, c, pooled_h, pooled_w), dtype=out_dt, device=r.device)
-    if numel:
-        with torch.cuda.device(r.device):
-            if layout != "cl":
-                fs = [t.contiguous() for t in fs]
-            P = _pyramid(fs, None, scales, min_level, max_level, canonical_level, canonical_box_size)
-            if layout == "nchw":
-                check(_C.lib().d2b_roi_pooler_rotated_forward(C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w, sampling_ratio,
-                                                              ptr(out), stream_ptr(r.device)), "roi_pooler_rotated_forward")
-            else:
-                if layout == "xpose":
-                    bufs = _to_nhwc(fs, P, n, c, r.device)
-                    for l, b in enumerate(bufs):
-                        P.feat[l] = b.data_ptr()
-                check(_C.lib().d2b_roi_pooler_rotated_forward_nhwc_t(C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w,
-                                                                     sampling_ratio, ptr(out), _C.DTYPE_CODE[out_dt],
-                                                                     stream_ptr(r.device)), "roi_pooler_rotated_forward_nhwc")
-    return out if out.dtype == feats[0].dtype else out.to(feats[0].dtype)
+    return _roi_forward(feats, rois, scales, pooled_h, pooled_w, sampling_ratio,
+                        (min_level, max_level, canonical_level, canonical_box_size), True)
 
 
 @roi_pooler_rotated_op.register_fake
@@ -515,34 +411,9 @@ def roi_pooler_rotated_backward_op(grad: Tensor, rois: Tensor, shapes: List[int]
     """Gradients of roi_pooler_rotated for every level; shapes = [n, c, h0, w0, h1, w1, ...].  `half_grads`: return NCHW
     gradients in `grad`'s fp16 / bf16 dtype (written by the layout-change launch) instead of fp32."""
     _C.require_cuda(grad, rois)
-    r = _f32c(rois)
-    nl = len(scales)
-    n, c = shapes[0], shapes[1]
-    hw = [(shapes[2 + 2 * l], shapes[3 + 2 * l]) for l in range(nl)]
-    layout = (_rot_pyramid_layout([(n, c, h, w) for (h, w) in hw], grad.numel(), channels_last, True, pooled_h * pooled_w)
-              if n * c else "nchw")
-    # the channels-last kernel reads fp16 / bf16 gradients in place; the NCHW kernel takes fp32
-    g = grad.contiguous() if (layout != "nchw" and grad.dtype in _C.DTYPE_CODE) else _f32c(grad)
-    with torch.cuda.device(g.device):
-        if layout == "nchw":
-            grads = [torch.empty((n, c, h, w), dtype=torch.float32, device=g.device) for (h, w) in hw]
-            P = _pyramid(grads, grads, scales, min_level, max_level, canonical_level, canonical_box_size)
-            check(_C.lib().d2b_roi_pooler_rotated_backward(C.byref(P), n, c, ptr(g), ptr(r), r.shape[0], pooled_h, pooled_w,
-                                                           sampling_ratio, stream_ptr(g.device)), "roi_pooler_rotated_backward")
-        else:
-            bufs = [torch.empty((n, h, w, c), dtype=torch.float32, device=g.device) for (h, w) in hw]
-            views = [b.permute(0, 3, 1, 2) for b in bufs]  # logical NCHW shape: _pyramid reads H, W from dims 2, 3
-            P = _pyramid(views, views, scales, min_level, max_level, canonical_level, canonical_box_size)
-            check(_C.lib().d2b_roi_pooler_rotated_backward_nhwc_t(C.byref(P), n, c, ptr(g), _C.DTYPE_CODE[g.dtype], ptr(r),
-                                                                  r.shape[0], pooled_h, pooled_w, sampling_ratio,
-                                                                  stream_ptr(g.device)), "roi_pooler_rotated_backward_nhwc")
-            if layout == "cl":
-                grads = views
-            else:
-                grads = _from_nhwc(bufs, n, c, g.device, grad.dtype if (half_grads and grad.dtype in _HALF) else torch.float32)
-    if half_grads and grad.dtype in _HALF:
-        grads = [t if t.dtype == grad.dtype else t.to(grad.dtype) for t in grads]
-    return grads
+    return _roi_backward(grad, rois, shapes, scales, pooled_h, pooled_w, sampling_ratio,
+                         (min_level, max_level, canonical_level, canonical_box_size), True, channels_last,
+                         half_grads=half_grads)
 
 
 @roi_pooler_rotated_backward_op.register_fake
@@ -554,25 +425,10 @@ def _(grad, rois, shapes, scales, pooled_h, pooled_w, sampling_ratio, min_level,
     return [o.contiguous(memory_format=torch.channels_last) for o in outs] if channels_last else outs
 
 
-def _pooler_rot_setup(ctx, inputs, output):
-    feats, rois, scales, ph, pw, sr, lo, hi, cl, cs = inputs
-    ctx.save_for_backward(rois)
-    shapes = [feats[0].shape[0], feats[0].shape[1]]
-    for t in feats:
-        shapes += [t.shape[2], t.shape[3]]
-    ctx.args = (shapes, scales, ph, pw, sr, lo, hi, cl, cs, [t.dtype for t in feats],
-                all(_is_channels_last(t) for t in feats))
-
-
-def _pooler_rot_bwd(ctx, grad):
-    (rois,) = ctx.saved_tensors
-    shapes, scales, ph, pw, sr, lo, hi, cl, cs, dts, chl = ctx.args
-    half = dts[0] in _HALF and grad.dtype == dts[0] and all(d == dts[0] for d in dts)
-    grads = roi_pooler_rotated_backward_op(grad, rois, shapes, scales, ph, pw, sr, lo, hi, cl, cs, chl, half)
-    return [g.to(dt) for g, dt in zip(grads, dts)], None, None, None, None, None, None, None, None, None
-
-
-roi_pooler_rotated_op.register_autograd(_pooler_rot_bwd, setup_context=_pooler_rot_setup)
+_register_roi_autograd(roi_align_op, roi_align_backward_op, False)
+_register_roi_autograd(roi_pooler_op, roi_pooler_backward_op, False)
+_register_roi_autograd(roi_align_rotated_op, roi_align_rotated_backward_op, True)
+_register_roi_autograd(roi_pooler_rotated_op, roi_pooler_rotated_backward_op, True)
 
 
 # =================================================================================== NMS / rotated IoU

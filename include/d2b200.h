@@ -41,7 +41,11 @@ const char* d2b_arch(void); /* "sm_90a" */
  * Replaces torchvision::roi_align / torchvision::_roi_align_backward as reached from
  * detectron2/layers/roi_align.py:58-65 (forward) and its autograd (backward).
  * input [N,C,H,W] fp32, rois [K,5] = (batch_idx,x1,y1,x2,y2) fp32, out [K,C,PH,PW] fp32.
- * sampling_ratio <= 0 -> adaptive ceil(roi/pooled) grid.  aligned: 0/1. */
+ * sampling_ratio <= 0 -> adaptive ceil(roi/pooled) grid.  aligned: 0/1.
+ * Every single-level entry point (d2b_roi_align_* and d2b_roi_align_rotated_*, both layouts) is the pyramid entry point
+ * of the same kind and layout called with a one-level pyramid: feat[0] / grad[0] = input / grad_in, H[0], W[0],
+ * scale[0] = spatial_scale.  Same kernels, same results.  A forward with K == 0 or C == 0 returns D2B_OK before any other
+ * check; a backward with a valid but empty grad_in (N*C*H*W == 0) returns D2B_OK without a launch. */
 int d2b_roi_align_forward(const float* input, int N, int C, int H, int W, const float* rois, int K,
                           float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
                           int aligned, float* out, void* stream);
@@ -160,6 +164,15 @@ int d2b_roi_pooler_rotated_forward_nhwc_t(const d2b_pyramid* pyr, int N, int C, 
 int d2b_roi_pooler_rotated_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
                                            const float* rois, int K, int pooled_h, int pooled_w, int sampling_ratio,
                                            void* stream);
+
+/* Which shapes the channels-last kernels take: D2B_OK, or D2B_EUNSUPPORTED where the channels-last entry points above
+ * (d2b_roi_align_*_nhwc, d2b_roi_pooler_*_nhwc[_t], d2b_roi_pooler_rotated_*_nhwc_t) return D2B_EUNSUPPORTED -- use the NCHW
+ * form then.  The launchers of those entry points ask the same function, so the answer cannot disagree with them.  Reads
+ * pyr->num_levels, H[] and W[] only: pointer alignment stays the caller's check.  Host-only, no CUDA call (safe during graph
+ * capture).  flags: D2B_ROI_ROTATED for the rotated kernels, | D2B_ROI_BACKWARD for the backward. */
+#define D2B_ROI_ROTATED 1
+#define D2B_ROI_BACKWARD 2
+int d2b_roi_pooler_nhwc_supported(const d2b_pyramid* pyr, int C, int pooled_h, int pooled_w, int flags);
 
 /* ---- NMS --------------------------------------------------------------------------------
  * Replaces torchvision::nms reached from detectron2/layers/nms.py:5-22 (nms, batched_nms) and

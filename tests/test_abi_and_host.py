@@ -142,6 +142,86 @@ def test_pooler_layout_policy_host_logic(monkeypatch):
         ops.pyramid_to_channels_last(nchw)
 
 
+def test_channels_last_limits_and_single_level_entry_points_without_a_gpu(monkeypatch):
+    """d2b_roi_pooler_nhwc_supported is the one statement of the channels-last kernels' shape limits; the layout chooser
+    sends every shape it refuses to the NCHW kernels.  The single-level entry points are one-level pyramid calls with the
+    status codes they always had.  Every call here returns before any CUDA call."""
+    import ctypes as C
+
+    from detectron2_b200 import _C, ops
+
+    lib = _C.lib()
+    EINVAL, UNSUPPORTED = -1, -3
+    ROT, BWD = _C.ROI_ROTATED, _C.ROI_BACKWARD
+
+    def pyr(hw):
+        P = _C.Pyramid()
+        P.num_levels = len(hw)
+        for l, (h, w) in enumerate(hw):
+            P.H[l], P.W[l] = h, w
+        return P
+
+    bench = pyr([(200 // 2 ** l, 336 // 2 ** l) for l in range(4)])  # bench.py's 800x1333 pyramid
+    q = lambda P, c, ph, pw, flags: lib.d2b_roi_pooler_nhwc_supported(C.byref(P), c, ph, pw, flags)  # noqa: E731
+    for flags in (0, BWD, ROT, ROT | BWD):
+        assert q(bench, 256, 7, 7, flags) == 0 and q(bench, 256, 14, 14, flags) == 0, flags
+        assert q(bench, 6, 7, 7, flags) == UNSUPPORTED, flags                         # C % 4 != 0
+        assert q(pyr([(16384, 16384)]), 4, 7, 7, flags) == UNSUPPORTED, flags        # H*W*C/4 >= 2^28
+    assert q(bench, 256, 32, 32, BWD) == UNSUPPORTED and q(bench, 256, 7, 40, BWD) == UNSUPPORTED  # backward tile > 180 KB
+    assert q(bench, 256, 32, 32, 0) == 0                                           # ... the forward takes them
+    assert q(bench, 256, 20, 20, ROT) == UNSUPPORTED and q(bench, 256, 20, 20, ROT | BWD) == UNSUPPORTED  # tile > 150 KB
+    assert lib.d2b_roi_pooler_nhwc_supported(None, 256, 7, 7, 0) == EINVAL
+
+    # the two calls the channels-last kernels refuse go to the NCHW kernels: ROIAlign((32, 32)) backward, single-level
+    # ROIAlignRotated((20, 20)) forward and backward -- channels-last inputs, and NCHW inputs under D2B_POOLER_LAYOUT=nhwc
+    x = torch.zeros(2, 256, 50, 84)
+    xcl = x.contiguous(memory_format=torch.channels_last)
+    monkeypatch.setattr(ops, "POOLER_LAYOUT", "auto")
+    assert ops._pick_layout([xcl], 10 ** 6, (32, 32)) == "cl"
+    assert ops._pick_layout([tuple(x.shape)], 10 ** 6, (32, 32), backward=True, channels_last=True) == "nchw"
+    assert ops._pick_layout([xcl], 10 ** 6, (20, 20), rotated=True) == "nchw"
+    assert ops._pick_layout([tuple(x.shape)], 10 ** 6, (20, 20), rotated=True, backward=True, channels_last=True) == "nchw"
+    monkeypatch.setattr(ops, "POOLER_LAYOUT", "nhwc")
+    assert ops._pick_layout([x], 1, (32, 32)) == "xpose"
+    assert ops._pick_layout([tuple(x.shape)], 1, (32, 32), backward=True, channels_last=False) == "nchw"
+    assert ops._pick_layout([x], 1, (20, 20), rotated=True) == "nchw"
+    assert ops._pick_layout([tuple(x.shape)], 1, (20, 20), rotated=True, backward=True, channels_last=False) == "nchw"
+
+    # single-level entry points (the pointers are never dereferenced: each call below fails or returns before a launch).
+    # Forwards: (input, N, C, H, W, rois, K, scale, PH, PW, sr[, aligned], out, stream), in the order
+    # axis-aligned NCHW, axis-aligned channels-last, rotated NCHW, rotated channels-last.
+    def fwd(which=range(4), inp=0x1000, n=2, c=8, h=16, w=16, rois=0x2000, k=3, ph=7, pw=7, out=0x3000):
+        calls = (lambda: lib.d2b_roi_align_forward(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, 1, out, None),
+                 lambda: lib.d2b_roi_align_forward_nhwc(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, 1, out, None),
+                 lambda: lib.d2b_roi_align_rotated_forward(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, out, None),
+                 lambda: lib.d2b_roi_align_rotated_forward_nhwc(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, out, None))
+        return tuple(calls[i]() for i in which)
+
+    assert fwd(k=0) == fwd(c=0) == fwd(k=0, n=-1, inp=None) == (0, 0, 0, 0)  # nothing to compute: before any check
+    for bad in (dict(inp=None), dict(rois=None), dict(out=None), dict(n=0), dict(h=0), dict(w=-1), dict(ph=0), dict(k=-2)):
+        assert fwd(**bad) == (EINVAL,) * 4, bad
+    assert fwd((1, 3), inp=0x1004) == (EINVAL, EINVAL)          # the channels-last forms need a 16-byte aligned map
+    assert fwd((1, 3), c=6) == (UNSUPPORTED, UNSUPPORTED)
+    assert fwd((3,), ph=20, pw=20) == (UNSUPPORTED,)
+
+    # Backwards: (grad_out, rois, K, scale, PH, PW, N, C, H, W, sr[, aligned], grad_in, stream), same order.  A backward
+    # with a non-empty gradient and valid arguments zero-fills it, so only the empty and the invalid cases are called here.
+    def bwd(which=range(4), go=0x1000, rois=0x2000, k=3, ph=7, pw=7, n=2, c=8, h=16, w=16, gin=0x3000):
+        calls = (lambda: lib.d2b_roi_align_backward(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, 1, gin, None),
+                 lambda: lib.d2b_roi_align_backward_nhwc(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, 1, gin, None),
+                 lambda: lib.d2b_roi_align_rotated_backward(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, gin, None),
+                 lambda: lib.d2b_roi_align_rotated_backward_nhwc(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, gin, None))
+        return tuple(calls[i]() for i in which)
+
+    for bad in (dict(gin=None), dict(n=-1), dict(c=-4), dict(h=-1), dict(w=-3)):
+        assert bwd(**bad) == (EINVAL,) * 4, bad
+    assert bwd(h=0) == bwd(n=0) == bwd(c=0, go=None) == (0, 0, 0, 0)  # empty gradient: nothing to write
+    assert bwd((3,), gin=0x3004) == bwd((3,), gin=0x3004, h=0) == (EINVAL,)
+    # the rotated backwards check their arguments before the zero-fill launch
+    assert bwd((2, 3), go=None) == bwd((2, 3), rois=None) == bwd((2, 3), ph=0) == (EINVAL, EINVAL)
+    assert bwd((3,), c=6) == bwd((3,), ph=20, pw=20) == (UNSUPPORTED,)
+
+
 def test_roi_pooler_no_images():  # /root/reference/tests/modeling/test_roi_pooler.py:107-115
     from detectron2_b200.poolers import ROIPooler
 

@@ -119,10 +119,11 @@ def test_roi_align_rotated_golden(L, golden):
 
 
 @pytest.mark.parametrize("layout", ["nchw", "nhwc", "cl"])
-@pytest.mark.parametrize("c,ph,pw,sr", [(132, 7, 7, 0), (64, 14, 14, 2), (8, 17, 5, 0)])
+@pytest.mark.parametrize("c,ph,pw,sr", [(132, 7, 7, 0), (64, 14, 14, 2), (8, 17, 5, 0), (32, 20, 20, 0)])
 def test_roi_align_rotated_layouts_vs_oracle(L, layout, c, ph, pw, sr, monkeypatch):
     # rotated RoIAlign: NCHW kernels, channels-last kernels via layout change, channels-last in place -- fwd and bwd.
-    # (17, 5) with adaptive sampling exceeds the shared tap table: taps on the fly.
+    # (17, 5) with adaptive sampling exceeds the shared tap table: taps on the fly.  (20, 20) is beyond the channels-last
+    # kernels' shared-memory tile: every layout runs the NCHW kernels.
     from detectron2_b200 import ops
 
     g = torch.Generator().manual_seed(c + ph + sr)
@@ -638,9 +639,11 @@ def test_pyramid_layout_change_is_exact():
 
 
 @pytest.mark.parametrize("c,ph,pw,sr,aligned", [(4, 7, 7, 0, True), (12, 7, 7, 2, False), (132, 7, 7, 0, True),
-                                                 (256, 14, 14, 0, True), (8, 17, 5, 0, True), (64, 3, 9, 3, False)])
+                                                 (256, 14, 14, 0, True), (8, 17, 5, 0, True), (64, 3, 9, 3, False),
+                                                 (8, 32, 32, 0, True)])
 def test_roi_align_channels_last_vs_oracle(L, c, ph, pw, sr, aligned):
-    # channels_last input is consumed in place (no NCHW copy); (17, 5) exercises the taps-on-the-fly path (pooled > 16)
+    # channels_last input is consumed in place (no NCHW copy); (17, 5) exercises the taps-on-the-fly path (pooled > 16);
+    # the backward of (32, 32) is beyond the channels-last kernel's shared-memory tile and runs the NCHW kernel
     g = torch.Generator().manual_seed(c + ph)
     x = torch.randn(2, c, 50, 76, generator=g)
     rois = _rand_rois(g, 97, 2, 304.0, 200.0, 4.0, 180.0)

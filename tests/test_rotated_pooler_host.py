@@ -75,15 +75,18 @@ def test_rotated_pooler_entry_points_validate_arguments_without_a_gpu():
     assert lib.d2b_roi_pooler_rotated_backward_nhwc_t(C.byref(_pyr()), 2, 6, 0x10, 0, 0x20, 3, 7, 7, 0, None) == -3
 
 
-def test_rotated_pooler_layout_falls_back_to_nchw_for_large_pooled_sizes(monkeypatch):
+def test_layout_chooser_sends_large_rotated_pooled_sizes_to_nchw(monkeypatch):
+    """The one RoIAlign layout chooser, for rotated pyramids: shapes beyond the channels-last kernels' shared-memory tile
+    (d2b_roi_pooler_nhwc_supported) go to the NCHW kernels whatever D2B_POOLER_LAYOUT says."""
     from detectron2_b200 import ops
 
     monkeypatch.setattr(ops, "POOLER_LAYOUT", "nhwc")
     shapes = [(2, 256, 200 // 2 ** l, 336 // 2 ** l) for l in range(4)]
-    assert ops._rot_pyramid_layout(shapes, 10, False, False, 7 * 7) == "xpose"
-    assert ops._rot_pyramid_layout(shapes, 10, True, True, 14 * 14) == "cl"
-    assert ops._rot_pyramid_layout(shapes, 10, True, False, 20 * 20) == "nchw"  # [128][400] fp32 tile > 150 KB
-    assert ops._rot_pyramid_layout(shapes, 10, False, True, 20 * 20) == "nchw"
+    assert ops._pick_layout(shapes, 10, (7, 7), rotated=True, backward=False, channels_last=False) == "xpose"
+    assert ops._pick_layout(shapes, 10, (14, 14), rotated=True, backward=True, channels_last=True) == "cl"
+    # [128][400] fp32 tile > 150 KB
+    assert ops._pick_layout(shapes, 10, (20, 20), rotated=True, backward=False, channels_last=True) == "nchw"
+    assert ops._pick_layout(shapes, 10, (20, 20), rotated=True, backward=True, channels_last=False) == "nchw"
 
 
 def test_assign_boxes_to_levels_rotated_area_is_w_times_h():
