@@ -24,11 +24,22 @@ def make_tap1(v, size):  # roi_align.cu make_tap1 / torchvision bilinear_interpo
     return lo, hi, 1.0 - frac, frac
 
 
-def tap_list(start, bin_size, grid, p, size):
-    """add_tap: the (index, weight) list of bin p along one axis, samples merged per index."""
+def sample_pos(start, bin_size, grid, p, i, fp32=False):
+    """Position of sample i of bin p along one axis; fp32: as the kernels compute it (start, bin_size fp32 values from
+    load_geom), start + p*bin + ((i + .5)*bin)/grid rounded after every operation."""
+    if not fp32:
+        return start + p * bin_size + (i + 0.5) * bin_size / grid
+    f = np.float32
+    s, b = f(start), f(bin_size)
+    return float((s + f(p) * b) + (f(i) + f(0.5)) * b / f(grid))
+
+
+def tap_list(start, bin_size, grid, p, size, fp32=False):
+    """add_tap: the (index, weight) list of bin p along one axis, samples merged per index.  fp32: sample positions in fp32
+    (sample_pos), weights and their sums in float64."""
     lst = []
     for i in range(grid):
-        lo, hi, wl, wh = make_tap1(start + p * bin_size + (i + 0.5) * bin_size / grid, size)
+        lo, hi, wl, wh = make_tap1(sample_pos(start, bin_size, grid, p, i, fp32), size)
         for idx, w in ((lo, wl), (hi, wh)):
             if w == 0:
                 continue
