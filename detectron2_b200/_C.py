@@ -51,6 +51,7 @@ class DenseLevels(C.Structure):
 
 
 LABELS_I8, LABELS_I64 = 0, 1  # D2B_LABELS_*
+SAMPLE_MAX_SAMPLES = 8192  # D2B_SAMPLE_MAX_SAMPLES
 LOSS_STATUS_INVALID_BOX, LOSS_STATUS_INVALID_CLASS, LOSS_STATUS_INVALID_BOX_ORDER = 1, 2, 4  # D2B_LOSS_STATUS_*
 LOSS_TYPES = {"smooth_l1": 0, "giou": 1}  # D2B_LOSS_SMOOTH_L1 / D2B_LOSS_GIOU
 
@@ -123,6 +124,8 @@ def _declare(lib):
         "d2b_match_workspace_bytes": (sz, [i, i, i]),
         "d2b_match_boxes": (i, [f32p, i64p, i, i, f32p, i64, i64p, i, C.POINTER(C.c_double), i, C.POINTER(C.c_int), i, f32p, d,
                                 i64p, i64, i64p, vp, f32p, i64p, vp, vp, sz, vp]),
+        "d2b_sample_labels_workspace_bytes": (sz, [i, i, i]),
+        "d2b_sample_labels": (i, [vp, i, i, i, i64, i, i, vp, vp, i64p, i64p, i64p, vp, sz, vp]),
         "d2b_deform_conv_tc_shape_supported": (i, [C.POINTER(DcnParams), i]),
         "d2b_deform_conv_forward_workspace_bytes": (sz, [C.POINTER(DcnParams), i, i]),
         "d2b_deform_conv_cols_bytes": (sz, [C.POINTER(DcnParams), i]),

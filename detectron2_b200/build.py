@@ -25,6 +25,7 @@ SOURCES = {
     "nms.cu": ["-fmad=false"],
     "postproc.cu": ["-fmad=false"],
     "match.cu": ["-fmad=false"],
+    "sampling.cu": [],
     "keypoints.cu": ["-fmad=false"],
     "losses.cu": ["-fmad=false"],
     "deform_conv.cu": [],

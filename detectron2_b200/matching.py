@@ -12,7 +12,10 @@ images go through ONE `d2b_match_boxes` (a zero-fill launch and two kernels, no 
     in a CUDA graph;
   * the reference-shaped wrappers make one host read (the per-image status: the reference's AssertionError) and then run
     the reference's own `subsample_labels` per image, in the reference's order, so that under the same seed they consume
-    the same random numbers and sample the same indices.
+    the same random numbers and sample the same indices;
+  * `rpn_label_and_sample_anchors_fixed` / `label_and_sample_proposals_fixed` follow `match_boxes_fixed` with ONE
+    `d2b_sample_labels` for all images (sampling.py): no host read from matching to loss, capturable in a CUDA graph, the
+    reference's sampling law but not its random stream.
 
 The box width selects the box type: 4 = (x1, y1, x2, y2), 5 = rotated (cx, cy, w, h, angle_deg).  CPU tensors take the
 host restatement below (`Matcher`, `pairwise_iou`; the rotated IoU is `ops.box_iou_rotated_op`).
@@ -25,7 +28,7 @@ from . import ops
 
 __all__ = ["Matcher", "pairwise_iou", "pairwise_iou_rotated", "subsample_labels", "match_boxes_fixed",
            "rpn_label_and_sample_anchors", "retinanet_label_anchors", "label_and_sample_proposals",
-           "cascade_match_and_label_boxes"]
+           "cascade_match_and_label_boxes", "rpn_label_and_sample_anchors_fixed", "label_and_sample_proposals_fixed"]
 
 
 # ----------------------------------------------------------------------------------------------- host restatement
@@ -207,6 +210,71 @@ def match_boxes_fixed(gt_boxes: torch.Tensor, gt_count: torch.Tensor, pred_boxes
                                        ptr(labels), ptr(out_boxes), ptr(classes), ptr(status), ptr(ws), ws_bytes,
                                        stream_ptr(device)), "match_boxes")
     return matches, labels, out_boxes, classes, status
+
+
+def rpn_label_and_sample_anchors_fixed(anchors, gt_boxes: torch.Tensor, gt_count: torch.Tensor, matcher: Matcher,
+                                       batch_size_per_image: int, positive_fraction: float, *, image_hw=None,
+                                       boundary_thresh: float = -1.0, seed: Optional[torch.Tensor] = None):
+    """RPN / RRPN.label_and_sample_anchors for all images with no host read (CUDA only, capturable in a CUDA graph):
+    match_boxes_fixed, then ONE d2b_sample_labels in the RPN form instead of the per-image _subsample_labels.
+    anchors [A, D] (or per-level list), gt_boxes [N, Gmax, D] with gt_count [N]; image_hw [N, 2] and boundary_thresh >= 0:
+    the anchor boundary rule (axis-aligned only, as RRPN).  seed: [1] int64 device tensor (None: torch's CUDA generator).
+    Returns (gt_labels [N, A] int8: 1 / 0 / -1, matched_gt_boxes [N, A, D], zeros for an image without GT), the inputs of
+    losses.rpn_losses_fixed.  The sample follows the reference's law, not its randperm stream (sampling.py)."""
+    from .sampling import sample_labels
+
+    if isinstance(anchors, (list, tuple)):
+        anchors = torch.cat(list(anchors), dim=0)
+    if anchors.shape[-1] == 5 and boundary_thresh >= 0:  # as RRPN.__init__ (proposal_generator/rrpn.py:139-142)
+        raise NotImplementedError("anchor_boundary_thresh is a legacy option not implemented for RRPN.")
+    _, labels, boxes, _, _ = match_boxes_fixed(gt_boxes, gt_count, anchors, matcher, image_hw=image_hw,
+                                               boundary_thresh=boundary_thresh)
+    gt_labels, _, _ = sample_labels(labels, batch_size_per_image, positive_fraction, 0, seed=seed, rpn_labels=True)
+    return gt_labels, boxes
+
+
+def label_and_sample_proposals_fixed(proposals: torch.Tensor, proposal_count: Optional[torch.Tensor],
+                                     gt_boxes: torch.Tensor, gt_count: torch.Tensor, gt_classes: torch.Tensor,
+                                     matcher: Matcher, num_classes: int, batch_size_per_image: int,
+                                     positive_fraction: float, *, proposal_append_gt: bool = True,
+                                     seed: Optional[torch.Tensor] = None):
+    """(R)ROIHeads.label_and_sample_proposals for all images with no host read (CUDA only, capturable in a CUDA graph):
+    match_boxes_fixed, then ONE d2b_sample_labels on the classes instead of the per-image _sample_proposals.
+    proposals [N, Pmax, D] with proposal_count [N] (device int64; None: all Pmax rows), gt_boxes [N, Gmax, D] with
+    gt_count [N], gt_classes [N, Gmax] int64.  Returns (sampled_idx, gt_classes, matched_idx, proposal_boxes, gt_boxes,
+    num_fg, num_bg), [N, B] unless noted, B = batch_size_per_image:
+      sampled_idx    rows of the image's proposals ++ GT (GT row g at proposal_count[n] + g, match_boxes_fixed's layout);
+      gt_classes     their classes (num_classes = background), matched_idx their matched GT (argmax over GT);
+      proposal_boxes [N, B, D] the sampled rows' boxes, gt_boxes [N, B, D] their matched GT boxes (zeros without GT);
+      num_fg, num_bg [N]: the sampled counts.  Foreground rows are the first num_fg[n] of each image's block.
+    Rows past num_fg + num_bg are padding: index, class and match -1, NaN proposal box (ROIPooler pools it to zeros with no
+    gradient), zero GT box.  The sample follows the reference's law, not its randperm stream (sampling.py)."""
+    from .sampling import sample_labels
+
+    matches, _, boxes, classes, _ = match_boxes_fixed(gt_boxes, gt_count, proposals, matcher, pred_count=proposal_count,
+                                                      append_gt=proposal_append_gt, gt_classes=gt_classes,
+                                                      num_classes=num_classes)
+    sampled, num_fg, num_bg = sample_labels(classes, batch_size_per_image, positive_fraction, num_classes, seed=seed)
+    n, pmax, d = proposals.shape
+    if classes.shape[1] == 0:  # no rows to sample from: every sample row is padding (keeps the gathers in bounds)
+        classes, matches, boxes = classes.new_full((n, 1), -1), matches.new_zeros((n, 1)), boxes.new_zeros((n, 1, d))
+    valid = sampled >= 0
+    idx = sampled.clamp(min=0)
+    # the sampled row's source: proposal p < proposal_count, else GT p - proposal_count (rows of cat([proposals, gt]))
+    if proposal_append_gt:
+        pc = (proposal_count.to(torch.int64) if proposal_count is not None
+              else torch.full((n,), pmax, dtype=torch.int64, device=proposals.device)).clamp(0, pmax)[:, None]
+        src = torch.where(idx < pc, idx, pmax + idx - pc)
+        rows = torch.cat([proposals.float(), gt_boxes.float()], dim=1)
+    else:
+        src, rows = idx, proposals.float()
+    if rows.shape[1] == 0:  # nothing to sample from: every row is padding
+        rows = rows.new_zeros((n, 1, d))
+    src = src.clamp(max=rows.shape[1] - 1)
+    prop = torch.where(valid[..., None], rows.gather(1, src[..., None].expand(-1, -1, d)), float("nan"))
+    gtb = torch.where(valid[..., None], boxes.gather(1, idx[..., None].expand(-1, -1, d)), 0.0)
+    return (sampled, torch.where(valid, classes.gather(1, idx), -1), torch.where(valid, matches.gather(1, idx), -1), prop,
+            gtb, num_fg, num_bg)
 
 
 def _fused(gt_boxes_list, preds, matcher, **kw):

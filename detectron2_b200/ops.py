@@ -489,6 +489,45 @@ def _(boxes1, boxes2):
     return boxes1.new_empty((boxes1.shape[0], boxes2.shape[0]), dtype=torch.float32)
 
 
+# =================================================================================== label sampling
+@torch.library.custom_op("d2b200::sample_labels", mutates_args=(), device_types="cuda")
+def sample_labels_op(labels: Tensor, num_samples: int, max_pos: int, bg_label: int, seed: Tensor, want_labels: bool,
+                     want_sampled: bool) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+    """d2b_sample_labels on labels [N, P] (int8 read as int8, any other integer type as int64) with seed [1] int64 (its
+    64 bits are the SplitMix64 seed).  Returns (out_labels [N, P] int8 in the RPN form, sampled [N, num_samples] int64,
+    num_pos [N] int64, num_neg [N] int64); an output not asked for is an empty tensor."""
+    _C.require_cuda(labels, seed)
+    if labels.dim() != 2 or seed.dtype != torch.int64 or seed.numel() != 1:
+        raise ValueError("sample_labels: labels [N, P] and seed [1] int64")
+    dev = labels.device
+    kind = _C.LABELS_I8 if labels.dtype == torch.int8 else _C.LABELS_I64
+    lab = labels.contiguous() if kind == _C.LABELS_I8 else labels.to(torch.int64).contiguous()
+    n, p = lab.shape
+    sd = seed.to(dev).contiguous()
+    out_labels = torch.empty((n, p) if want_labels else (0,), dtype=torch.int8, device=dev)
+    sampled = torch.empty((n, num_samples) if want_sampled else (0,), dtype=torch.int64, device=dev)
+    num_pos = torch.zeros((n,), dtype=torch.int64, device=dev)
+    num_neg = torch.zeros((n,), dtype=torch.int64, device=dev)
+    if out_labels.numel() or sampled.numel():  # else num_samples or P is 0: nothing is sampled, the counts are 0
+        lib = _C.lib()
+        ws_bytes = int(lib.d2b_sample_labels_workspace_bytes(n, p, num_samples))
+        ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            check(lib.d2b_sample_labels(ptr(lab), kind, n, p, int(bg_label), int(num_samples), int(max_pos), ptr(sd),
+                                        ptr(out_labels) if want_labels else None, ptr(sampled) if want_sampled else None,
+                                        ptr(num_pos), ptr(num_neg), ptr(ws), ws_bytes, stream_ptr(dev)), "sample_labels")
+    return out_labels, sampled, num_pos, num_neg
+
+
+@sample_labels_op.register_fake
+def _(labels, num_samples, max_pos, bg_label, seed, want_labels, want_sampled):
+    n, p = labels.shape
+    e = labels.new_empty
+    return (e((n, p) if want_labels else (0,), dtype=torch.int8),
+            e((n, num_samples) if want_sampled else (0,), dtype=torch.int64), e((n,), dtype=torch.int64),
+            e((n,), dtype=torch.int64))
+
+
 # =================================================================================== deformable conv
 def _dcn_params(x, weight, stride, padding, dilation, groups, deformable_groups):
     n, cin, h, w = x.shape

@@ -338,6 +338,32 @@ int d2b_match_boxes(const float* gt_boxes, const int64_t* gt_count, int N, int G
                     float* matched_gt_boxes, int64_t* classes, int* status, void* workspace, size_t workspace_bytes,
                     void* stream);
 
+/* ---- Sampling of the training labels --------------------------------------------------------------------------------
+ * Replaces subsample_labels (modeling/sampling.py:9-54) and the per-image loops around it in RPN._subsample_labels
+ * (proposal_generator/rpn.py:286-303, rrpn.py:184) and ROIHeads._sample_proposals (roi_heads/roi_heads.py:181-217,
+ * rotated_fast_rcnn.py:218-270), for all images at once, without the reference's nonzero() host syncs.
+ *   labels [N,P] of label_kind (D2B_LABELS_I8: int8, e.g. the match_labels of d2b_match_boxes; D2B_LABELS_I64: int64, e.g.
+ *   its classes).  Per image: positive = label != -1 && label != bg_label, negative = label == bg_label (padding rows, label
+ *   -1, are never sampled).  max_pos = int(num_samples * positive_fraction), computed by the caller (HOST, sampling.py:41);
+ *   k_pos = min(#pos, max_pos), k_neg = min(#neg, num_samples - k_pos).
+ *   Keys: mix = the SplitMix64 finaliser, arithmetic mod 2^64; s_n = mix(*seed + (n+1) * 0xD1B54A32D192ED03),
+ *   key(n, i) = mix(s_n + (i+1) * 0x9E3779B97F4A7C15).  The sample is the k_pos smallest-key positives, then the k_neg
+ *   smallest-key negatives, each in ascending key order (unsigned compare): the reference's law (a uniform random subset
+ *   in uniform random order), not torch.randperm's random stream.  seed: one uint64 in device memory.
+ * Outputs (NULL-able, not both NULL): out_labels [N,P] int8 in the RPN form (1 sampled positive, 0 sampled negative, -1
+ *   otherwise; must not alias labels); sampled [N,num_samples] int64: the k_pos positive indices, then the k_neg negative
+ *   ones, then -1.  num_pos / num_neg [N] int64 (device): k_pos, k_neg.
+ * 0 <= num_samples <= D2B_SAMPLE_MAX_SAMPLES, 0 <= max_pos <= num_samples, N <= 65535.  workspace:
+ *   d2b_sample_labels_workspace_bytes(N, P, num_samples) bytes, 256-byte aligned, no initialisation needed.
+ * Exact for every input (a radix select on the keys, refined until the threshold bin fits its buffer).  Five launches on
+ * `stream`, no allocation, no host synchronisation: capturable in a CUDA graph.  All arguments are checked before the first
+ * CUDA call. */
+#define D2B_SAMPLE_MAX_SAMPLES 8192
+size_t d2b_sample_labels_workspace_bytes(int N, int P, int num_samples);
+int d2b_sample_labels(const void* labels, int label_kind, int N, int P, int64_t bg_label, int num_samples, int max_pos,
+                      const uint64_t* seed, int8_t* out_labels, int64_t* sampled, int64_t* num_pos, int64_t* num_neg,
+                      void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- Mask-head training targets + loss (SURVEY 8f-4) ------------------------------------------------------
  * Replaces, for one image, BitMasks.crop_and_resize (detectron2/structures/masks.py:193-224) + the class gather and
  * binary_cross_entropy_with_logits of mask_rcnn_loss (modeling/roi_heads/mask_head.py:60-112).
