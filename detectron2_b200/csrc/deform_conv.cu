@@ -18,6 +18,7 @@
 // The wgmma (bf16 / bf16x3) forward and backward live in deform_conv_tc.cu; this file is the fp32 FFMA path used for
 // parity (<= 1e-4 rel) and for shapes the tensor-core kernels do not take, plus the public entry points that pick one.
 #include "common.cuh"
+#include "deform_conv_tc.cuh"
 
 namespace {
 
@@ -371,20 +372,6 @@ __global__ void __launch_bounds__(256) dcn_bias_grad_kernel(const float* __restr
 }
 
 }  // namespace
-
-int d2b_deform_conv_tc_supported(const d2b_dcn_params* p);
-int d2b_deform_conv_tc_bwd_supported(const d2b_dcn_params* p);
-size_t d2b_deform_conv_tc_fwd_workspace(const d2b_dcn_params* p, int x_nhwc);
-size_t d2b_deform_conv_tc_cols_bytes(const d2b_dcn_params* p, int precision);
-int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float* mask, const float* weight,
-                               const float* scale, const float* shift, int relu, const d2b_dcn_params* p, int precision,
-                               int tcflags, float* out, void* cols, void* workspace, size_t workspace_bytes, void* stream);
-size_t d2b_deform_conv_tc_bwd_workspace(const d2b_dcn_params* p, int x_nhwc, int need_data, int need_weight);
-int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float* mask, const float* weight,
-                                const float* grad_out, const float* scale, const float* y_saved, int relu,
-                                const d2b_dcn_params* p, int precision, int tcflags, const void* cols, float* grad_x,
-                                float* grad_offset, float* grad_mask, float* grad_weight, void* workspace,
-                                size_t workspace_bytes, void* stream);
 
 // precision: 0 = fp32 FFMA, 1 = bf16x3 on wgmma, 2 = bf16 on wgmma, -1 = auto (1 when the tensor-core kernels take
 // the shape, else 0 -- both are fp32-class, so "auto" never lowers accuracy)

@@ -32,6 +32,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "deform_conv_tc.cuh"
 #include "tc_common.cuh"
 
 using namespace d2b_tc;
@@ -1300,7 +1301,7 @@ int to_nhwc(const float* x, const TC& d, float* dst, cudaStream_t stream) {
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ host entry points
-// (internal linkage across the library: declared again in deform_conv.cu)
+// (library-internal, declared in deform_conv_tc.cuh for deform_conv.cu)
 int d2b_deform_conv_tc_supported(const d2b_dcn_params* p) {
   TC d;
   K1P k1;

@@ -112,9 +112,66 @@ def test_fake_kernels_trace_shapes():
         off = torch.empty(2, 18, 10, 15, device="cuda")
         out = ops.deform_conv_op(x, off, None, w, None, [2, 2], [1, 1], [1, 1], 2, 1, -1)
         assert out.shape == (2, 24, 10, 15)
+        _check_dcn_fakes(ops, x, w, off)
         assert ops.box_iou_rotated_op(torch.empty(5, 5, device="cuda"), torch.empty(9, 5, device="cuda")).shape == (5, 9)
         pm = ops.paste_masks_op(torch.empty(3, 28, 28, device="cuda"), torch.empty(3, 4, device="cuda"), 40, 50, 0.5)
         assert pm.shape == (3, 40, 50) and pm.dtype == torch.bool  # threshold >= 0: bool output like the reference
+
+
+_DCN_SCHEMAS = {
+    "deform_conv": "d2b200::deform_conv(Tensor x, Tensor offset, Tensor? mask, Tensor weight, Tensor? bias, SymInt[] stride, "
+                   "SymInt[] padding, SymInt[] dilation, SymInt groups, SymInt deformable_groups, SymInt precision) -> Tensor",
+    "deform_conv_train": "d2b200::deform_conv_train(Tensor x, Tensor offset, Tensor? mask, Tensor weight, Tensor? bias, "
+                         "SymInt[] stride, SymInt[] padding, SymInt[] dilation, SymInt groups, SymInt deformable_groups, "
+                         "SymInt precision) -> (Tensor, Tensor, Tensor)",
+    "deform_conv_backward": "d2b200::deform_conv_backward(Tensor x, Tensor offset, Tensor? mask, Tensor weight, "
+                            "Tensor grad_out, SymInt[] stride, SymInt[] padding, SymInt[] dilation, SymInt groups, "
+                            "SymInt deformable_groups, bool with_bias, bool need_data, bool need_weight, SymInt precision, "
+                            "Tensor? cols=None) -> (Tensor, Tensor, Tensor, Tensor, Tensor)",
+    "deform_conv_fused": "d2b200::deform_conv_fused(Tensor x, Tensor offset_mask, Tensor weight, Tensor? scale, "
+                         "Tensor? shift, bool relu, SymInt[] stride, SymInt[] padding, SymInt[] dilation, SymInt groups, "
+                         "SymInt deformable_groups, SymInt precision) -> Tensor",
+    "deform_conv_fused_train": "d2b200::deform_conv_fused_train(Tensor x, Tensor offset_mask, Tensor weight, Tensor? scale, "
+                               "Tensor? shift, bool relu, SymInt[] stride, SymInt[] padding, SymInt[] dilation, "
+                               "SymInt groups, SymInt deformable_groups, SymInt precision) -> (Tensor, Tensor, Tensor)",
+    "deform_conv_fused_backward": "d2b200::deform_conv_fused_backward(Tensor x, Tensor offset_mask, Tensor weight, "
+                                  "Tensor? scale, bool relu, Tensor y, Tensor grad_out, SymInt[] stride, SymInt[] padding, "
+                                  "SymInt[] dilation, SymInt groups, SymInt deformable_groups, SymInt precision, "
+                                  "Tensor? cols=None) -> (Tensor, Tensor, Tensor)",
+}
+
+
+def _check_dcn_fakes(ops, x, w, off):
+    """The six deformable-conv ops: schemas as released, and the shapes / dtypes of their fake outputs."""
+    for name, schema in _DCN_SCHEMAS.items():
+        assert str(getattr(torch.ops.d2b200, name).default._schema) == schema, name
+    geo = ([2, 2], [1, 1], [1, 1], 2, 1)
+    f32, u8, bf16 = torch.float32, torch.uint8, torch.bfloat16
+    mask = torch.empty(2, 9, 10, 15, device="cuda")
+    om = torch.empty(2, 27, 10, 15, device="cuda")
+    sc, sh = torch.empty(24, device="cuda"), torch.empty(24, device="cuda")
+    xb = x.to(bf16)
+
+    def meta(ts):
+        return [(tuple(t.shape), t.dtype) for t in ts]
+
+    y = ops.deform_conv_op(xb, off, mask, w, sh, *geo, 1)
+    assert meta([y]) == [((2, 24, 10, 15), bf16)]
+    assert meta(ops.deform_conv_train_op(xb, off, mask, w, sh, *geo, -1)) == [((2, 24, 10, 15), bf16), ((0,), f32),
+                                                                               ((0,), u8)]
+    go = torch.empty(2, 24, 10, 15, device="cuda")
+    assert meta(ops.deform_conv_backward_op(x, off, mask, w, go, *geo, True, True, True, 1)) == [
+        ((2, 16, 20, 30), f32), ((2, 18, 10, 15), f32), ((2, 9, 10, 15), f32), ((24, 8, 3, 3), f32), ((24,), f32)]
+    assert meta(ops.deform_conv_backward_op(x, off, None, w, go, *geo, False, False, True, 0)) == [
+        ((0,), f32), ((0,), f32), ((0,), f32), ((24, 8, 3, 3), f32), ((0,), f32)]
+    assert meta(ops.deform_conv_backward_op(x, off, mask, w, go, *geo, True, True, False, -1)) == [
+        ((2, 16, 20, 30), f32), ((2, 18, 10, 15), f32), ((2, 9, 10, 15), f32), ((0,), f32), ((0,), f32)]
+    y = ops.deform_conv_fused_op(xb, om, w, sc, sh, True, *geo, -1)
+    assert meta([y]) == [((2, 24, 10, 15), bf16)]
+    assert meta(ops.deform_conv_fused_train_op(xb, om, w, None, sh, False, *geo, 2)) == [((2, 24, 10, 15), bf16),
+                                                                                        ((0,), f32), ((0,), u8)]
+    assert meta(ops.deform_conv_fused_backward_op(x, om, w, sc, True, go, go, *geo, 1)) == [
+        ((2, 16, 20, 30), f32), ((2, 27, 10, 15), f32), ((24, 8, 3, 3), f32)]
 
 
 def test_pooler_layout_policy_host_logic(monkeypatch):
