@@ -26,15 +26,16 @@ __all__ = ["mask_rcnn_loss", "mask_loss_per_roi"]
 @torch.library.custom_op("d2b200::mask_loss", mutates_args=(), device_types="cuda")
 def mask_loss_per_roi(logits: Tensor, gt_masks: Tensor, boxes: Tensor, mask_index: Optional[Tensor],
                       classes: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
-    """One image.  logits [K,C,S,S]; gt_masks [G,H,W] bool / uint8; boxes [K,4]; mask_index [K] (None: proposal k <-> mask k);
-    classes [K] (None: class-agnostic).  Returns (loss sum per proposal [K] fp32, targets [K,S,S] bool)."""
+    """One image.  logits [K,C,S,S]; gt_masks [G,H,W] bool / uint8 / float (nonzero = 1); boxes [K,4]; mask_index [K]
+    (None: proposal k <-> mask k); classes [K] (None: class-agnostic).  Returns (loss sum per proposal [K] fp32, targets
+    [K,S,S] bool)."""
     _C.require_cuda(logits, gt_masks, boxes, mask_index, classes)
     if logits.dim() != 4 or logits.shape[2] != logits.shape[3]:
         raise RuntimeError("mask_loss: logits must be K x C x S x S")
     lg = logits.to(dtype=torch.float32).contiguous()
     k, c, s, _ = lg.shape
     gm = gt_masks.contiguous()
-    gm = gm.view(torch.uint8) if gm.dtype == torch.bool else gm.to(torch.uint8)
+    gm = (gm if gm.dtype == torch.bool else gm != 0).view(torch.uint8)  # any nonzero value is 1, as BitMasks reads it
     if gm.dim() != 3 or boxes.shape != (k, 4):
         raise RuntimeError("mask_loss: gt_masks must be G x H x W and boxes K x 4")
     bx = boxes.to(dtype=torch.float32).contiguous()

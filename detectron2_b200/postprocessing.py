@@ -24,7 +24,7 @@ def crop_and_resize(bit_masks: torch.Tensor, boxes: torch.Tensor, mask_size: int
     device = bit_masks.device
     batch_inds = torch.arange(len(boxes), device=device).to(dtype=boxes.dtype)[:, None]
     rois = torch.cat([batch_inds, boxes.to(device=device)], dim=1)  # N x 5: every mask is pooled with its own box
-    masks = bit_masks.to(dtype=torch.float32)
+    masks = (bit_masks != 0).to(dtype=torch.float32)  # BitMasks stores `tensor.to(torch.bool)`: any nonzero value is 1
     output = ROIAlign((mask_size, mask_size), 1.0, 0, aligned=True).forward(masks[:, None, :, :], rois).squeeze(1)
     return output >= 0.5
 
