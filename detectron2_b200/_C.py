@@ -100,6 +100,7 @@ def _declare(lib):
                                   i64p, i64p, vp]),
         "d2b_dense_prepare": (i, [C.POINTER(DenseLevels), i, i, C.POINTER(C.c_float), f, f32p, f32p, f32p, f32p, i64p, i64p,
                                   vp]),
+        "d2b_dense_prepare_linear": (i, [C.POINTER(DenseLevels), i, i, f32p, f32p, f32p, f32p, i64p, i64p, vp]),
         "d2b_rrpn_prepare": (i, [C.POINTER(RpnLevels), i, f32p, f, i, f32p, f32p, f32p, f32p, i64p, vp, vp]),
         "d2b_frcnn_rotated_prepare": (i, [f32p, f32p, C.POINTER(C.c_int), i, i, i, f32p, f, i, i, f32p, f32p, f32p, f32p, i64p,
                                           i64p, i64p, i64p, vp]),
@@ -115,6 +116,11 @@ def _declare(lib):
                                        C.POINTER(C.c_float), f32p, f32p, i64p, i64p, vp, vp, sz, vp]),
         "d2b_dense_loss_backward": (i, [C.POINTER(DenseLossLevels), i, i, i, i, f32p, f32p, vp, i, f, f, f, i, f,
                                         C.POINTER(C.c_float), f32p, f32p, vp]),
+        "d2b_fcos_loss_workspace_bytes": (sz, [C.POINTER(DenseLossLevels), i, i, i]),
+        "d2b_fcos_loss_forward": (i, [C.POINTER(DenseLossLevels), C.POINTER(C.c_void_p), i, i, i, f32p, f32p, i64p, f, f, f32p,
+                                      f32p, f32p, i64p, vp, vp, sz, vp]),
+        "d2b_fcos_loss_backward": (i, [C.POINTER(DenseLossLevels), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), i, i, i,
+                                       f32p, f32p, i64p, f, f, f32p, f32p, f32p, vp]),
         "d2b_frcnn_loss_workspace_bytes": (sz, [i]),
         "d2b_frcnn_loss_forward": (i, [vp, vp, i, i, i, i, i, f32p, f32p, i64p, f, i, f, C.POINTER(C.c_float), f32p, f32p, i64p,
                                        i64p, i64p, i64p, vp, vp, sz, vp]),
@@ -124,6 +130,7 @@ def _declare(lib):
         "d2b_match_workspace_bytes": (sz, [i, i, i]),
         "d2b_match_boxes": (i, [f32p, i64p, i, i, f32p, i64, i64p, i, C.POINTER(C.c_double), i, C.POINTER(C.c_int), i, f32p, d,
                                 i64p, i64, i64p, vp, f32p, i64p, vp, vp, sz, vp]),
+        "d2b_fcos_assign": (i, [f32p, C.POINTER(C.c_int), i, f32p, i64p, i, i, i64p, i64, d, i64p, i64p, f32p, vp]),
         "d2b_sample_labels_workspace_bytes": (sz, [i, i, i]),
         "d2b_sample_labels": (i, [vp, i, i, i, i64, i, i, vp, vp, i64p, i64p, i64p, vp, sz, vp]),
         "d2b_deform_conv_tc_shape_supported": (i, [C.POINTER(DcnParams), i]),

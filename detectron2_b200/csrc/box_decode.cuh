@@ -33,3 +33,26 @@ __device__ __forceinline__ DecodedBox apply_deltas(float4 an, float4 d, float wx
   b.y2 = pcy + 0.5f * ph;
   return b;
 }
+
+// Box2BoxTransformLinear.apply_deltas (box_regression.py:275-307) with normalize_by_size=True, op for op: relu(deltas)
+// times the anchor's stride (width, height), then the centre minus (l, t) and plus (r, b).  Shared by the FCOS inference
+// decode (postproc.cu) and the FCOS GIoU loss (losses.cu).
+struct LinearBox {
+  float x1, y1, x2, y2;
+  float sw, sh;  // the stride, what the backward multiplies by
+};
+
+// F.relu = clamp_min(0): NaN stays NaN
+__device__ __forceinline__ float relu_nan(float v) { return v != v ? v : (v > 0.f ? v : 0.f); }
+
+__device__ __forceinline__ LinearBox apply_deltas_linear(float4 an, float4 d) {
+  LinearBox b;
+  const float ctr_x = 0.5f * (an.x + an.z), ctr_y = 0.5f * (an.y + an.w);
+  b.sw = an.z - an.x;
+  b.sh = an.w - an.y;
+  b.x1 = ctr_x - relu_nan(d.x) * b.sw;
+  b.y1 = ctr_y - relu_nan(d.y) * b.sh;
+  b.x2 = ctr_x + relu_nan(d.z) * b.sw;
+  b.y2 = ctr_y + relu_nan(d.w) * b.sh;
+  return b;
+}

@@ -8,6 +8,8 @@
 //       Box2BoxTransform[Rotated].get_deltas computed on the fly.  One launch: classification CTAs stream the logits
 //       (16-byte vectors, the row label re-read only when the row changes), regression CTAs own one anchor row per
 //       thread; a second single-CTA launch adds the per-CTA partials in a fixed order.
+//   d2b_fcos_loss_forward / _backward    FCOS.losses + compute_ctrness_targets (meta_arch/fcos.py:193-251): the same kernel
+//       with kFcos -- GIoU of Box2BoxTransformLinear's decode and, on the positive rows, the centerness BCE as a third sum.
 //   d2b_frcnn_loss_forward / _backward   FastRCNNOutputLayers.losses / box_reg_loss (roi_heads/fast_rcnn.py:307-352,
 //       424-463) and _log_classification_stats (:88-115): one warp per proposal row -- max, log-sum-exp, argmax, the class
 //       gather of the deltas, the targets and smooth-L1 -- then the same fixed-order finish.
@@ -166,6 +168,30 @@ __device__ __forceinline__ float giou_row(const float* an, const float (&d)[4], 
   return loss;
 }
 
+// FCOS GIoU regression of one row: the deltas decoded by Box2BoxTransformLinear.apply_deltas on the anchor point, the loss
+// against the GT box, and g = d loss / d deltas through the decode and the relu (threshold_backward: 0 where delta <= 0).
+__device__ __forceinline__ float giou_row_linear(const float* an, const float (&d)[4], const float* gt, float (&g)[4],
+                                                bool& ordered) {
+  const LinearBox b = apply_deltas_linear(make_float4(an[0], an[1], an[2], an[3]), make_float4(d[0], d[1], d[2], d[3]));
+  const float p[4] = {b.x1, b.y1, b.x2, b.y2};
+  float gp[4];
+  const float loss = giou_loss(p, gt, gp, ordered);
+  g[0] = d[0] <= 0.f ? 0.f : -gp[0] * b.sw;
+  g[1] = d[1] <= 0.f ? 0.f : -gp[1] * b.sh;
+  g[2] = d[2] <= 0.f ? 0.f : gp[2] * b.sw;
+  g[3] = d[3] <= 0.f ? 0.f : gp[3] * b.sh;
+  return loss;
+}
+
+// FCOS.compute_ctrness_targets (meta_arch/fcos.py:240-251) of one row: Box2BoxTransformLinear.get_deltas (l, t, r, b
+// divided by the stride, box_regression.py:243-273), then sqrt((min(l, r) / max(l, r)) * (min(t, b) / max(t, b))).
+__device__ __forceinline__ float ctrness_target(const float* an, const float* gt) {
+  const float cx = 0.5f * (an[0] + an[2]), cy = 0.5f * (an[1] + an[3]);
+  const float sw = an[2] - an[0], sh = an[3] - an[1];
+  const float l = (cx - gt[0]) / sw, t = (cy - gt[1]) / sh, r = (gt[2] - cx) / sw, b = (gt[3] - cy) / sh;
+  return sqrtf((tmin(l, r) / tmax(l, r)) * (tmin(t, b) / tmax(t, b)));
+}
+
 // fvcore sigmoid_focal_loss of one element; g = d loss / d x.  ce = binary_cross_entropy_with_logits as torch writes it,
 // (1 - t) x - log_sigmoid(x) with log_sigmoid(x) = min(x, 0) - log1p(exp(-|x|)).  gamma = 0 is taken analytically
 // (g = sigmoid(x) - t, where autograd of (1 - p_t) ** 0 would give 0 * inf at saturation).
@@ -194,14 +220,13 @@ __device__ __forceinline__ float focal(float x, float t, float gamma, float alph
 
 // ---- per-CTA partials and the fixed-order finish ------------------------------------------------------------------
 struct Partial {
-  float sum[2];      // classification, regression
-  long long cnt[4];  // dense: num_pos, num_neg; Fast R-CNN: num_fg, num_accurate, fg_num_accurate, num_false_negative
+  float sum[3];      // classification, regression, FCOS centerness
   int status;
-  int pad;
+  long long cnt[4];  // dense: num_pos, num_neg; Fast R-CNN: num_fg, num_accurate, fg_num_accurate, num_false_negative
 };
 
 struct BlockRed {
-  float f[2][kWarps];
+  float f[3][kWarps];
   long long c[4][kWarps];
   int s[kWarps];
 };
@@ -219,11 +244,12 @@ __device__ __forceinline__ long long warp_sum(long long v) {
 }
 
 // Sums of the CTA in a fixed order (lanes by butterfly, then warps 0..7), written by thread 0 to `out`.
-__device__ __forceinline__ void block_partial(float s0, float s1, const long long (&c)[4], int status, BlockRed& red,
-                                              Partial* __restrict__ out) {
+__device__ __forceinline__ void block_partial(float s0, float s1, float s2, const long long (&c)[4], int status,
+                                              BlockRed& red, Partial* __restrict__ out) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   s0 = warp_sum(s0);
   s1 = warp_sum(s1);
+  s2 = warp_sum(s2);
   long long w[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) w[i] = warp_sum(c[i]);
@@ -231,6 +257,7 @@ __device__ __forceinline__ void block_partial(float s0, float s1, const long lon
   if (lane == 0) {
     red.f[0][warp] = s0;
     red.f[1][warp] = s1;
+    red.f[2][warp] = s2;
 #pragma unroll
     for (int i = 0; i < 4; ++i) red.c[i][warp] = w[i];
     red.s[warp] = status;
@@ -241,6 +268,7 @@ __device__ __forceinline__ void block_partial(float s0, float s1, const long lon
     for (int k = 0; k < kWarps; ++k) {
       p.sum[0] += red.f[0][k];
       p.sum[1] += red.f[1][k];
+      p.sum[2] += red.f[2][k];
 #pragma unroll
       for (int i = 0; i < 4; ++i) p.cnt[i] += red.c[i][k];
       p.status |= red.s[k];
@@ -251,26 +279,29 @@ __device__ __forceinline__ void block_partial(float s0, float s1, const long lon
 
 __global__ void __launch_bounds__(kThreads) finish_kernel(const Partial* __restrict__ part, int nparts,
                                                           float* __restrict__ sum0, float* __restrict__ sum1,
+                                                          float* __restrict__ sum2,
                                                           int64_t* __restrict__ c0, int64_t* __restrict__ c1,
                                                           int64_t* __restrict__ c2, int64_t* __restrict__ c3,
                                                           int* __restrict__ status) {
-  __shared__ double s_f[2][kThreads];
+  __shared__ double s_f[3][kThreads];
   __shared__ long long s_c[4][kThreads];
   __shared__ int s_s[kThreads];
   const int tid = threadIdx.x;
-  double f0 = 0.0, f1 = 0.0;
+  double f0 = 0.0, f1 = 0.0, f2 = 0.0;
   long long c[4] = {0, 0, 0, 0};
   int st = 0;
   for (int i = tid; i < nparts; i += kThreads) {
     const Partial p = part[i];
     f0 += (double)p.sum[0];
     f1 += (double)p.sum[1];
+    f2 += (double)p.sum[2];
 #pragma unroll
     for (int k = 0; k < 4; ++k) c[k] += p.cnt[k];
     st |= p.status;
   }
   s_f[0][tid] = f0;
   s_f[1][tid] = f1;
+  s_f[2][tid] = f2;
 #pragma unroll
   for (int k = 0; k < 4; ++k) s_c[k][tid] = c[k];
   s_s[tid] = st;
@@ -279,6 +310,7 @@ __global__ void __launch_bounds__(kThreads) finish_kernel(const Partial* __restr
     if (tid < o) {
       s_f[0][tid] += s_f[0][tid + o];
       s_f[1][tid] += s_f[1][tid + o];
+      s_f[2][tid] += s_f[2][tid + o];
 #pragma unroll
       for (int k = 0; k < 4; ++k) s_c[k][tid] += s_c[k][tid + o];
       s_s[tid] |= s_s[tid + o];
@@ -288,6 +320,7 @@ __global__ void __launch_bounds__(kThreads) finish_kernel(const Partial* __restr
   if (tid == 0) {
     *sum0 = (float)s_f[0][0];
     *sum1 = (float)s_f[1][0];
+    if (sum2) *sum2 = (float)s_f[2][0];
     if (c0) *c0 = s_c[0][0];
     if (c1) *c1 = s_c[1][0];
     if (c2) *c2 = s_c[2][0];
@@ -303,6 +336,8 @@ struct DenseLevels {
   const void* deltas[D2B_MAX_LEVELS];
   void* grad_logits[D2B_MAX_LEVELS];
   void* grad_deltas[D2B_MAX_LEVELS];
+  const void* ctr[D2B_MAX_LEVELS];        // FCOS centerness logits [N, R_l]
+  void* grad_ctr[D2B_MAX_LEVELS];
   int R[D2B_MAX_LEVELS];
   int a0[D2B_MAX_LEVELS + 1];             // first anchor of each level
   long long blk0[D2B_MAX_LEVELS + 1];     // first classification CTA of each level
@@ -336,10 +371,13 @@ struct DenseArgs {
   BoxWeights w;
   const float* grad_cls;  // backward: d loss / d classification sum (device scalar)
   const float* grad_reg;
+  const float* grad_ctr;  // FCOS
   Partial* part;          // forward
 };
 
-template <int DT, class Box, class Lab, bool kBackward>
+// kFcos: FCOS.losses -- the regression is the GIoU of Box2BoxTransformLinear's decode, and the positive rows add the
+// centerness term, binary_cross_entropy_with_logits against ctrness_target (the third sum; gradient sigmoid(x) - t).
+template <int DT, class Box, class Lab, bool kBackward, bool kFcos = false>
 __global__ void __launch_bounds__(kThreads) dense_loss_kernel(const DenseLevels P, const DenseArgs A) {
   using E = Elem<DT>;
   using T = typename E::T;
@@ -349,7 +387,7 @@ __global__ void __launch_bounds__(kThreads) dense_loss_kernel(const DenseLevels 
   const int tid = threadIdx.x;
   const long long b = blockIdx.x;
   const typename Lab::T* __restrict__ labels = (const typename Lab::T*)A.labels;
-  float s_cls = 0.f, s_reg = 0.f;
+  float s_cls = 0.f, s_reg = 0.f, s_ctr = 0.f;
   long long cnt[4] = {0, 0, 0, 0};
   int status = 0;
   if (b < A.cls_blocks) {
@@ -422,7 +460,19 @@ __global__ void __launch_bounds__(kThreads) dense_loss_kernel(const DenseLevels 
       float g[D];
 #pragma unroll
       for (int q = 0; q < D; ++q) g[q] = 0.f;
-      if (pos) {
+      if constexpr (kFcos) {
+        float gc = 0.f;
+        const size_t oc = (size_t)n * P.R[l] + r;
+        if (pos) {
+          const float* gt = A.gt_boxes + (size_t)row * 4;
+          const float dv[4] = {E::ld(dl[0]), E::ld(dl[1]), E::ld(dl[2]), E::ld(dl[3])};
+          bool ordered;
+          s_reg += giou_row_linear(an, dv, gt, g, ordered);
+          if (!ordered) status |= D2B_LOSS_STATUS_INVALID_BOX_ORDER;
+          s_ctr += focal(E::ld(((const T*)P.ctr[l])[oc]), ctrness_target(an, gt), 0.f, -1.f, gc);
+        }
+        if (kBackward) ((T*)P.grad_ctr[l])[oc] = E::st(gc * *A.grad_ctr);
+      } else if (pos) {
         if constexpr (D == 4) {
           if (A.giou) {
             const float dv[4] = {E::ld(dl[0]), E::ld(dl[1]), E::ld(dl[2]), E::ld(dl[3])};
@@ -446,7 +496,7 @@ __global__ void __launch_bounds__(kThreads) dense_loss_kernel(const DenseLevels 
       }
     }
   }
-  if (!kBackward) block_partial(s_cls, s_reg, cnt, status, red, A.part + b);
+  if (!kBackward) block_partial(s_cls, s_reg, s_ctr, cnt, status, red, A.part + b);
 }
 
 // ---- Fast R-CNN ----------------------------------------------------------------------------------------------------
@@ -572,7 +622,7 @@ __global__ void __launch_bounds__(kThreads) frcnn_loss_kernel(const FrcnnArgs A)
       if (fg && lane < D) gd[col + lane] = E::st(g * gs);
     }
   }
-  if (!kBackward) block_partial(s_cls, s_reg, cnt, status, red, A.part + blockIdx.x);
+  if (!kBackward) block_partial(s_cls, s_reg, 0.f, cnt, status, red, A.part + blockIdx.x);
 }
 
 // ---- host side -----------------------------------------------------------------------------------------------------
@@ -625,9 +675,9 @@ long long dense_levels(const d2b_dense_loss_levels* lv, int N, int K, int dtype,
 
 long long dense_reg_blocks(int N, int Rtot) { return ((long long)N * Rtot + kThreads - 1) / kThreads; }
 
-template <int DT, class Box, class Lab, bool kBackward>
+template <int DT, class Box, class Lab, bool kBackward, bool kFcos = false>
 void launch_dense(long long blocks, const DenseLevels& P, const DenseArgs& A, cudaStream_t st) {
-  dense_loss_kernel<DT, Box, Lab, kBackward><<<(unsigned)blocks, kThreads, 0, st>>>(P, A);
+  dense_loss_kernel<DT, Box, Lab, kBackward, kFcos><<<(unsigned)blocks, kThreads, 0, st>>>(P, A);
 }
 
 template <bool kBackward>
@@ -678,6 +728,33 @@ int dense_setup(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int 
   A.giou = loss_type == D2B_LOSS_GIOU;
   A.scale_clamp = scale_clamp;
   A.w = box_weights(weights, box_dim);
+  return D2B_OK;
+}
+
+// FCOS: the dense rules with xyxy anchors, int64 labels and the GIoU flag, plus the per-level centerness logits.
+int fcos_setup(const d2b_dense_loss_levels* lv, const void* const* ctr, void* const* grad_ctr, int N, int K, int dtype,
+               const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma, float alpha, bool backward,
+               DenseLevels& P, DenseArgs& A, long long& blocks) {
+  const float ones[4] = {1.f, 1.f, 1.f, 1.f};
+  const int rc = dense_setup(lv, N, K, 4, dtype, anchors, gt_boxes, labels, D2B_LABELS_I64, gamma, alpha, 0.f,
+                             D2B_LOSS_GIOU, 0.f, ones, backward, P, A, blocks);
+  if (rc) return rc;
+  if (!ctr || (backward && !grad_ctr)) return D2B_EINVAL;
+  for (int l = 0; l < P.L; ++l) {
+    const bool some = (long long)N * P.R[l] > 0;
+    if (some && (!ctr[l] || (backward && !grad_ctr[l]))) return D2B_EINVAL;
+    P.ctr[l] = ctr[l];
+    P.grad_ctr[l] = backward ? grad_ctr[l] : nullptr;
+  }
+  return D2B_OK;
+}
+
+template <bool kBackward>
+int fcos_dispatch(long long blocks, int dtype, const DenseLevels& P, const DenseArgs& A, cudaStream_t st) {
+  if (dtype == D2B_F32) launch_dense<D2B_F32, XyxyBox, LabelsI64, kBackward, true>(blocks, P, A, st);
+  if (dtype == D2B_F16) launch_dense<D2B_F16, XyxyBox, LabelsI64, kBackward, true>(blocks, P, A, st);
+  if (dtype == D2B_BF16) launch_dense<D2B_BF16, XyxyBox, LabelsI64, kBackward, true>(blocks, P, A, st);
+  D2B_CHECK_LAUNCH();
   return D2B_OK;
 }
 
@@ -751,7 +828,8 @@ D2B_API int d2b_dense_loss_forward(const d2b_dense_loss_levels* lv, int N, int K
     const int e = dense_dispatch<false>(blocks, dtype, box_dim, label_kind, P, A, st);
     if (e) return e;
   }
-  finish_kernel<<<1, kThreads, 0, st>>>(A.part, (int)blocks, cls_sum, reg_sum, num_pos, num_neg, nullptr, nullptr, status);
+  finish_kernel<<<1, kThreads, 0, st>>>(A.part, (int)blocks, cls_sum, reg_sum, nullptr, num_pos, num_neg, nullptr, nullptr,
+                                        status);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }
@@ -772,6 +850,51 @@ D2B_API int d2b_dense_loss_backward(const d2b_dense_loss_levels* lv, int N, int 
   A.grad_cls = grad_cls;
   A.grad_reg = grad_reg;
   return dense_dispatch<true>(blocks, dtype, box_dim, label_kind, P, A, (cudaStream_t)stream);
+}
+
+D2B_API size_t d2b_fcos_loss_workspace_bytes(const d2b_dense_loss_levels* lv, int N, int K, int dtype) {
+  return d2b_dense_loss_workspace_bytes(lv, N, K, dtype);
+}
+
+D2B_API int d2b_fcos_loss_forward(const d2b_dense_loss_levels* lv, const void* const* ctr, int N, int K, int dtype,
+                                  const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma,
+                                  float alpha, float* cls_sum, float* reg_sum, float* ctr_sum, int64_t* num_pos,
+                                  int* status, void* workspace, size_t workspace_bytes, void* stream) {
+  DenseLevels P;
+  DenseArgs A;
+  long long blocks = 0;
+  const int rc = fcos_setup(lv, ctr, nullptr, N, K, dtype, anchors, gt_boxes, labels, gamma, alpha, false, P, A, blocks);
+  if (rc) return rc;
+  if (!cls_sum || !reg_sum || !ctr_sum || !num_pos || !status) return D2B_EINVAL;
+  if (blocks > 0 && (!workspace || !aligned16(workspace))) return D2B_EINVAL;
+  if (workspace_bytes < (size_t)blocks * sizeof(Partial)) return D2B_EWORKSPACE;
+  const cudaStream_t st = (cudaStream_t)stream;
+  A.part = (Partial*)workspace;
+  if (blocks > 0) {
+    const int e = fcos_dispatch<false>(blocks, dtype, P, A, st);
+    if (e) return e;
+  }
+  finish_kernel<<<1, kThreads, 0, st>>>(A.part, (int)blocks, cls_sum, reg_sum, ctr_sum, num_pos, nullptr, nullptr, nullptr,
+                                        status);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
+}
+
+D2B_API int d2b_fcos_loss_backward(const d2b_dense_loss_levels* lv, const void* const* ctr, void* const* grad_ctr, int N,
+                                   int K, int dtype, const float* anchors, const float* gt_boxes, const int64_t* labels,
+                                   float gamma, float alpha, const float* grad_cls, const float* grad_reg,
+                                   const float* grad_ctr_sum, void* stream) {
+  DenseLevels P;
+  DenseArgs A;
+  long long blocks = 0;
+  const int rc = fcos_setup(lv, ctr, grad_ctr, N, K, dtype, anchors, gt_boxes, labels, gamma, alpha, true, P, A, blocks);
+  if (rc) return rc;
+  if (!grad_cls || !grad_reg || !grad_ctr_sum) return D2B_EINVAL;
+  if (blocks == 0) return D2B_OK;
+  A.grad_cls = grad_cls;
+  A.grad_reg = grad_reg;
+  A.grad_ctr = grad_ctr_sum;
+  return fcos_dispatch<true>(blocks, dtype, P, A, (cudaStream_t)stream);
 }
 
 D2B_API size_t d2b_frcnn_loss_workspace_bytes(int R) {
@@ -797,7 +920,7 @@ D2B_API int d2b_frcnn_loss_forward(const void* scores, const void* deltas, int R
     const int e = frcnn_dispatch<false>(dtype, box_dim, A, st);
     if (e) return e;
   }
-  finish_kernel<<<1, kThreads, 0, st>>>(A.part, d2b_cdiv(R, kWarps), cls_sum, reg_sum, num_fg, num_accurate,
+  finish_kernel<<<1, kThreads, 0, st>>>(A.part, d2b_cdiv(R, kWarps), cls_sum, reg_sum, nullptr, num_fg, num_accurate,
                                         fg_num_accurate, num_false_negative, status);
   D2B_CHECK_LAUNCH();
   return D2B_OK;

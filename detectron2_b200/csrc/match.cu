@@ -24,6 +24,9 @@
 //
 // The box type is a template policy (XyxyBox: pairwise_iou of structures/boxes.py:312-358 op for op; RotBox: the rotated IoU
 // of nms.cu, shared through rotated_iou.cuh).  Compiled with -fmad=false like nms.cu / postproc.cu: bit-exact IoUs.
+//
+// d2b_fcos_assign (FCOS._match_anchors + label_anchors, meta_arch/fcos.py:97-191) shares the GT tiling: one launch,
+// fcos_assign_kernel, one thread per (image, point), no G x R matrix; the quality and its argmax are bit-exact.
 #include <climits>
 
 #include "common.cuh"
@@ -239,6 +242,89 @@ __global__ void __launch_bounds__(kThreads) match_label_kernel(const MatchArgs a
                             : (lab == 1 ? a.gt_classes[(size_t)n * a.Gmax + m] : (lab == 0 ? a.num_classes : -1LL));
 }
 
+// ---- FCOS point assignment (FCOS._match_anchors + label_anchors, meta_arch/fcos.py:97-191) -------------------------
+// One thread per (image, point), the image's GT boxes staged in shared memory with their centre and 1e8 - area.  The
+// quality of GT g at point p is float(centre test && inside test && scale test) * (1e8 - area_g), every value rounded in
+// fp32 as the reference's tensor ops; the argmax over g is torch.max(dim=0)'s (a NaN beats every number, the first NaN
+// wins, ties go to the lowest index).  Unmatched (q < 1e-5; a NaN maximum is matched) points keep GT 0's box and get
+// label K, as the reference's `matched_idxs.clip(min=0)` gathers.
+struct FcosArgs {
+  const float* anchors;          // [R, 4]
+  int R, lvl0_end, last_begin;   // points [0, lvl0_end): lower bound 0; [last_begin, R): upper bound +inf
+  float radius;
+  const float* gt;               // [N, Gmax, 4]
+  const long long* gt_count;     // [N]
+  int Gmax;
+  const long long* gt_classes;   // [N, Gmax]
+  long long num_classes;
+  long long* matches;            // [N, R]
+  long long* labels;             // [N, R]
+  float* out_boxes;              // [N, R, 4]
+};
+
+constexpr int kFcosGt = 7;  // x0, y0, x1, y1, centre x, centre y, 1e8 - area
+
+__global__ void __launch_bounds__(kThreads) fcos_assign_kernel(const FcosArgs a) {
+  __shared__ float s_gt[kTile * kFcosGt];
+  const int n = blockIdx.y, tid = threadIdx.x;
+  const int p = blockIdx.x * kThreads + tid;
+  const int G = (int)min(max(a.gt_count[n], 0LL), (long long)a.Gmax);
+  const bool live = p < a.R;
+  float cx = 0.f, cy = 0.f, rs = 0.f, lo = 0.f, hi = 0.f;
+  if (live) {
+    const float* an = a.anchors + (size_t)p * 4;
+    cx = (an[0] + an[2]) / 2.f;  // Boxes.get_centers
+    cy = (an[1] + an[3]) / 2.f;
+    const float size = an[2] - an[0];
+    rs = a.radius * size;
+    lo = p < a.lvl0_end ? 0.f : size * 4.f;
+    hi = p >= a.last_begin ? INFINITY : size * 8.f;
+  }
+  float best = -INFINITY;
+  int arg = 0;
+  const float* gt = a.gt + (size_t)n * a.Gmax * 4;
+  for (int g0 = 0; g0 < G; g0 += kTile) {
+    const int ng = min(kTile, G - g0);
+    __syncthreads();  // previous tile consumed
+    for (int t = tid; t < ng; t += kThreads) {
+      const float* b = gt + (size_t)(g0 + t) * 4;
+      float* s = s_gt + t * kFcosGt;
+      s[0] = b[0];
+      s[1] = b[1];
+      s[2] = b[2];
+      s[3] = b[3];
+      s[4] = (b[0] + b[2]) / 2.f;
+      s[5] = (b[1] + b[3]) / 2.f;
+      s[6] = 1e8f - (b[2] - b[0]) * (b[3] - b[1]);  // 1e8 - Boxes.area()
+    }
+    __syncthreads();
+    if (live) {
+      for (int j = 0; j < ng; ++j) {
+        const float* s = s_gt + j * kFcosGt;
+        bool in = nan_max(fabsf(cx - s[4]), fabsf(cy - s[5])) < rs;               // centre sampling
+        // pairwise_point_box_distance: (x - x0, y - y0, x1 - x, y1 - y)
+        const float l = cx - s[0], t = cy - s[1], r = s[2] - cx, b = s[3] - cy;
+        in = in && nan_min(nan_min(l, t), nan_min(r, b)) > 0.f;                   // inside the box
+        const float m = nan_max(nan_max(l, t), nan_max(r, b));
+        in = in && m > lo && m < hi;                                              // the level's scale range
+        const float q = (in ? 1.f : 0.f) * s[6];
+        if (q != q ? best == best : q > best) {  // GreaterOrNan, strict: the first index wins ties and NaNs
+          best = q;
+          arg = g0 + j;
+        }
+      }
+    }
+  }
+  if (!live) return;
+  const size_t o = (size_t)n * a.R + p;
+  const bool matched = G > 0 && !(best < 1e-5f);
+  a.matches[o] = matched ? arg : -1;
+  a.labels[o] = matched ? a.gt_classes[(size_t)n * a.Gmax + arg] : a.num_classes;
+  const int src = matched ? arg : 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) a.out_boxes[o * 4 + q] = G > 0 ? gt[(size_t)src * 4 + q] : 0.f;
+}
+
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 template <class Box>
@@ -319,4 +405,40 @@ D2B_API int d2b_match_boxes(const float* gt_boxes, const int64_t* gt_count, int 
   a.mval = (float*)((char*)workspace + align256(sizeof(unsigned) * (size_t)N * Gmax));
   return rotated ? launch<RotBox>(a, N, (cudaStream_t)stream)
                  : launch<XyxyBox>(a, N, (cudaStream_t)stream);
+}
+
+D2B_API int d2b_fcos_assign(const float* anchors, const int* level_counts, int num_levels, const float* gt_boxes,
+                            const int64_t* gt_count, int N, int Gmax, const int64_t* gt_classes, int64_t num_classes,
+                            double center_sampling_radius, int64_t* matches, int64_t* labels, float* matched_gt_boxes,
+                            void* stream) {
+  if (num_levels < 1 || num_levels > D2B_MAX_LEVELS || !level_counts) return D2B_EINVAL;
+  long long R = 0;
+  for (int l = 0; l < num_levels; ++l) {
+    if (level_counts[l] < 0) return D2B_EINVAL;
+    R += level_counts[l];
+  }
+  if (R > INT_MAX - kThreads || N < 0 || N > 65535 || Gmax < 0 || num_classes < 0) return D2B_EINVAL;
+  if (N == 0 || R == 0) return D2B_OK;
+  if (!anchors || !gt_count || !matches || !labels || !matched_gt_boxes) return D2B_EINVAL;
+  if (Gmax > 0 && (!gt_boxes || !gt_classes)) return D2B_EINVAL;
+  FcosArgs a = {};
+  a.anchors = anchors;
+  a.R = (int)R;
+  a.lvl0_end = level_counts[0];
+  // upper_bound[-R_last:] = inf: with an empty last level that slice is the whole tensor
+  const int last = level_counts[num_levels - 1];
+  a.last_begin = last == 0 ? 0 : (int)R - last;
+  a.radius = (float)center_sampling_radius;  // the python float meets an fp32 tensor: rounded to fp32
+  a.gt = gt_boxes;
+  a.gt_count = (const long long*)gt_count;
+  a.Gmax = Gmax;
+  a.gt_classes = (const long long*)gt_classes;
+  a.num_classes = num_classes;
+  a.matches = (long long*)matches;
+  a.labels = (long long*)labels;
+  a.out_boxes = matched_gt_boxes;
+  const dim3 grid((unsigned)d2b_cdiv(R, kThreads), (unsigned)N);
+  fcos_assign_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(a);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
 }

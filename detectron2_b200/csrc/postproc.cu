@@ -247,6 +247,8 @@ D2B_API int d2b_rpn_select_rotated(const int64_t* keep, const int64_t* num_keep,
 //   d2b_dense_prepare   DenseDetector._decode_per_level_predictions (meta_arch/dense_detector.py:186-235) after the per-level
 //                       top-k: Box2BoxTransform.apply_deltas (box_regression.py:78-116, same fp32 expression order) on the
 //                       selected (anchor, class) pairs only, class ids, coordinate offsets.
+//   d2b_dense_prepare_linear  the same for FCOS (meta_arch/fcos.py:253-301): Box2BoxTransformLinear.apply_deltas
+//                       (box_regression.py:275-307) as the decode.
 namespace {
 
 struct FrcnnImages {
@@ -421,6 +423,8 @@ struct DenseLevels {
   int R[D2B_MAX_LEVELS], k[D2B_MAX_LEVELS], t0[D2B_MAX_LEVELS + 1];
 };
 
+// kLinear: Box2BoxTransformLinear.apply_deltas (FCOS) instead of Box2BoxTransform.apply_deltas (weights unused)
+template <bool kLinear>
 __global__ void __launch_bounds__(kThreads) dense_prepare_kernel(const DenseLevels P, int T, int K, float wx, float wy, float ww,
                                                                  float wh, float scale_clamp, float* __restrict__ flat_boxes,
                                                                  float* __restrict__ nms_boxes, float* __restrict__ nms_scores,
@@ -444,8 +448,14 @@ __global__ void __launch_bounds__(kThreads) dense_prepare_kernel(const DenseLeve
     const long long cls = f - a * K;
     const float4 an = *reinterpret_cast<const float4*>(P.anchors[l] + (size_t)a * 4);
     const float4 d = *reinterpret_cast<const float4*>(P.deltas[l] + ((size_t)n * P.R[l] + a) * 4);
-    const DecodedBox db = apply_deltas(an, d, wx, wy, ww, wh, scale_clamp);
-    const float x1 = db.x1, y1 = db.y1, x2 = db.x2, y2 = db.y2;
+    float x1, y1, x2, y2;
+    if constexpr (kLinear) {
+      const LinearBox lb = apply_deltas_linear(an, d);
+      x1 = lb.x1, y1 = lb.y1, x2 = lb.x2, y2 = lb.y2;
+    } else {
+      const DecodedBox db = apply_deltas(an, d, wx, wy, ww, wh, scale_clamp);
+      x1 = db.x1, y1 = db.y1, x2 = db.x2, y2 = db.y2;
+    }
     const size_t o = (size_t)n * T + t;
     *reinterpret_cast<float4*>(flat_boxes + o * 4) = make_float4(x1, y1, x2, y2);
     raw_scores[o] = s;
@@ -586,9 +596,12 @@ D2B_API int d2b_rrpn_prepare(const d2b_rpn_levels* lv, int N, const float* image
                              cat_ids, nonfinite, stream);
 }
 
-D2B_API int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
-                              float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
-                              int64_t* cat_ids, void* stream) {
+namespace {
+
+template <bool kLinear>
+int dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
+                  float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
+                  int64_t* cat_ids, void* stream) {
   if (!lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0 || num_classes <= 0 || !weights) return D2B_EINVAL;
   if (N == 0) return D2B_OK;
   DenseLevels P = {};
@@ -611,11 +624,29 @@ D2B_API int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes
   P.t0[P.L] = T;
   if (T == 0) return D2B_OK;
   if (!flat_boxes || !nms_boxes || !nms_scores || !raw_scores || !classes || !cat_ids) return D2B_EINVAL;
-  dense_prepare_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(P, T, num_classes, weights[0], weights[1], weights[2], weights[3],
-                                                                 scale_clamp, flat_boxes, nms_boxes, nms_scores, raw_scores,
-                                                                 (long long*)classes, (long long*)cat_ids);
+  dense_prepare_kernel<kLinear><<<N, kThreads, 0, (cudaStream_t)stream>>>(P, T, num_classes, weights[0], weights[1],
+                                                                          weights[2], weights[3], scale_clamp, flat_boxes,
+                                                                          nms_boxes, nms_scores, raw_scores,
+                                                                          (long long*)classes, (long long*)cat_ids);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
+}
+
+}  // namespace
+
+D2B_API int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
+                              float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
+                              int64_t* cat_ids, void* stream) {
+  return dense_prepare<false>(lv, N, num_classes, weights, scale_clamp, flat_boxes, nms_boxes, nms_scores, raw_scores,
+                              classes, cat_ids, stream);
+}
+
+D2B_API int d2b_dense_prepare_linear(const d2b_dense_levels* lv, int N, int num_classes, float* flat_boxes,
+                                     float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
+                                     int64_t* cat_ids, void* stream) {
+  const float unused[4] = {1.f, 1.f, 1.f, 1.f};
+  return dense_prepare<true>(lv, N, num_classes, unused, 0.f, flat_boxes, nms_boxes, nms_scores, raw_scores, classes,
+                             cat_ids, stream);
 }
 
 // ================================================================================================ mask targets + loss

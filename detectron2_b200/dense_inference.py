@@ -28,7 +28,7 @@ from . import ops
 from ._batched_select import first_k_per_image, nms_select
 from .fast_rcnn_inference import Detections
 
-__all__ = ["apply_deltas", "dense_detector_inference", "retinanet_inference"]
+__all__ = ["apply_deltas", "apply_deltas_linear", "dense_detector_inference", "retinanet_inference"]
 
 _DEFAULT_SCALE_CLAMP = math.log(1000.0 / 16)  # box_regression.py:17
 
@@ -60,15 +60,43 @@ def apply_deltas(deltas: torch.Tensor, boxes: torch.Tensor, weights: Sequence[fl
     return torch.stack((x1, y1, x2, y2), dim=-1).reshape(deltas.shape)
 
 
+def apply_deltas_linear(deltas: torch.Tensor, boxes: torch.Tensor) -> torch.Tensor:
+    """Box2BoxTransformLinear(normalize_by_size=True).apply_deltas (box_regression.py:275-307), op for op: deltas (R, k*4),
+    boxes (R, 4) -> (R, k*4)."""
+    deltas = torch.nn.functional.relu(deltas)
+    boxes = boxes.to(deltas.dtype)
+    ctr_x = 0.5 * (boxes[:, 0] + boxes[:, 2])
+    ctr_y = 0.5 * (boxes[:, 1] + boxes[:, 3])
+    stride_w = boxes[:, 2] - boxes[:, 0]
+    stride_h = boxes[:, 3] - boxes[:, 1]
+    deltas = deltas * torch.stack([stride_w, stride_h, stride_w, stride_h], dim=1).repeat(1, deltas.shape[1] // 4)
+    pred = torch.zeros_like(deltas)
+    pred[:, 0::4] = ctr_x[:, None] - deltas[:, 0::4]
+    pred[:, 1::4] = ctr_y[:, None] - deltas[:, 1::4]
+    pred[:, 2::4] = ctr_x[:, None] + deltas[:, 2::4]
+    pred[:, 3::4] = ctr_y[:, None] + deltas[:, 3::4]
+    return pred
+
+
+_TRANSFORMS = ("delta", "linear")  # Box2BoxTransform (RetinaNet), Box2BoxTransformLinear (FCOS)
+
+
+def _check_transform(transform: str):
+    if transform not in _TRANSFORMS:
+        raise ValueError("box transform must be one of %s, got %r" % (_TRANSFORMS, transform))
+
+
 def dense_detector_inference_fixed(anchors: List[torch.Tensor], pred_scores: List[torch.Tensor],
                                    pred_deltas: List[torch.Tensor], num_images: int, score_thresh: float,
                                    topk_candidates: int, nms_thresh: float, max_detections_per_image: int,
                                    box2box_weights: Sequence[float] = (1.0, 1.0, 1.0, 1.0),
-                                   scale_clamp: float = _DEFAULT_SCALE_CLAMP):
+                                   scale_clamp: float = _DEFAULT_SCALE_CLAMP, transform: str = "delta"):
     """Sync-free, fixed-capacity form (CUDA tensors only): (boxes [N, D, 4], scores [N, D], classes [N, D], counts [N]) with
     D = max_detections_per_image, rows beyond counts[i] zero.  Launch sequence: per level one `where` + batched `topk`
     (library), then d2b_dense_prepare (decode + class ids + NMS offsets of ALL levels and images), memset + 3 NMS kernels,
-    d2b_rpn_select, one gather.  Static shapes: capturable in a CUDA graph."""
+    d2b_rpn_select, one gather.  Static shapes: capturable in a CUDA graph.
+    transform: "delta" decodes with Box2BoxTransform(box2box_weights, scale_clamp) (RetinaNet), "linear" with
+    Box2BoxTransformLinear(normalize_by_size=True) (FCOS; weights and scale_clamp unused)."""
     import ctypes as C
 
     from . import _C
@@ -104,11 +132,17 @@ def dense_detector_inference_fixed(anchors: List[torch.Tensor], pred_scores: Lis
     flat_boxes, nms_boxes = torch.empty((m, 4), **f32), torch.empty((m, 4), **f32)
     nms_scores, raw_scores = torch.empty((m,), **f32), torch.empty((m,), **f32)
     classes, cat_ids = torch.empty((m,), **i64), torch.empty((m,), **i64)
+    _check_transform(transform)
     w = (C.c_float * 4)(*[float(x) for x in box2box_weights])
     with torch.cuda.device(device):
-        check(_C.lib().d2b_dense_prepare(C.byref(lv), n, ncls, w, float(scale_clamp), ptr(flat_boxes), ptr(nms_boxes),
-                                         ptr(nms_scores), ptr(raw_scores), ptr(classes), ptr(cat_ids), stream_ptr(device)),
-              "dense_prepare")
+        if transform == "linear":
+            check(_C.lib().d2b_dense_prepare_linear(C.byref(lv), n, ncls, ptr(flat_boxes), ptr(nms_boxes), ptr(nms_scores),
+                                                    ptr(raw_scores), ptr(classes), ptr(cat_ids), stream_ptr(device)),
+                  "dense_prepare_linear")
+        else:
+            check(_C.lib().d2b_dense_prepare(C.byref(lv), n, ncls, w, float(scale_clamp), ptr(flat_boxes), ptr(nms_boxes),
+                                             ptr(nms_scores), ptr(raw_scores), ptr(classes), ptr(cat_ids),
+                                             stream_ptr(device)), "dense_prepare")
     out_boxes, out_scores, out_index, counts = nms_select(nms_boxes, nms_scores, cat_ids, flat_boxes, raw_scores, n, t, topk,
                                                           nms_thresh, False, max(t, 1))
     out_classes = classes[out_index.reshape(-1)].reshape(n, topk) if m else out_index
@@ -120,16 +154,18 @@ def dense_detector_inference(anchors: List[torch.Tensor], pred_scores: List[torc
                              pred_deltas: List[torch.Tensor], image_sizes: List[Tuple[int, int]], score_thresh: float,
                              topk_candidates: int, nms_thresh: float, max_detections_per_image: int,
                              box2box_weights: Sequence[float] = (1.0, 1.0, 1.0, 1.0),
-                             scale_clamp: float = _DEFAULT_SCALE_CLAMP) -> List[Detections]:
+                             scale_clamp: float = _DEFAULT_SCALE_CLAMP, transform: str = "delta") -> List[Detections]:
     """anchors[l]: (R_l, 4) anchors of level l; pred_scores[l]: (N, R_l, K) class scores (already sigmoid-ed);
     pred_deltas[l]: (N, R_l, 4) box regression outputs.  Returns one `Detections` per image with the fields of the
-    reference's `Instances` (pred_boxes, scores, pred_classes), in the reference's order (descending score)."""
+    reference's `Instances` (pred_boxes, scores, pred_classes), in the reference's order (descending score).
+    transform: "delta" (Box2BoxTransform, RetinaNet) or "linear" (Box2BoxTransformLinear, FCOS)."""
     if not pred_scores[0].is_cuda:
         return _dense_detector_inference_host(anchors, pred_scores, pred_deltas, image_sizes, score_thresh, topk_candidates,
-                                              nms_thresh, max_detections_per_image, box2box_weights, scale_clamp)
+                                              nms_thresh, max_detections_per_image, box2box_weights, scale_clamp,
+                                              transform)
     ob, osc, ocl, counts = dense_detector_inference_fixed(anchors, pred_scores, pred_deltas, len(image_sizes), score_thresh,
                                                           topk_candidates, nms_thresh, max_detections_per_image,
-                                                          box2box_weights, scale_clamp)
+                                                          box2box_weights, scale_clamp, transform)
     counts_host = counts.tolist()  # the one host sync: the reference contract returns exactly-sized results
     return [Detections(sz, ob[i, :counts_host[i]], osc[i, :counts_host[i]], ocl[i, :counts_host[i]])
             for i, sz in enumerate(image_sizes)]
@@ -139,9 +175,10 @@ def _dense_detector_inference_host(anchors: List[torch.Tensor], pred_scores: Lis
                                    pred_deltas: List[torch.Tensor], image_sizes: List[Tuple[int, int]], score_thresh: float,
                                    topk_candidates: int, nms_thresh: float, max_detections_per_image: int,
                                    box2box_weights: Sequence[float] = (1.0, 1.0, 1.0, 1.0),
-                                   scale_clamp: float = _DEFAULT_SCALE_CLAMP) -> List[Detections]:
+                                   scale_clamp: float = _DEFAULT_SCALE_CLAMP, transform: str = "delta") -> List[Detections]:
     """The same selection written with torch ops (host-logic restatement pinned to the real reference functions by
     tests/test_host_logic_cpu.py with the NMS replaced by the oracle; the CUDA path above is the product)."""
+    _check_transform(transform)
     num_images = len(image_sizes)
     device = pred_scores[0].device
     ncls = pred_scores[0].shape[2]
@@ -160,7 +197,10 @@ def _dense_detector_inference_host(anchors: List[torch.Tensor], pred_scores: Lis
         # 2. decode the selected boxes only (:226-230)
         sel_deltas = deltas_i[batch_idx[:, None], anchor_idxs]                       # N x k x 4
         sel_anchors = anchors_i[anchor_idxs]                                         # N x k x 4
-        decoded = apply_deltas(sel_deltas.reshape(-1, 4), sel_anchors.reshape(-1, 4), box2box_weights, scale_clamp)
+        if transform == "linear":
+            decoded = apply_deltas_linear(sel_deltas.reshape(-1, 4), sel_anchors.reshape(-1, 4))
+        else:
+            decoded = apply_deltas(sel_deltas.reshape(-1, 4), sel_anchors.reshape(-1, 4), box2box_weights, scale_clamp)
         boxes_l.append(decoded.reshape(n, k, 4))
         scores_l.append(top_s)
         cls_l.append(classes)

@@ -6,6 +6,8 @@
     over the valid anchors plus box regression, normalised by the EMA of the positive count (DenseDetector._ema_update).
   * `fast_rcnn_losses` / `fast_rcnn_losses_fixed` -- FastRCNNOutputLayers.losses / box_reg_loss and
     _log_classification_stats (roi_heads/fast_rcnn.py:88-115, 307-352, 424-463), for the standard, cascade and rotated heads.
+  * `fcos_loss_op` -- FCOS.losses (meta_arch/fcos.py:193-251) on the dense kernel with the linear GIoU and the centerness
+    term; its Python surface is detectron2_b200/fcos.py.
 
 The reference concatenates the levels, gathers the valid rows behind a boolean mask, builds an int64 one-hot target and
 reads the host about ten times per step (.item() counts, get_deltas' assertion, nonzero).  Here `d2b_dense_loss_*` reads the
@@ -32,7 +34,7 @@ from ._C import check, ptr, stream_ptr
 Tensor = torch.Tensor
 
 __all__ = ["rpn_losses", "rpn_losses_fixed", "retinanet_losses", "retinanet_losses_fixed", "fast_rcnn_losses",
-           "fast_rcnn_losses_fixed", "dense_loss_op", "frcnn_loss_op"]
+           "fast_rcnn_losses_fixed", "dense_loss_op", "frcnn_loss_op", "fcos_loss_op"]
 
 _SCALE_CLAMP = 4.135166556742356  # math.log(1000.0 / 16), box_regression.py:14
 
@@ -157,6 +159,101 @@ def _dense_bwd(ctx, g_cls, g_reg, *_):
 
 
 dense_loss_op.register_autograd(_dense_bwd, setup_context=_dense_setup)
+
+
+def _fcos_ctr(ctr: List[Tensor], logits: List[Tensor], dt: torch.dtype) -> List[Tensor]:
+    """Centerness logits [N, R_l] (or [N, R_l, 1]) of the logits' dtype, contiguous."""
+    if len(ctr) != len(logits):
+        raise ValueError("fcos_loss: one centerness tensor per level")
+    out = []
+    for c, x in zip(ctr, logits):
+        if c.shape not in ((x.shape[0], x.shape[1]), (x.shape[0], x.shape[1], 1)):
+            raise ValueError("fcos_loss: centerness must be [N, R_l] or [N, R_l, 1]")
+        out.append(c.reshape(x.shape[0], x.shape[1]).to(dt).contiguous())
+    return out
+
+
+def _ptr_array(ts: List[Tensor]):
+    return (C.c_void_p * max(len(ts), 1))(*[t.data_ptr() for t in ts])
+
+
+@torch.library.custom_op("d2b200::fcos_loss", mutates_args=(), device_types="cuda")
+def fcos_loss_op(logits: List[Tensor], deltas: List[Tensor], ctr: List[Tensor], anchors: Tensor, gt_boxes: Tensor,
+                 labels: Tensor, num_classes: int, gamma: float, alpha: float
+                 ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """FCOS.losses on the dense kernel: per level logits [N, R_l, K], deltas [N, R_l, 4] and centerness logits [N, R_l]
+    (fp32 / fp16 / bf16), anchors [R, 4], matched gt_boxes [N, R, 4], labels [N, R] int64 (K = background, -1 ignored).
+    Returns (cls_sum, reg_sum, ctr_sum, num_pos, status) as 0-dim device tensors (fp32 x3, int64, int32)."""
+    _C.require_cuda(anchors, gt_boxes, labels, *logits, *deltas, *ctr)
+    dt, xs, ds, an, gt, lab = _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, False)
+    cs = _fcos_ctr(ctr, xs, dt)
+    dev = an.device
+    n = gt.shape[0]
+    lv = _dense_levels(xs, ds)
+    cls_sum, reg_sum, ctr_sum = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(3))
+    num_pos = torch.empty((), dtype=torch.int64, device=dev)
+    status = torch.empty((), dtype=torch.int32, device=dev)
+    lib = _C.lib()
+    code = _C.DTYPE_CODE[dt]
+    ws_bytes = int(lib.d2b_fcos_loss_workspace_bytes(C.byref(lv), n, num_classes, code))
+    ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.d2b_fcos_loss_forward(C.byref(lv), _ptr_array(cs), n, num_classes, code, ptr(an), ptr(gt), ptr(lab),
+                                        float(gamma), float(alpha), ptr(cls_sum), ptr(reg_sum), ptr(ctr_sum), ptr(num_pos),
+                                        ptr(status), ptr(ws), ws_bytes, stream_ptr(dev)), "fcos_loss_forward")
+    return cls_sum, reg_sum, ctr_sum, num_pos, status
+
+
+@fcos_loss_op.register_fake
+def _(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, gamma, alpha):
+    e = anchors.new_empty
+    return (e((), dtype=torch.float32), e((), dtype=torch.float32), e((), dtype=torch.float32), e((), dtype=torch.int64),
+            e((), dtype=torch.int32))
+
+
+@torch.library.custom_op("d2b200::fcos_loss_backward", mutates_args=(), device_types="cuda")
+def fcos_loss_backward_op(logits: List[Tensor], deltas: List[Tensor], ctr: List[Tensor], anchors: Tensor, gt_boxes: Tensor,
+                          labels: Tensor, num_classes: int, gamma: float, alpha: float, grad_cls: Tensor,
+                          grad_reg: Tensor, grad_ctr: Tensor) -> List[Tensor]:
+    """Gradients of every level's logits, then deltas, then centerness logits, in the inputs' dtypes and shapes."""
+    dt, xs, ds, an, gt, lab = _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, False)
+    cs = _fcos_ctr(ctr, xs, dt)
+    dev = an.device
+    gxs = [torch.empty_like(x) for x in xs]
+    gds = [torch.empty_like(x) for x in ds]
+    gcs = [torch.empty_like(x) for x in cs]
+    lv = _dense_levels(xs, ds, gxs, gds)
+    g = [t.to(torch.float32).reshape(()).contiguous() for t in (grad_cls, grad_reg, grad_ctr)]
+    with torch.cuda.device(dev):
+        check(_C.lib().d2b_fcos_loss_backward(C.byref(lv), _ptr_array(cs), _ptr_array(gcs), gt.shape[0], num_classes,
+                                              _C.DTYPE_CODE[dt], ptr(an), ptr(gt), ptr(lab), float(gamma), float(alpha),
+                                              ptr(g[0]), ptr(g[1]), ptr(g[2]), stream_ptr(dev)), "fcos_loss_backward")
+    ins = list(logits) + list(deltas) + list(ctr)
+    return [gr.to(x.dtype).reshape(x.shape) for gr, x in zip(gxs + gds + gcs, ins)]
+
+
+@fcos_loss_backward_op.register_fake
+def _(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, gamma, alpha, grad_cls, grad_reg, grad_ctr):
+    return [torch.empty_like(t) for t in list(logits) + list(deltas) + list(ctr)]
+
+
+def _fcos_setup(ctx, inputs, output):
+    logits, deltas, ctr, anchors, gt_boxes, labels = inputs[:6]
+    ctx.save_for_backward(*logits, *deltas, *ctr, anchors, gt_boxes, labels)
+    ctx.num_levels = len(logits)
+    ctx.params = inputs[6:]
+
+
+def _fcos_bwd(ctx, g_cls, g_reg, g_ctr, *_):
+    saved = ctx.saved_tensors
+    nl = ctx.num_levels
+    logits, deltas, ctr = list(saved[:nl]), list(saved[nl:2 * nl]), list(saved[2 * nl:3 * nl])
+    anchors, gt_boxes, labels = saved[3 * nl:]
+    grads = fcos_loss_backward_op(logits, deltas, ctr, anchors, gt_boxes, labels, *ctx.params, g_cls, g_reg, g_ctr)
+    return (grads[:nl], grads[nl:2 * nl], grads[2 * nl:]) + (None,) * 6
+
+
+fcos_loss_op.register_autograd(_fcos_bwd, setup_context=_fcos_setup)
 
 
 def _frcnn_prepare(scores, deltas, proposals, gt_boxes, gt_classes):

@@ -275,6 +275,11 @@ int d2b_frcnn_prepare(const float* boxes, const float* scores, const int* row_st
 int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
                       float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
                       int64_t* cat_ids, void* stream);
+/* d2b_dense_prepare_linear: d2b_dense_prepare for FCOS (meta_arch/fcos.py:253-301), the same arguments without weights and
+ *   scale_clamp: the boxes are decoded by Box2BoxTransformLinear.apply_deltas (box_regression.py:275-307,
+ *   normalize_by_size): relu(deltas) times the anchor's (width, height), then the centre minus (l, t), plus (r, b). */
+int d2b_dense_prepare_linear(const d2b_dense_levels* lv, int N, int num_classes, float* flat_boxes, float* nms_boxes,
+                             float* nms_scores, float* raw_scores, int64_t* classes, int64_t* cat_ids, void* stream);
 
 /* ---- Rotated RRPN proposal selection and rotated Fast R-CNN inference around the NMS -----------------------------
  * Replace the per-image Python loops of detectron2/modeling/proposal_generator/rrpn.py:20-127 (find_top_rrpn_proposals)
@@ -337,6 +342,26 @@ int d2b_match_boxes(const float* gt_boxes, const int64_t* gt_count, int N, int G
                     const int64_t* gt_classes, int64_t num_classes, int64_t* matches, int8_t* match_labels,
                     float* matched_gt_boxes, int64_t* classes, int* status, void* workspace, size_t workspace_bytes,
                     void* stream);
+
+/* ---- FCOS point assignment -------------------------------------------------------------------------------------------
+ * Replaces FCOS._match_anchors + label_anchors (meta_arch/fcos.py:97-191) for all images in one launch, without the
+ * reference's [G,R,2] / [G,R,4] tensors.  anchors [R,4] fp32: the point boxes of every level concatenated (R = sum of the
+ * level_counts[num_levels], HOST, 1 <= num_levels <= D2B_MAX_LEVELS); gt_boxes [N,Gmax,4] fp32 with gt_count [N] (device,
+ * int64, clamped to [0, Gmax]; rows past it are never read), gt_classes [N,Gmax] int64.
+ * Per point (fp32): centre (a[:2] + a[2:]) / 2, size a[2] - a[0], lower bound 4 * size (0 on the first level), upper bound
+ * 8 * size (+inf on the last level; on every point when the last level is empty, as the reference's [-0:] slice).
+ * Per GT g: quality = float(max(|centre - centre_g|) < radius * size && min(l, t, r, b) > 0 && lower < max(l, t, r, b)
+ *   < upper) * (1e8 - area_g), radius = center_sampling_radius rounded to fp32, (l, t, r, b) the distances of the centre to
+ *   g's edges.  Boxes whose areas differ by less than the fp32 spacing at 1e8 tie; a GT with a non-finite area has NaN
+ *   quality at every point.
+ * Outputs [N,R]: matches int64 = torch.max(dim=0)'s argmax over GT (NaN beats every number, first index on ties), -1 when
+ *   the maximum is < 1e-5 (a NaN maximum is matched) or the image has no GT; labels int64 = gt_classes[match], num_classes
+ *   when unmatched; matched_gt_boxes [N,R,4] = gt_boxes[max(match, 0)] (GT 0 for the unmatched points of an image with GT,
+ *   zeros for an image without GT).
+ * No host synchronisation, static shapes: capturable in a CUDA graph.  All arguments are checked before the first CUDA call. */
+int d2b_fcos_assign(const float* anchors, const int* level_counts, int num_levels, const float* gt_boxes,
+                    const int64_t* gt_count, int N, int Gmax, const int64_t* gt_classes, int64_t num_classes,
+                    double center_sampling_radius, int64_t* matches, int64_t* labels, float* matched_gt_boxes, void* stream);
 
 /* ---- Sampling of the training labels --------------------------------------------------------------------------------
  * Replaces subsample_labels (modeling/sampling.py:9-54) and the per-image loops around it in RPN._subsample_labels
@@ -474,6 +499,25 @@ int d2b_dense_loss_forward(const d2b_dense_loss_levels* lv, int N, int K, int bo
 int d2b_dense_loss_backward(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int dtype, const float* anchors,
                             const float* gt_boxes, const void* labels, int label_kind, float gamma, float alpha, float beta,
                             int loss_type, float scale_clamp, const float* weights, const float* grad_cls, const float* grad_reg, void* stream);
+/* FCOS: FCOS.losses + compute_ctrness_targets (meta_arch/fcos.py:193-251) on the dense kernel, xyxy boxes and D2B_LABELS_I64
+ *   labels [N,R] (-1 ignored, 0..K-1 positive, K background; e.g. d2b_fcos_assign's).  cls_sum as the dense loss
+ *   (sigmoid_focal_loss with gamma, alpha); reg_sum = fvcore giou_loss of the deltas decoded by Box2BoxTransformLinear
+ *   (relu(deltas) * stride; the relu gradient is 0 at <= 0) over the positive rows, INVALID_BOX_ORDER where fvcore asserts;
+ *   ctr_sum = binary_cross_entropy_with_logits of ctr[l] [N,R_l] (`dtype`, read in place) over the positive rows against
+ *   sqrt((min(l,r) / max(l,r)) * (min(t,b) / max(t,b))), (l,t,r,b) = Box2BoxTransformLinear.get_deltas(anchor, gt box).
+ *   num_pos = the positive rows.  ctr / grad_ctr: HOST arrays of lv->num_levels device pointers.  workspace:
+ *   d2b_fcos_loss_workspace_bytes(lv, N, K, dtype) bytes, 16-byte aligned.  Backward: grad_cls / grad_reg / grad_ctr_sum
+ *   (device scalars); lv->grad_logits, lv->grad_deltas and grad_ctr are fully written (0 on non-positive rows for the
+ *   deltas and the centerness, sigmoid(x) - t times grad_ctr_sum on the positive ones). */
+size_t d2b_fcos_loss_workspace_bytes(const d2b_dense_loss_levels* lv, int N, int K, int dtype);
+int d2b_fcos_loss_forward(const d2b_dense_loss_levels* lv, const void* const* ctr, int N, int K, int dtype,
+                          const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma, float alpha,
+                          float* cls_sum, float* reg_sum, float* ctr_sum, int64_t* num_pos, int* status, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int d2b_fcos_loss_backward(const d2b_dense_loss_levels* lv, const void* const* ctr, void* const* grad_ctr, int N, int K,
+                           int dtype, const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma,
+                           float alpha, const float* grad_cls, const float* grad_reg, const float* grad_ctr_sum,
+                           void* stream);
 size_t d2b_frcnn_loss_workspace_bytes(int R);
 int d2b_frcnn_loss_forward(const void* scores, const void* deltas, int R, int K, int kreg, int box_dim, int dtype,
                            const float* proposals, const float* gt_boxes, const int64_t* gt_classes, float beta,
