@@ -44,7 +44,7 @@ def _compile(name, extra, force):
     src = os.path.join(CSRC, name)
     obj = os.path.join(OBJ, name.replace(".cu", ".o"))
     deps = [src, os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "tc_common.cuh"),
-            os.path.join(CSRC, "deform_conv_tc.cuh"), os.path.join(CSRC, "rotated_iou.cuh"), os.path.join(CSRC, "box_decode.cuh"),
+            os.path.join(CSRC, "deform_conv_tc.cuh"), os.path.join(CSRC, "rotated_iou.cuh"), os.path.join(CSRC, "boxes.cuh"),
             os.path.join(HERE, "..", "include", "d2b200.h"), __file__]
     if force or _stale(obj, deps):
         cmd = [NVCC] + ARCH + COMMON + extra + ["-c", src, "-o", obj]

@@ -1,5 +1,7 @@
 // Shared helpers for the sm_90a kernels behind include/d2b200.h.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -22,6 +24,60 @@
   } while (0)
 
 __host__ __device__ static inline int d2b_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// Element type of an ABI dtype code (D2B_F32 / D2B_F16 / D2B_BF16): half-precision tensors are read and written in place,
+// with fp32 arithmetic, instead of a separate cast pass per tensor.  ld(const T*) reads through the read-only data cache;
+// ld(T) widens a value already in registers.
+template <int DT>
+struct Elem;
+template <>
+struct Elem<D2B_F32> {
+  using T = float;
+  static __device__ __forceinline__ float ld(const T* __restrict__ p) { return __ldg(p); }
+  static __device__ __forceinline__ float ld(T v) { return v; }
+  static __device__ __forceinline__ T st(float v) { return v; }
+};
+template <>
+struct Elem<D2B_F16> {
+  using T = __half;
+  static __device__ __forceinline__ float ld(const T* __restrict__ p) { return __half2float(__ldg(p)); }
+  static __device__ __forceinline__ float ld(T v) { return __half2float(v); }
+  static __device__ __forceinline__ T st(float v) { return __float2half_rn(v); }
+};
+template <>
+struct Elem<D2B_BF16> {
+  using T = __nv_bfloat16;
+  static __device__ __forceinline__ float ld(const T* __restrict__ p) { return __bfloat162float(__ldg(p)); }
+  static __device__ __forceinline__ float ld(T v) { return __bfloat162float(v); }
+  static __device__ __forceinline__ T st(float v) { return __float2bfloat16_rn(v); }
+};
+
+// Exclusive prefix sum of one value per thread over the CTA (shuffle scan inside the warps); `total` receives the sum
+// over the CTA.  warp_tot: 32 elements of shared memory.  blockDim.x <= 1024, multiple of 32; every thread calls it.
+// Barriers: the one inside separates the warp totals' writes from their reads.  Nothing follows the reads, so a caller
+// that writes warp_tot again -- a second call included -- puts a __syncthreads() between this call and that write.
+template <class T>
+__device__ __forceinline__ T block_exclusive_scan(T v, T* __restrict__ warp_tot, T& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  T inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  if (lane == 31) warp_tot[warp] = inc;
+  __syncthreads();
+  const T wt = lane < nwarps ? warp_tot[lane] : T(0);
+  T winc = wt;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T t = __shfl_up_sync(0xffffffffu, winc, o);
+    if (lane >= o) winc += t;
+  }
+  total = __shfl_sync(0xffffffffu, winc, 31);
+  const T wbase = __shfl_sync(0xffffffffu, winc, warp) - __shfl_sync(0xffffffffu, wt, warp);
+  return wbase + inc - v;
+}
 
 // SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe): grid sizing in waves.  Queried once per device
 // ordinal and cached, so it costs no CUDA call inside a graph capture after the first eager call (abi.cu).

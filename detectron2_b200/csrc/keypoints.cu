@@ -25,9 +25,6 @@
 // four-tap sums, whose first FMA adds x0 * c0 to the rounded x1 * c1) is the one the sm_90 SASS of that kernel in
 // libtorch_cuda.so shows; on an H100 it reproduced PyTorch's CUDA bicubic output bit for bit over every pixel tested,
 // where each other candidate pattern missed some.
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
 #include <climits>
 
 #include "common.cuh"
@@ -264,23 +261,6 @@ __global__ void __launch_bounds__(kThreads) keypoints_finish_kernel(const float*
 }
 
 // ---- keypoint loss ------------------------------------------------------------------------------------------------
-template <int DT> struct Elem;
-template <> struct Elem<D2B_F32> {
-  using T = float;
-  static __device__ __forceinline__ float ld(const T* p) { return __ldg(p); }
-  static __device__ __forceinline__ T st(float v) { return v; }
-};
-template <> struct Elem<D2B_F16> {
-  using T = __half;
-  static __device__ __forceinline__ float ld(const T* p) { return __half2float(__ldg(p)); }
-  static __device__ __forceinline__ T st(float v) { return __float2half_rn(v); }
-};
-template <> struct Elem<D2B_BF16> {
-  using T = __nv_bfloat16;
-  static __device__ __forceinline__ float ld(const T* p) { return __bfloat162float(__ldg(p)); }
-  static __device__ __forceinline__ T st(float v) { return __float2bfloat16_rn(v); }
-};
-
 // One coordinate of _keypoints_to_heatmap: floor((c - lo) * (S / (hi - lo))), where torch evaluates S / t as
 // t.reciprocal() * S; c == hi maps to S - 1.  Returns -1 when the cell is outside [0, S).
 __device__ __forceinline__ int heatmap_cell(float c, float lo, float hi, int S) {

@@ -16,13 +16,10 @@
 //
 // Reductions are deterministic (per-CTA partials, no float atomics): loss and gradients are bitwise reproducible.
 // Compiled with -fmad=false so that the targets round like the reference's separate torch ops.
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
 #include <climits>
 #include <cmath>
 
-#include "box_decode.cuh"
+#include "boxes.cuh"
 #include "common.cuh"
 
 namespace {
@@ -31,63 +28,9 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr int kItems = 4;  // 16-byte vectors per thread in one classification CTA
 
-template <int DT> struct Elem;
-template <> struct Elem<D2B_F32> {
-  using T = float;
-  static __device__ __forceinline__ float ld(T v) { return v; }
-  static __device__ __forceinline__ T st(float v) { return v; }
-};
-template <> struct Elem<D2B_F16> {
-  using T = __half;
-  static __device__ __forceinline__ float ld(T v) { return __half2float(v); }
-  static __device__ __forceinline__ T st(float v) { return __float2half_rn(v); }
-};
-template <> struct Elem<D2B_BF16> {
-  using T = __nv_bfloat16;
-  static __device__ __forceinline__ float ld(T v) { return __bfloat162float(v); }
-  static __device__ __forceinline__ T st(float v) { return __float2bfloat16_rn(v); }
-};
-
 template <class T> struct alignas(16) Vec {
   static constexpr int N = 16 / sizeof(T);
   T v[N];
-};
-
-// ---- box targets: the box types of postproc.cu / match.cu, here with the reference's get_deltas --------------------
-struct BoxWeights {
-  float w[5];  // RotBox: w[4] = wa * pi / 180 rounded to fp32, the scalar torch multiplies by
-};
-
-// Box2BoxTransform.get_deltas (box_regression.py:43-76), op for op; the source width decides the assertion.
-struct XyxyBox {
-  static constexpr int D = 4;
-  static __device__ __forceinline__ float src_width(const float* s) { return s[2] - s[0]; }
-  static __device__ __forceinline__ void deltas(const float* s, const float* t, const BoxWeights& w, float* d) {
-    const float sw = s[2] - s[0], sh = s[3] - s[1];
-    const float scx = s[0] + 0.5f * sw, scy = s[1] + 0.5f * sh;
-    const float tw = t[2] - t[0], th = t[3] - t[1];
-    const float tcx = t[0] + 0.5f * tw, tcy = t[1] + 0.5f * th;
-    d[0] = w.w[0] * (tcx - scx) / sw;
-    d[1] = w.w[1] * (tcy - scy) / sh;
-    d[2] = w.w[2] * logf(tw / sw);
-    d[3] = w.w[3] * logf(th / sh);
-  }
-};
-
-// Box2BoxTransformRotated.get_deltas (box_regression.py:145-180) on (cx, cy, w, h, angle_deg).
-struct RotBox {
-  static constexpr int D = 5;
-  static __device__ __forceinline__ float src_width(const float* s) { return s[2]; }
-  static __device__ __forceinline__ void deltas(const float* s, const float* t, const BoxWeights& w, float* d) {
-    d[0] = w.w[0] * (t[0] - s[0]) / s[2];
-    d[1] = w.w[1] * (t[1] - s[1]) / s[3];
-    d[2] = w.w[2] * logf(t[2] / s[2]);
-    d[3] = w.w[3] * logf(t[3] / s[3]);
-    // (da + 180) % 360 - 180 with torch.remainder: fmod, plus the divisor when the signs differ
-    float m = fmodf((t[4] - s[4]) + 180.f, 360.f);
-    if (m != 0.f && m < 0.f) m += 360.f;
-    d[4] = (m - 180.f) * w.w[4];
-  }
 };
 
 // fvcore smooth_l1_loss: |d| for beta < 1e-5, else 0.5 d^2 / beta inside |d| < beta and |d| - 0.5 beta outside.
@@ -450,7 +393,7 @@ __global__ void __launch_bounds__(kThreads) dense_loss_kernel(const DenseLevels 
       const long long lab = labels[row];
       const float* an = A.anchors + (size_t)a * D;
       // get_deltas' assertion covers every anchor (smooth-L1 only: the GIoU branch decodes, it has no targets)
-      if (!A.giou && n == 0 && !(Box::src_width(an) > 0.f)) status |= D2B_LOSS_STATUS_INVALID_BOX;
+      if (!A.giou && n == 0 && !(Box::width(an) > 0.f)) status |= D2B_LOSS_STATUS_INVALID_BOX;
       if (!Lab::in_range(lab, A.K)) status |= D2B_LOSS_STATUS_INVALID_CLASS;
       const bool pos = Lab::pos(lab, A.K);
       cnt[0] = pos ? 1 : 0;
@@ -483,7 +426,7 @@ __global__ void __launch_bounds__(kThreads) dense_loss_kernel(const DenseLevels 
         }
         if (!A.giou) {
           float t[D];
-          Box::deltas(an, A.gt_boxes + (size_t)row * D, A.w, t);
+          Box::get_deltas(an, A.gt_boxes + (size_t)row * D, A.w, t);
 #pragma unroll
           for (int q = 0; q < D; ++q) s_reg += smooth_l1(E::ld(dl[q]) - t[q], A.beta, g[q]);
         }
@@ -606,9 +549,9 @@ __global__ void __launch_bounds__(kThreads) frcnn_loss_kernel(const FrcnnArgs A)
     }
     if (!A.giou && fg && lane < D) {
       const float* pr = A.proposals + (size_t)r * D;
-      if (lane == 0 && !(Box::src_width(pr) > 0.f)) status |= D2B_LOSS_STATUS_INVALID_BOX;
+      if (lane == 0 && !(Box::width(pr) > 0.f)) status |= D2B_LOSS_STATUS_INVALID_BOX;
       float t[D];
-      Box::deltas(pr, A.gt_boxes + (size_t)r * D, A.w, t);
+      Box::get_deltas(pr, A.gt_boxes + (size_t)r * D, A.w, t);
       float tq = t[0];
 #pragma unroll
       for (int q = 1; q < D; ++q) tq = lane == q ? t[q] : tq;

@@ -23,48 +23,19 @@
 //                       the classes (1 -> gt_classes[match], 0 -> num_classes, -1 -> -1; an image without GT: num_classes).
 //
 // The box type is a template policy (XyxyBox: pairwise_iou of structures/boxes.py:312-358 op for op; RotBox: the rotated IoU
-// of nms.cu, shared through rotated_iou.cuh).  Compiled with -fmad=false like nms.cu / postproc.cu: bit-exact IoUs.
+// of nms.cu; boxes.cuh).  Compiled with -fmad=false like nms.cu / postproc.cu: bit-exact IoUs.
 //
 // d2b_fcos_assign (FCOS._match_anchors + label_anchors, meta_arch/fcos.py:97-191) shares the GT tiling: one launch,
 // fcos_assign_kernel, one thread per (image, point), no G x R matrix; the quality and its argmax are bit-exact.
 #include <climits>
 
+#include "boxes.cuh"
 #include "common.cuh"
-#include "rotated_iou.cuh"
 
 namespace {
 
 constexpr int kThreads = 256;  // predictions per CTA
 constexpr int kTile = 256;     // GT boxes staged per shared-memory tile
-
-// torch.min / torch.max propagate NaN; fminf / fmaxf would drop it
-__device__ __forceinline__ float nan_min(float a, float b) { return (a != a || b != b) ? a + b : fminf(a, b); }
-__device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? a + b : fmaxf(a, b); }
-
-struct XyxyBox {
-  static constexpr int D = 4;
-  static constexpr bool kRotated = false;
-  // pairwise_iou(boxes1 = gt, boxes2 = prediction): the same fp32 operations in the same order
-  static __device__ __forceinline__ float iou(const float* __restrict__ g, const float* __restrict__ a) {
-    const float area1 = (g[2] - g[0]) * (g[3] - g[1]);
-    const float area2 = (a[2] - a[0]) * (a[3] - a[1]);
-    float w = nan_min(g[2], a[2]) - nan_max(g[0], a[0]);
-    float h = nan_min(g[3], a[3]) - nan_max(g[1], a[1]);
-    w = w < 0.f ? 0.f : w;  // clamp_(min=0): NaN stays NaN
-    h = h < 0.f ? 0.f : h;
-    const float inter = w * h;
-    return inter > 0.f ? inter / (area1 + area2 - inter) : 0.f;
-  }
-};
-
-struct RotBox {
-  static constexpr int D = 5;
-  static constexpr bool kRotated = true;
-  // box_iou_rotated(boxes1 = gt, boxes2 = prediction)[g, a]
-  static __device__ __forceinline__ float iou(const float* __restrict__ g, const float* __restrict__ a) {
-    return rotated_iou(g, a);
-  }
-};
 
 struct MatchArgs {
   const float* gt;               // [N, Gmax, D]

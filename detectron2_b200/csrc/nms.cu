@@ -353,30 +353,6 @@ constexpr int kScanThreads = 512;
 constexpr int kScanWarps = kScanThreads / 32;
 constexpr int kMaxColsPerWarp = 10;  // register-prefetched column words per warp (covers segments <= 64*16*10 = 10240)
 
-// Exclusive prefix sum of one int per thread over the CTA (shuffle scan inside the warps, one barrier); `total` receives
-// the sum over the CTA.  warp_tot: 32 ints of shared memory.  blockDim.x <= 1024, multiple of 32.
-__device__ __forceinline__ int block_excl_scan(int v, int* __restrict__ warp_tot, int& total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) warp_tot[warp] = inc;
-  __syncthreads();
-  const int wt = lane < nwarps ? warp_tot[lane] : 0;
-  int winc = wt;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, winc, o);
-    if (lane >= o) winc += t;
-  }
-  total = __shfl_sync(0xffffffffu, winc, 31);
-  const int wbase = __shfl_sync(0xffffffffu, winc, warp) - __shfl_sync(0xffffffffu, wt, warp);
-  return wbase + inc - v;
-}
-
 // ---- kernel 3: greedy scan over the bitmask, one CTA per category segment (plain NMS = one segment), then -- in the CTA
 // that finishes last -- compaction of the kept boxes in global score order.
 // dynamic smem: removed[] (uint64), one word per 64-box block of the segment.  Per block b: (B) warp 0 resolves the greedy
@@ -516,7 +492,7 @@ __global__ void __launch_bounds__(kScanThreads, 1) nms_scan_kernel(const unsigne
   int cnt = 0;
   for (int r = r0; r < r1; ++r) cnt += kf[r] ? 1 : 0;
   int total;
-  int idx = block_excl_scan(cnt, warp_tot, total);
+  int idx = block_exclusive_scan(cnt, warp_tot, total);
   for (int r = r0; r < r1; ++r)
     if (kf[r]) keep[idx++] = (long long)orig_of_grank[r];
   for (int r = total + tid; r < M; r += kScanThreads) keep[r] = 0;  // deterministic padding

@@ -14,13 +14,13 @@
 // sync-free launch sequence with static shapes: capturable in a CUDA graph; the reference loops over images in Python
 // with boolean indexing and one `.item()` per image.  Compiled with -fmad=false like nms.cu (bit-exact clip / offsets).
 //
-// The box type is a template policy (XyxyBox / RotBox below) of every candidate and selection kernel in this file:
+// The box type is a template policy (XyxyBox / RotBox, boxes.cuh) of every candidate and selection kernel in this file:
 // rpn_prepare_kernel, frcnn_prepare_kernel (d2b_frcnn_prepare / d2b_frcnn_rotated_prepare) and rpn_select_kernel; the
 // rotated calls run d2b_nms with D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET.
 #include <climits>
 #include <type_traits>
 
-#include "box_decode.cuh"
+#include "boxes.cuh"
 #include "common.cuh"
 
 namespace {
@@ -36,122 +36,6 @@ struct RpnLevels {
 };
 
 __device__ __forceinline__ bool finitef(float v) { return fabsf(v) <= 3.402823466e38f; }  // false for inf and NaN
-
-// Box policies of the candidate kernels: layout, the reference's clip, and the batched-NMS coordinate offsets, per box type.
-//   XyxyBox  Boxes (x1, y1, x2, y2): clip = clamp to the image; torchvision's offsets idx * (max coordinate + 1) on all four.
-//   RotBox   RotatedBoxes (cx, cy, w, h, angle_deg): RotatedBoxes.clip (structures/rotated_boxes.py:248-303); the offsets of
-//            batched_nms_rotated (layers/nms.py:137-146), idx * (max - min + 1), on the centre only.
-struct XyxyBox {
-  static constexpr int D = 4;
-  static constexpr bool kRotated = false;
-  float v[4];
-  __device__ __forceinline__ void clip(float ih, float iw) {  // clamp(min=0, max=w / h)
-    v[0] = fminf(fmaxf(v[0], 0.f), iw);
-    v[1] = fminf(fmaxf(v[1], 0.f), ih);
-    v[2] = fminf(fmaxf(v[2], 0.f), iw);
-    v[3] = fminf(fmaxf(v[3], 0.f), ih);
-  }
-  __device__ __forceinline__ float width() const { return v[2] - v[0]; }
-  __device__ __forceinline__ float height() const { return v[3] - v[1]; }
-  __device__ __forceinline__ float hi() const { return fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])); }  // boxes.max()
-  __device__ __forceinline__ float lo() const { return 0.f; }                                          // not part of the range
-  static __device__ __forceinline__ float scale(bool any, float mx, float) { return (any ? mx : 0.f) + 1.0f; }
-  __device__ __forceinline__ void shift(float off) {
-    v[0] += off;
-    v[1] += off;
-    v[2] += off;
-    v[3] += off;
-  }
-};
-
-struct RotBox {
-  static constexpr int D = 5;
-  static constexpr bool kRotated = true;
-  float v[5];
-  __device__ __forceinline__ void clip(float ih, float iw) {
-    // normalize_angles: (a + 180) % 360 - 180 with torch's float remainder (the result takes the divisor's sign)
-    float m = fmodf(v[4] + 180.f, 360.f);
-    if (m < 0.f) m += 360.f;
-    v[4] = m - 180.f;
-    if (fabsf(v[4]) <= 1.0f) {  // clip_angle_threshold: only near-horizontal boxes are clipped, as xyxy boxes
-      const float x1 = fminf(fmaxf(v[0] - v[2] / 2.f, 0.f), iw), y1 = fminf(fmaxf(v[1] - v[3] / 2.f, 0.f), ih);
-      const float x2 = fminf(fmaxf(v[0] + v[2] / 2.f, 0.f), iw), y2 = fminf(fmaxf(v[1] + v[3] / 2.f, 0.f), ih);
-      v[0] = (x1 + x2) / 2.f;
-      v[1] = (y1 + y2) / 2.f;
-      v[2] = fminf(v[2], x2 - x1);  // widths and heights never grow through rounding
-      v[3] = fminf(v[3], y2 - y1);
-    }
-  }
-  __device__ __forceinline__ float width() const { return v[2]; }
-  __device__ __forceinline__ float height() const { return v[3]; }
-  __device__ __forceinline__ float hi() const { return fmaxf(v[0], v[1]) + fmaxf(v[2], v[3]) / 2; }
-  __device__ __forceinline__ float lo() const { return fminf(v[0], v[1]) - fmaxf(v[2], v[3]) / 2; }
-  static __device__ __forceinline__ float scale(bool any, float mx, float mn) { return (any ? mx - mn : 0.f) + 1.0f; }
-  __device__ __forceinline__ void shift(float off) {
-    v[0] += off;
-    v[1] += off;
-  }
-};
-
-template <class Box>
-__device__ __forceinline__ Box load_box(const float* __restrict__ p) {  // scalar loads: rows of the inputs need no alignment
-  Box b;
-#pragma unroll
-  for (int q = 0; q < Box::D; ++q) b.v[q] = p[q];
-  return b;
-}
-
-template <class Box>
-__device__ __forceinline__ Box load_box_aligned(const float* __restrict__ p) {  // xyxy buffers are 16-byte aligned
-  if constexpr (Box::D == 4) {
-    const float4 q = *reinterpret_cast<const float4*>(p);
-    return Box{{q.x, q.y, q.z, q.w}};
-  } else {
-    return load_box<Box>(p);
-  }
-}
-
-template <class Box>
-__device__ __forceinline__ void store_box(float* __restrict__ p, const Box& b) {  // xyxy buffers are 16-byte aligned
-  if constexpr (Box::D == 4) {
-    *reinterpret_cast<float4*>(p) = make_float4(b.v[0], b.v[1], b.v[2], b.v[3]);
-  } else {
-#pragma unroll
-    for (int q = 0; q < Box::D; ++q) p[q] = b.v[q];
-  }
-}
-
-template <class Box>
-__device__ __forceinline__ Box zero_box() {
-  Box b;
-#pragma unroll
-  for (int q = 0; q < Box::D; ++q) b.v[q] = 0.f;
-  return b;
-}
-
-// Exclusive prefix sum of one int per thread over a 1024-thread CTA; `total` = sum.
-__device__ __forceinline__ int block_scan(int v, int* __restrict__ warp_tot, int& total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  __syncthreads();  // warp_tot reuse between calls
-  if (lane == 31) warp_tot[warp] = inc;
-  __syncthreads();
-  const int wt = warp_tot[lane];
-  int winc = wt;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, winc, o);
-    if (lane >= o) winc += t;
-  }
-  total = __shfl_sync(0xffffffffu, winc, 31);
-  const int wbase = __shfl_sync(0xffffffffu, winc, warp) - __shfl_sync(0xffffffffu, wt, warp);
-  return wbase + inc - v;
-}
 
 // D = 4: xyxy boxes (d2b_rpn_select), D = 5: rotated boxes (d2b_rpn_select_rotated).
 template <int D>
@@ -176,7 +60,8 @@ __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* _
       mine = (kidx / T == n && cat_ids[kidx] >= 0) ? 1 : 0;
     }
     int total;
-    const int rank = have + block_scan(mine, warp_tot, total);
+    __syncthreads();  // the previous scan is done reading warp_tot
+    const int rank = have + block_exclusive_scan(mine, warp_tot, total);
     if (mine && rank < post_topk) {
       const size_t o = (size_t)n * post_topk + rank;
       store_box(out_boxes + o * D, load_box_aligned<Box>(flat_boxes + (size_t)kidx * D));
@@ -305,8 +190,10 @@ __global__ void __launch_bounds__(kThreads) frcnn_prepare_kernel(const FrcnnImag
         for (int c = 0; c < K; ++c) cnt += srow[c] > score_thresh ? 1 : 0;
     }
     int total, total_rows;
-    const int off = have + block_scan(cnt, warp_tot, total);
-    const int vrank = have_rows + block_scan(valid, warp_tot, total_rows);
+    __syncthreads();  // the previous scan is done reading warp_tot
+    const int off = have + block_exclusive_scan(cnt, warp_tot, total);
+    __syncthreads();
+    const int vrank = have_rows + block_exclusive_scan(valid, warp_tot, total_rows);
     if (r < R) row_map[rs + r] = valid ? vrank : -1;  // index of the row among the valid rows (:138-140)
     if (cnt) {
       int pos = off;
@@ -382,7 +269,7 @@ __global__ void __launch_bounds__(kThreads) rpn_prepare_kernel(const RpnLevels P
 #pragma unroll
     for (int q = 0; q < D; ++q) fin = fin && finitef(b.v[q]);
     b.clip(ih, iw);
-    const bool valid = fin && b.width() > min_box_size && b.height() > min_box_size;
+    const bool valid = fin && Box::width(b.v) > min_box_size && Box::height(b.v) > min_box_size;
     const size_t o = (size_t)n * T + t;
     store_box(flat_boxes + o * D, valid ? b : zero_box<Box>());
     raw_scores[o] = s;

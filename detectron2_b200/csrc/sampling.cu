@@ -99,33 +99,6 @@ __global__ void __launch_bounds__(kThreads) hist_kernel(const SampleArgs a) {
     if (h[t]) atomicAdd(&g[t], h[t]);
 }
 
-// Block-wide exclusive scan of one value per thread (blockDim.x = kBins); returns the exclusive prefix, *total the sum.
-__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned* s_warp, unsigned* total) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  unsigned x = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const unsigned y = __shfl_up_sync(0xffffffffu, x, d);
-    if (lane >= d) x += y;
-  }
-  if (lane == 31) s_warp[w] = x;
-  __syncthreads();
-  if (w == 0) {
-    unsigned t = lane < (int)(blockDim.x >> 5) ? s_warp[lane] : 0u;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const unsigned y = __shfl_up_sync(0xffffffffu, t, d);
-      if (lane >= d) t += y;
-    }
-    s_warp[lane] = t;  // inclusive prefix over the warps
-  }
-  __syncthreads();
-  const unsigned before = (w ? s_warp[w - 1] : 0u) + x - v;
-  *total = s_warp[(blockDim.x >> 5) - 1];
-  __syncthreads();
-  return before;
-}
-
 // The bin whose [before, before + count) contains the need-th smallest key (need >= 1): one thread of the block finds it.
 __device__ __forceinline__ void find_bin(unsigned before, unsigned count, unsigned need, int* s_bin, unsigned* s_below,
                                          unsigned* s_count) {
@@ -144,8 +117,10 @@ __global__ void __launch_bounds__(kBins) thresh_kernel(const SampleArgs a) {
   const unsigned* g = a.hist + (size_t)n * 2 * kBins;
   const unsigned hp = g[t], hn = g[kBins + t];
   unsigned npos, nneg;
-  const unsigned before_p = block_exclusive_scan(hp, s_warp, &npos);
-  const unsigned before_n = block_exclusive_scan(hn, s_warp, &nneg);
+  const unsigned before_p = block_exclusive_scan(hp, s_warp, npos);
+  __syncthreads();  // s_warp reuse
+  const unsigned before_n = block_exclusive_scan(hn, s_warp, nneg);
+  __syncthreads();
   // sampling.py:41-47: k_pos = min(#pos, int(num_samples * positive_fraction)), k_neg = min(#neg, num_samples - k_pos)
   const int k_pos = (int)min((unsigned)a.max_pos, npos);
   const int k_neg = (int)min((unsigned)(a.num_samples - k_pos), nneg);
@@ -237,7 +212,8 @@ __global__ void __launch_bounds__(kFinishThreads) finish_kernel(const SampleArgs
       if (t == 0) s_count = 0u;
       unsigned total;
       const unsigned v = h[t];
-      const unsigned before = block_exclusive_scan(v, s_warp, &total);
+      const unsigned before = block_exclusive_scan(v, s_warp, total);
+      __syncthreads();
       find_bin(before, v, need, &s_bin, &s_below, &s_count);
       __syncthreads();
       const unsigned long long b = (unsigned long long)s_bin;

@@ -30,6 +30,7 @@ from torch.nn import functional as F
 
 from . import _C
 from ._C import check, ptr, stream_ptr
+from .dense_inference import apply_deltas as _apply_deltas
 
 Tensor = torch.Tensor
 
@@ -524,25 +525,6 @@ def _get_deltas(src: Tensor, tgt: Tensor, weights: Sequence[float]) -> Tensor:
         out = [wx * (tx - sx) / sw, wy * (ty - sy) / sh, ww * torch.log(tw / sw), wh * torch.log(th / sh)]
     assert bool((sw > 0).all()), "Input boxes to %s are not valid!" % _transform_name(src.shape[-1])
     return torch.stack(out, dim=1)
-
-
-def _apply_deltas(deltas: Tensor, boxes: Tensor, weights: Sequence[float], scale_clamp: float) -> Tensor:
-    """Box2BoxTransform.apply_deltas (box_regression.py:78-116) for [R, 4] deltas."""
-    deltas = deltas.float()
-    boxes = boxes.to(deltas.dtype)
-    widths = boxes[:, 2] - boxes[:, 0]
-    heights = boxes[:, 3] - boxes[:, 1]
-    ctr_x = boxes[:, 0] + 0.5 * widths
-    ctr_y = boxes[:, 1] + 0.5 * heights
-    wx, wy, ww, wh = weights
-    dx, dy = deltas[:, 0::4] / wx, deltas[:, 1::4] / wy
-    dw = torch.clamp(deltas[:, 2::4] / ww, max=scale_clamp)
-    dh = torch.clamp(deltas[:, 3::4] / wh, max=scale_clamp)
-    px = dx * widths[:, None] + ctr_x[:, None]
-    py = dy * heights[:, None] + ctr_y[:, None]
-    pw = torch.exp(dw) * widths[:, None]
-    ph = torch.exp(dh) * heights[:, None]
-    return torch.stack((px - 0.5 * pw, py - 0.5 * ph, px + 0.5 * pw, py + 0.5 * ph), dim=-1).reshape(deltas.shape)
 
 
 def _smooth_l1_loss(input: Tensor, target: Tensor, beta: float) -> Tensor:
