@@ -371,27 +371,31 @@ __global__ void __launch_bounds__(256) dcn_bias_grad_kernel(const float* __restr
   }
 }
 
-}  // namespace
-
-// precision: 0 = fp32 FFMA, 1 = bf16x3 on wgmma, 2 = bf16 on wgmma, -1 = auto (1 when the tensor-core kernels take
-// the shape, else 0 -- both are fp32-class, so "auto" never lowers accuracy)
-D2B_API int d2b_deform_conv_tc_shape_supported(const d2b_dcn_params* p, int backward) {
-  return backward ? d2b_deform_conv_tc_bwd_supported(p) : d2b_deform_conv_tc_supported(p);
+// precision: 0 = fp32 FFMA, 1 = bf16x3 on wgmma, 2 = bf16 on wgmma, -1 = auto.  Auto is 1 when the tensor-core kernels take
+// the shape in every direction `dirs` names, else 0 -- both are fp32-class, so "auto" never lowers accuracy.  The fused ops
+// have no FFMA path and name no direction: their auto is 1.  Saved columns are written by the forward and read by the
+// backward, so they name both.  Other values are returned as they are; the calls reject those outside [-1, 2].
+enum { kFused = 0, kFwd = 1, kBwd = 2 };
+int dcn_precision(const d2b_dcn_params* p, int precision, int dirs) {
+  if (precision != -1) return precision;
+  const bool fwd = !(dirs & kFwd) || d2b_deform_conv_tc_shape_supported(p, 0);
+  const bool bwd = !(dirs & kBwd) || d2b_deform_conv_tc_shape_supported(p, 1);
+  return fwd && bwd ? 1 : 0;
 }
 
+}  // namespace
+
 D2B_API size_t d2b_deform_conv_forward_workspace_bytes(const d2b_dcn_params* p, int precision, int flags) {
-  if (precision == 0) return 0;
-  if (precision == -1 && !d2b_deform_conv_tc_supported(p)) return 0;
-  return d2b_deform_conv_tc_fwd_workspace(p, (flags & D2B_DCN_X_NHWC) ? 1 : 0);
+  precision = dcn_precision(p, precision, kFwd);
+  return precision ? d2b_deform_conv_tc_fwd_workspace(p, precision, (flags & D2B_DCN_X_NHWC) ? 1 : 0) : 0;
 }
 
 // Saved columns (training): the tensor-core forward can keep the sampled columns it builds -- bf16 hi [| lo] tiles in the
 // tensor core's operand layout -- and the backward's weight-gradient kernel then streams them back instead of sampling x a
 // second time.  0 when the shape / precision has no tensor-core path (pass cols = NULL then).
 D2B_API size_t d2b_deform_conv_cols_bytes(const d2b_dcn_params* p, int precision) {
-  if (precision == -1) precision = (d2b_deform_conv_tc_supported(p) && d2b_deform_conv_tc_bwd_supported(p)) ? 1 : 0;
-  if (precision == 0 || !d2b_deform_conv_tc_bwd_supported(p)) return 0;
-  return d2b_deform_conv_tc_cols_bytes(p, precision);
+  precision = dcn_precision(p, precision, kFwd | kBwd);
+  return precision ? d2b_deform_conv_tc_cols_bytes(p, precision) : 0;
 }
 
 D2B_API int d2b_deform_conv_forward(const float* x, const float* offset, const float* mask, const float* weight,
@@ -402,7 +406,7 @@ D2B_API int d2b_deform_conv_forward(const float* x, const float* offset, const f
   if (d.N == 0) return D2B_OK;
   if (!x || !offset || !weight || !out) return D2B_EINVAL;
   if (precision < -1 || precision > 2) return D2B_EINVAL;
-  if (precision == -1) precision = d2b_deform_conv_tc_supported(p) ? 1 : 0;
+  precision = dcn_precision(p, precision, kFwd);
   if (precision != 0)  // no silent precision / path change: an unsupported shape is reported, not rerouted
     return d2b_deform_conv_forward_tc(x, offset, mask, weight, nullptr, bias, 0, p, precision,
                                       (flags & D2B_DCN_X_NHWC) ? 1 : 0, out, cols, workspace, workspace_bytes, stream);
@@ -416,9 +420,9 @@ D2B_API int d2b_deform_conv_forward(const float* x, const float* offset, const f
 
 D2B_API size_t d2b_deform_conv_backward_workspace_bytes(const d2b_dcn_params* p, int precision, int flags, int need_data,
                                                         int need_weight) {
-  if (precision == 0) return 0;  // the FFMA path never materialises grad_columns
-  if (precision == -1 && !d2b_deform_conv_tc_bwd_supported(p)) return 0;
-  return d2b_deform_conv_tc_bwd_workspace(p, (flags & D2B_DCN_X_NHWC) ? 1 : 0, need_data, need_weight);
+  precision = dcn_precision(p, precision, kBwd);  // the FFMA path (0) never materialises grad_columns
+  return precision ? d2b_deform_conv_tc_bwd_workspace(p, precision, (flags & D2B_DCN_X_NHWC) ? 1 : 0, need_data, need_weight)
+                   : 0;
 }
 
 D2B_API int d2b_deform_conv_backward(const float* x, const float* offset, const float* mask, const float* weight,
@@ -430,7 +434,7 @@ D2B_API int d2b_deform_conv_backward(const float* x, const float* offset, const 
   Dims d;
   if (!make_dims(p, d)) return D2B_EINVAL;
   if (precision < -1 || precision > 2) return D2B_EINVAL;
-  if (precision == -1) precision = d2b_deform_conv_tc_bwd_supported(p) ? 1 : 0;
+  precision = dcn_precision(p, precision, kBwd);
   if (d.N > 0 && (!x || !offset || !weight || !grad_out)) return D2B_EINVAL;
   if (cols && precision == 0) return D2B_EINVAL;
   if (grad_bias) {
@@ -495,7 +499,7 @@ D2B_API int d2b_deform_conv_fused_forward(const float* x, const float* offset_ma
   if (!make_dims(p, d)) return D2B_EINVAL;
   if (d.N == 0) return D2B_OK;
   if (!x || !offset_mask || !weight || !out || precision == 0 || precision < -1 || precision > 2) return D2B_EINVAL;
-  if (precision == -1) precision = 1;
+  precision = dcn_precision(p, precision, kFused);
   return d2b_deform_conv_forward_tc(x, offset_mask, nullptr, weight, scale, shift, relu, p, precision,
                                     ((flags & D2B_DCN_X_NHWC) ? 1 : 0) | 2, out, cols, workspace, workspace_bytes, stream);
 }
@@ -509,7 +513,7 @@ D2B_API int d2b_deform_conv_fused_backward(const float* x, const float* offset_m
   Dims d;
   if (!make_dims(p, d)) return D2B_EINVAL;
   if (precision == 0 || precision < -1 || precision > 2) return D2B_EINVAL;
-  if (precision == -1) precision = 1;
+  precision = dcn_precision(p, precision, kFused);
   if (d.N > 0 && (!x || !offset_mask || !weight || !grad_out)) return D2B_EINVAL;
   return d2b_deform_conv_backward_tc(x, offset_mask, nullptr, weight, grad_out, scale, y, relu, p, precision,
                                      ((flags & D2B_DCN_X_NHWC) ? 1 : 0) | 2, cols, grad_x, grad_offset_mask, nullptr,

@@ -16,7 +16,8 @@
 // Layout decisions
 //   * x is gathered from channels-last storage [N,H,W,C] fp32: the 64 channels of a tap are 256 contiguous bytes, a
 //     half-warp reads them as 16 x LDG.128, a warp keeps 8 such loads in flight per lane.  NCHW inputs are re-laid out once
-//     per call by nchw_to_nhwc_kernel (roi_align.cu); channels_last inputs are used in place.
+//     per call by nchw_to_nhwc_kernel (roi_align.cu), and their gradient back by nhwc_to_nchw_kernel; channels_last inputs
+//     are used in place.
 //   * k' is ordered (kernel point, 64-channel block): one "unit" = 64 k' = one 128-byte swizzle row of bf16, so the
 //     bilinear taps of a (pixel, kernel point) are computed once (tap table in shared memory) and reused by all channels.
 //   * grouped convolutions with fewer than 64 channels per group are packed into "super-groups" of 64 input channels
@@ -30,6 +31,7 @@
 // kSideRegs registers so that the workers get kWorkerRegs (setmaxnreg).
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 #include "deform_conv_tc.cuh"
@@ -217,6 +219,74 @@ bool plan_k3(const TC& d, K3P& k) {
   k.S = 3;
   while (k.S > 1 && k.S * k.stage_bytes + 4096 + 1024 + 128 > kMaxSmem) --k.S;
   return k.S >= 2;
+}
+
+// ------------------------------------------------------------------------------------------------ call plans
+// One plan per direction holds what a host call decides before it launches: the kernels' plans and the byte offset of
+// each workspace region.  The size queries return a plan's total and the launchers carve from its offsets, so the two
+// cannot disagree.  A plan that does not build means the tensor-core kernels do not take the shape.
+struct Carve {  // regions laid out one after the other, each 256-byte aligned; an absent region has 0 bytes
+  size_t total = 0;
+  size_t add(size_t bytes) {
+    const size_t at = total;
+    total += align256(bytes);
+    return at;
+  }
+};
+
+struct FwdPlan {
+  TC d;
+  K1P k1, kc;   // kc: the column-fed launch, when colfed
+  bool colfed;  // saved columns over several output-channel tiles: K1 gathers tile 0, K1c computes the others from cols
+  int split;    // bf16x3 operands (precision 1)
+  size_t wt, x, total;  // workspace: weight tiles, NHWC copy of an NCHW x
+  size_t cols_bytes;    // the columns one call saves for the backward
+};
+
+bool plan_fwd(const d2b_dcn_params* p, int precision, int x_nhwc, bool cols, FwdPlan& P) {
+  if (!make_tc(p, P.d) || !plan_k1(P.d, P.k1)) return false;
+  const TC& d = P.d;
+  Carve ws;
+  P.wt = ws.add((size_t)d.SG * P.k1.noct * d.U * 2 * P.k1.BN * 128);
+  P.x = ws.add(x_nhwc ? 0 : sizeof(float) * (size_t)d.N * d.H * d.W * d.Cin);
+  P.total = ws.total;
+  P.cols_bytes = (size_t)d.N * d.tiles_img * d.SG * d.U * (size_t)(precision == 1 ? 2 : 1) * kTile;
+  P.split = precision == 1 ? 1 : 0;
+  // With saved columns, x is sampled once per layer rather than once per output-channel tile.
+  P.colfed = false;
+  K1P k1;
+  if (cols && P.k1.noct > 1 && plan_k1(d, k1, true) && plan_k1c(d, k1, P.kc)) {
+    P.k1 = k1;
+    P.colfed = true;
+  }
+  return true;
+}
+
+struct BwdPlan {
+  TC d;
+  K2P k2;
+  K3P k3;
+  int split;  // bf16x3 operands (precision 1)
+  // workspace: NHWC copies of an NCHW x and of its gradient, grad_out as pixel-row tiles (K2) and as channel-row tiles (K3),
+  // W^T tiles (K2), the weight gradient in the accumulator tiles' layout (gw_bytes)
+  size_t x, gx, gt_px, wt, gt_oc, gw, gw_bytes, total;
+};
+
+bool plan_bwd(const d2b_dcn_params* p, int precision, int x_nhwc, int need_data, int need_weight, BwdPlan& P) {
+  if (!make_tc(p, P.d) || !plan_k2(P.d, P.k2) || !plan_k3(P.d, P.k3)) return false;
+  const TC& d = P.d;
+  const size_t xbytes = sizeof(float) * (size_t)d.N * d.H * d.W * d.Cin;
+  P.gw_bytes = sizeof(float) * (size_t)d.SG * d.MC * 128 * d.ops;
+  Carve ws;
+  P.x = ws.add(x_nhwc ? 0 : xbytes);
+  P.gx = ws.add(need_data && !x_nhwc ? xbytes : 0);
+  P.gt_px = ws.add(need_data ? (size_t)d.N * d.tiles_img * d.SG * d.nks * 2 * kTile : 0);
+  P.wt = ws.add(need_data ? (size_t)d.SG * d.MC * d.nks * 2 * kTile : 0);
+  P.gt_oc = ws.add(need_weight ? (size_t)d.N * d.stages_img * d.SG * P.k3.noct * 2 * P.k3.BN * 128 : 0);
+  P.gw = ws.add(need_weight ? P.gw_bytes : 0);
+  P.total = ws.total;
+  P.split = precision == 1 ? 1 : 0;
+  return true;
 }
 
 // ------------------------------------------------------------------------------------------------ sampling taps
@@ -1256,25 +1326,6 @@ __global__ void dcn_gout_oc_tiles_kernel(const float* __restrict__ gout, const f
   *reinterpret_cast<uint4*>(base + BN * 128 + swz128((uint32_t)r, (uint32_t)c16)) = lo;
 }
 
-// [N,HW,C] -> [N,C,HW]  (grad_x back to the reference's layout)
-__global__ void __launch_bounds__(256) nhwc_to_nchw_kernel(const float* __restrict__ src, int C, int HW,
-                                                           float* __restrict__ dst) {
-  __shared__ float t[64][33];
-  const int hw0 = blockIdx.x * 64, c0 = blockIdx.y * 32;
-  const float* __restrict__ s = src + (size_t)blockIdx.z * HW * C;
-  float* __restrict__ o = dst + (size_t)blockIdx.z * C * HW;
-  const int tid = threadIdx.x;
-  for (int e = tid; e < 64 * 32; e += 256) {
-    const int pp = e >> 5, cc = e & 31;
-    t[pp][cc] = (hw0 + pp < HW && c0 + cc < C) ? __ldg(s + (size_t)(hw0 + pp) * C + c0 + cc) : 0.f;
-  }
-  __syncthreads();
-  for (int e = tid; e < 64 * 32; e += 256) {
-    const int cc = e >> 6, pp = e & 63;
-    if (hw0 + pp < HW && c0 + cc < C) o[(size_t)(c0 + cc) * HW + hw0 + pp] = t[pp][cc];
-  }
-}
-
 // y = relu(y * scale + shift) in place: the forward's epilogue when the reduction was split over kernel points
 __global__ void dcn_epilogue_kernel(float* __restrict__ y, long long total, int Cout, int HoWo, const Epi ep) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1287,49 +1338,63 @@ __global__ void dcn_epilogue_kernel(float* __restrict__ y, long long total, int 
   y[i] = v;
 }
 
-int to_nhwc(const float* x, const TC& d, float* dst, cudaStream_t stream) {
+// x and grad_x change layout through the library's pyramid layout change (roi_align.cu), as a one-level pyramid
+int change_layout(const float* src, const TC& d, float* dst, bool to_nhwc, cudaStream_t stream) {
   d2b_pyramid P = {};
   P.num_levels = 1;
-  P.feat[0] = x;
+  P.feat[0] = src;
   P.H[0] = d.H;
   P.W[0] = d.W;
   P.scale[0] = 1.f;
   float* dsts[1] = {dst};
-  return d2b_pyramid_nchw_to_nhwc(&P, d.N, d.Cin, dsts, (void*)stream);
+  return (to_nhwc ? d2b_pyramid_nchw_to_nhwc : d2b_pyramid_nhwc_to_nchw)(&P, d.N, d.Cin, dsts, (void*)stream);
+}
+
+// Launches one of the warp-specialised kernels, which need more than 48 KB of dynamic shared memory.  Every kernel is its
+// own instantiation, so each keeps its own opt-in record.
+template <auto kernel, class... Args>
+int launch_big_smem(dim3 grid, int smem_bytes, cudaStream_t stream, Args... args) {
+  D2B_ALLOW_BIG_SMEM(kernel);
+  kernel<<<grid, kThreads, smem_bytes, stream>>>(args...);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
+}
+
+// The GEMM kernels are instantiated per output-channel tile width: calls launch(std::integral_constant<int, W>()) for the
+// plan's width BN, W one of the widths the kernel is instantiated for (the last when BN is none of the others).
+template <int W, int... More, class Launch>
+int with_tile_width(int BN, Launch launch) {
+  if constexpr (sizeof...(More) > 0)
+    if (BN != W) return with_tile_width<More...>(BN, launch);
+  return launch(std::integral_constant<int, W>());
 }
 
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ host entry points
+// 1 when the plan of the direction builds: the tensor-core kernels take the shape
+D2B_API int d2b_deform_conv_tc_shape_supported(const d2b_dcn_params* p, int backward) {
+  FwdPlan f;
+  BwdPlan b;
+  return backward ? plan_bwd(p, 1, 1, 1, 1, b) : plan_fwd(p, 1, 1, false, f);
+}
+
 // (library-internal, declared in deform_conv_tc.cuh for deform_conv.cu)
-int d2b_deform_conv_tc_supported(const d2b_dcn_params* p) {
-  TC d;
-  K1P k1;
-  return make_tc(p, d) && plan_k1(d, k1);
+size_t d2b_deform_conv_tc_fwd_workspace(const d2b_dcn_params* p, int precision, int x_nhwc) {
+  FwdPlan P;
+  return plan_fwd(p, precision, x_nhwc, false, P) ? P.total : 0;
 }
 
-int d2b_deform_conv_tc_bwd_supported(const d2b_dcn_params* p) {
-  TC d;
-  K2P k2;
-  K3P k3;
-  return make_tc(p, d) && plan_k2(d, k2) && plan_k3(d, k3);
+size_t d2b_deform_conv_tc_bwd_workspace(const d2b_dcn_params* p, int precision, int x_nhwc, int need_data, int need_weight) {
+  BwdPlan P;
+  return plan_bwd(p, precision, x_nhwc, need_data, need_weight, P) ? P.total : 0;
 }
 
-size_t d2b_deform_conv_tc_fwd_workspace(const d2b_dcn_params* p, int x_nhwc) {
-  TC d;
-  K1P k;
-  if (!make_tc(p, d) || !plan_k1(d, k)) return 0;
-  size_t b = align256((size_t)d.SG * k.noct * d.U * 2 * k.BN * 128);
-  if (!x_nhwc) b += align256(sizeof(float) * (size_t)d.N * d.H * d.W * d.Cin);
-  return b;
-}
-
-// bytes of the column tiles one forward call saves for the backward (0: shape not taken by the tensor-core kernels)
+// the forward writes the columns and the backward reads them: 0 unless both plans build
 size_t d2b_deform_conv_tc_cols_bytes(const d2b_dcn_params* p, int precision) {
-  TC d;
-  K1P k;
-  if (precision == 0 || !make_tc(p, d) || !plan_k1(d, k)) return 0;
-  return (size_t)d.N * d.tiles_img * d.SG * d.U * (size_t)(precision == 1 ? 2 : 1) * kTile;
+  FwdPlan f;
+  BwdPlan b;
+  return plan_fwd(p, precision, 1, false, f) && plan_bwd(p, precision, 1, 0, 0, b) ? f.cols_bytes : 0;
 }
 
 // tcflags: bit 0 = x is NHWC, bit 1 = `offset` is the fused [N, 3*DG*KK, Ho, Wo] offset + mask-logit tensor (mask must be null)
@@ -1339,26 +1404,25 @@ int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float*
                                int tcflags, float* out, void* cols, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   const int x_nhwc = tcflags & 1;
-  TC d;
-  K1P k;
-  if (!make_tc(p, d) || !plan_k1(d, k)) return D2B_EUNSUPPORTED;  // argument validity was checked by the caller
+  FwdPlan P;  // argument validity was checked by the caller
+  if (!plan_fwd(p, precision, x_nhwc, cols != nullptr, P)) return D2B_EUNSUPPORTED;
+  TC& d = P.d;
+  const K1P& k = P.k1;
   if (d.N == 0) return D2B_OK;
   if (tcflags & 2) {
     if (mask) return D2B_EINVAL;
     mask = use_fused_offset_mask(d, offset);
   }
-  if (!workspace || workspace_bytes < d2b_deform_conv_tc_fwd_workspace(p, x_nhwc)) return D2B_EWORKSPACE;
+  if (!workspace || workspace_bytes < P.total) return D2B_EWORKSPACE;
   if ((reinterpret_cast<uintptr_t>(workspace) & 255) || (x_nhwc && (reinterpret_cast<uintptr_t>(x) & 15)) ||
       (reinterpret_cast<uintptr_t>(cols) & 15))
     return D2B_EINVAL;
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-  uint8_t* wt = ws;
-  ws += align256((size_t)d.SG * k.noct * d.U * 2 * k.BN * 128);
+  uint8_t* wt = ws + P.wt;
   const float* xh = x;
   if (!x_nhwc) {
-    float* xn = reinterpret_cast<float*>(ws);
-    int rc = to_nhwc(x, d, xn, stream);
-    if (rc) return rc;
+    float* xn = reinterpret_cast<float*>(ws + P.x);
+    if (int rc = change_layout(x, d, xn, true, stream)) return rc;
     xh = xn;
   }
   {
@@ -1366,49 +1430,25 @@ int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float*
     dcn_wtile_fwd_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(weight, d, k.BN, k.noct, wt);
     D2B_CHECK_LAUNCH();
   }
-  // With saved columns, the gathering K1 computes output-channel tile 0 only and K1c the others from its columns, so that x
-  // is sampled once per layer rather than once per output-channel tile.
-  K1P kc;
-  bool colfed = false;
-  if (cols && k.noct > 1) {
-    K1P k1;
-    if (plan_k1(d, k1, true) && plan_k1c(d, k1, kc)) {
-      k = k1;
-      colfed = true;
-    }
-  }
   if (k.red) D2B_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)d.N * d.Cout * d.HoWo, stream));
-  const int smem_bytes = k.S * k.stage_bytes + k.tap_bytes + 1024 + 128;
-  const int split = precision == 1 ? 1 : 0;
   const Epi ep = {scale, shift, relu};
-  dim3 grid(d.N * d.tiles_img, d.SG * k.goct, k.ksplit);
-#define D2B_LAUNCH_K1(BN)                                                                                              \
-  {                                                                                                                    \
-    D2B_ALLOW_BIG_SMEM(dcn_fwd_tc_kernel<BN>);                                                                         \
-    dcn_fwd_tc_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(xh, offset, mask, wt, ep, d, k, split, out,        \
-                                                                    reinterpret_cast<uint8_t*>(cols));                 \
-  }
-  if (k.BN == 16) D2B_LAUNCH_K1(16)
-  else if (k.BN == 32) D2B_LAUNCH_K1(32)
-  else if (k.BN == 64) D2B_LAUNCH_K1(64)
-  else D2B_LAUNCH_K1(128)
-#undef D2B_LAUNCH_K1
-  D2B_CHECK_LAUNCH();
-  if (colfed) {
+  const dim3 grid(d.N * d.tiles_img, d.SG * k.goct, k.ksplit);
+  const int smem_bytes = k.S * k.stage_bytes + k.tap_bytes + 1024 + 128;
+  int rc = with_tile_width<16, 32, 64, 128>(k.BN, [&](auto bn) {
+    return launch_big_smem<dcn_fwd_tc_kernel<decltype(bn)::value>>(grid, smem_bytes, stream, xh, offset, mask, wt, ep, d, k,
+                                                                    P.split, out, reinterpret_cast<uint8_t*>(cols));
+  });
+  if (rc) return rc;
+  if (P.colfed) {
+    const K1P& kc = P.kc;
+    const dim3 grid_c(d.N * d.tiles_img * kc.goct, d.SG, kc.ksplit);
     const int smem_c = kc.S * kc.stage_bytes + 1024 + 128;
-    dim3 grid_c(d.N * d.tiles_img * kc.goct, d.SG, kc.ksplit);
     const uint8_t* cl = reinterpret_cast<const uint8_t*>(cols);
-#define D2B_LAUNCH_K1C(BN)                                                                                             \
-  {                                                                                                                    \
-    D2B_ALLOW_BIG_SMEM(dcn_fwd_cols_kernel<BN>);                                                                       \
-    dcn_fwd_cols_kernel<BN><<<grid_c, kThreads, smem_c, stream>>>(cl, wt, ep, d, kc, split, out);                      \
-  }
-    if (kc.BN == 16) D2B_LAUNCH_K1C(16)
-    else if (kc.BN == 32) D2B_LAUNCH_K1C(32)
-    else if (kc.BN == 64) D2B_LAUNCH_K1C(64)
-    else D2B_LAUNCH_K1C(128)
-#undef D2B_LAUNCH_K1C
-    D2B_CHECK_LAUNCH();
+    rc = with_tile_width<16, 32, 64, 128>(kc.BN, [&](auto bn) {
+      return launch_big_smem<dcn_fwd_cols_kernel<decltype(bn)::value>>(grid_c, smem_c, stream, cl, wt, ep, d, kc, P.split,
+                                                                        out);
+    });
+    if (rc) return rc;
   }
   if (k.red && (scale || relu)) {
     const long long total = (long long)d.N * d.Cout * d.HoWo;
@@ -1416,26 +1456,6 @@ int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float*
     D2B_CHECK_LAUNCH();
   }
   return D2B_OK;
-}
-
-size_t d2b_deform_conv_tc_bwd_workspace(const d2b_dcn_params* p, int x_nhwc, int need_data, int need_weight) {
-  TC d;
-  K2P k2;
-  K3P k3;
-  if (!make_tc(p, d) || !plan_k2(d, k2) || !plan_k3(d, k3)) return 0;
-  size_t b = 0;
-  const size_t xbytes = align256(sizeof(float) * (size_t)d.N * d.H * d.W * d.Cin);
-  if (!x_nhwc) b += xbytes;                     // x in NHWC
-  if (need_data && !x_nhwc) b += xbytes;        // grad_x accumulated in NHWC
-  if (need_data) {
-    b += align256((size_t)d.N * d.tiles_img * d.SG * d.nks * 2 * kTile);  // gout, pixel-row tiles
-    b += align256((size_t)d.SG * d.MC * d.nks * 2 * kTile);               // W^T tiles
-  }
-  if (need_weight) {
-    b += align256((size_t)d.N * d.stages_img * d.SG * k3.noct * 2 * k3.BN * 128);  // gout, oc-row tiles
-    b += align256(sizeof(float) * (size_t)d.SG * d.MC * 128 * d.ops);  // weight gradient in the accumulator tiles' layout
-  }
-  return b;
 }
 
 // grad_x: NCHW (or NHWC when x_nhwc) fully written; grad_offset / grad_mask / grad_weight fully written.
@@ -1448,11 +1468,12 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
                                 size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   const int x_nhwc = tcflags & 1;
-  TC d;
-  K2P k2;
-  K3P k3;
-  if (!make_tc(p, d) || !plan_k2(d, k2) || !plan_k3(d, k3)) return D2B_EUNSUPPORTED;
   const int need_data = (grad_x || grad_offset || grad_mask) ? 1 : 0, need_weight = grad_weight ? 1 : 0;
+  BwdPlan P;
+  if (!plan_bwd(p, precision, x_nhwc, need_data, need_weight, P)) return D2B_EUNSUPPORTED;
+  TC& d = P.d;
+  const K2P& k2 = P.k2;
+  const K3P& k3 = P.k3;
   const bool fused_om = (tcflags & 2) != 0;
   if (fused_om && (mask || grad_mask)) return D2B_EINVAL;
   if (relu && !y_saved) return D2B_EINVAL;
@@ -1468,46 +1489,30 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
     size_t zb[3] = {noff * 4, nm * 4, nw * 4};
     return d2b_zero_buffers(zp, zb, 3, stream);
   }
-  if (!workspace || workspace_bytes < d2b_deform_conv_tc_bwd_workspace(p, x_nhwc, need_data, need_weight)) return D2B_EWORKSPACE;
+  if (!workspace || workspace_bytes < P.total) return D2B_EWORKSPACE;
   if ((reinterpret_cast<uintptr_t>(workspace) & 255) || (x_nhwc && (reinterpret_cast<uintptr_t>(x) & 15)) ||
       (x_nhwc && grad_x && (reinterpret_cast<uintptr_t>(grad_x) & 15)) || (reinterpret_cast<uintptr_t>(cols) & 15))
     return D2B_EINVAL;
-  const int split = precision == 1 ? 1 : 0;
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-  const size_t xbytes = align256(sizeof(float) * nx);
   const float* xh = x;
   if (!x_nhwc) {
-    float* xn = reinterpret_cast<float*>(ws);
-    ws += xbytes;
-    int rc = to_nhwc(x, d, xn, stream);
-    if (rc) return rc;
+    float* xn = reinterpret_cast<float*>(ws + P.x);
+    if (int rc = change_layout(x, d, xn, true, stream)) return rc;
     xh = xn;
   }
-  float* gxh = nullptr;
-  if (need_data && grad_x) gxh = x_nhwc ? grad_x : reinterpret_cast<float*>(ws);
-  uint8_t* gt_px = nullptr;
-  uint8_t* wt = nullptr;
-  if (need_data) {
-    if (!x_nhwc) ws += xbytes;
-    gt_px = ws;
-    ws += align256((size_t)d.N * d.tiles_img * d.SG * d.nks * 2 * kTile);
-    wt = ws;
-    ws += align256((size_t)d.SG * d.MC * d.nks * 2 * kTile);
-  }
-  uint8_t* gt_oc = need_weight ? ws : nullptr;
-  float* gw_part = nullptr;
-  if (need_weight) {
-    ws += align256((size_t)d.N * d.stages_img * d.SG * k3.noct * 2 * k3.BN * 128);
-    gw_part = reinterpret_cast<float*>(ws);
-  }
+  float* gxh = grad_x ? (x_nhwc ? grad_x : reinterpret_cast<float*>(ws + P.gx)) : nullptr;
+  uint8_t* gt_oc = need_weight ? ws + P.gt_oc : nullptr;
+  float* gw_part = need_weight ? reinterpret_cast<float*>(ws + P.gw) : nullptr;
   {  // every accumulated output of the call zero-filled by one launch (grad_mask of the fused layout lives inside grad_offset;
     // grad_weight is accumulated in the staging matrix and then written element by element)
     void* zp[4] = {grad_offset, fused_om ? nullptr : grad_mask, gxh, gw_part};
-    size_t zb[4] = {noff * 4, nm * 4, nx * 4, sizeof(float) * (size_t)d.SG * d.MC * 128 * d.ops};
+    size_t zb[4] = {noff * 4, nm * 4, nx * 4, P.gw_bytes};
     int rc = d2b_zero_buffers(zp, zb, 4, stream);
     if (rc) return rc;
   }
   if (need_data) {
+    uint8_t* gt_px = ws + P.gt_px;
+    uint8_t* wt = ws + P.wt;
     // grad_out is read once: pixel-row tiles for K2 and (when the weight gradient is wanted too) channel-row tiles for K3
     dcn_gout_px_tiles_kernel<<<dim3((unsigned)((size_t)d.N * d.tiles_img * d.SG * d.nks), 4), 256, 0, stream>>>(
         grad_out, y_saved, ep, d, gt_px, gt_oc, k3.BN, k3.noct);
@@ -1518,15 +1523,12 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
       D2B_CHECK_LAUNCH();
     }
     const int smem_bytes = 2 * 4 * kTile + 128 * kGcolPitch * 4 + k2.tap_bytes + 1024 + 128;
-    D2B_ALLOW_BIG_SMEM(dcn_bwd_data_tc_kernel);
-    dim3 grid(d.N * d.tiles_img, d.SG, k2.msplit);
-    dcn_bwd_data_tc_kernel<<<grid, kThreads, smem_bytes, stream>>>(xh, offset, mask, gt_px, wt, d, k2, split, gxh, grad_offset,
-                                                                  mask ? grad_mask : nullptr);
-    D2B_CHECK_LAUNCH();
+    if (int rc = launch_big_smem<dcn_bwd_data_tc_kernel>(dim3(d.N * d.tiles_img, d.SG, k2.msplit), smem_bytes, stream, xh,
+                                                         offset, mask, gt_px, wt, d, k2, P.split, gxh, grad_offset,
+                                                         mask ? grad_mask : nullptr))
+      return rc;
     if (grad_x && !x_nhwc) {
-      dim3 g2(d2b_cdiv(d.H * d.W, 64), d2b_cdiv(d.Cin, 32), d.N);
-      nhwc_to_nchw_kernel<<<g2, 256, 0, stream>>>(gxh, d.Cin, d.H * d.W, grad_x);
-      D2B_CHECK_LAUNCH();
+      if (int rc = change_layout(gxh, d, grad_x, false, stream)) return rc;
     }
   }
   if (need_weight) {
@@ -1537,40 +1539,32 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
     }
     // output-channel tile fastest, then the unit pair: the CTAs that read one column (or gathered) tile and those that read one
     // grad_out tile run in the same wave and share them in L2
-    dim3 grid(d.SG * k3.noct, d.MC, k3.nsplit);
+    const dim3 grid(d.SG * k3.noct, d.MC, k3.nsplit);
+    int rc;
     if (cols) {  // the forward kept its sampled columns: stream them back (no second pass over x)
       const int S = std::min(6, (kMaxSmem - 2048) / k3.stage_bytes);
       const int smem_bytes = S * k3.stage_bytes + 1024 + 128;
       const uint8_t* cl = reinterpret_cast<const uint8_t*>(cols);
-#define D2B_LAUNCH_K3C(BN)                                                                                             \
-  {                                                                                                                      \
-    D2B_ALLOW_BIG_SMEM(dcn_bwd_weight_cols_kernel<BN>);                                                                \
-    dcn_bwd_weight_cols_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(cl, gt_oc, d, k3, S, split, gw_part);       \
-  }
-      if (k3.BN == 64) D2B_LAUNCH_K3C(64)
-      else D2B_LAUNCH_K3C(128)
-#undef D2B_LAUNCH_K3C
+      rc = with_tile_width<64, 128>(k3.BN, [&](auto bn) {
+        return launch_big_smem<dcn_bwd_weight_cols_kernel<decltype(bn)::value>>(grid, smem_bytes, stream, cl, gt_oc, d, k3, S,
+                                                                                 P.split, gw_part);
+      });
     } else {
       const int smem_bytes = k3.S * k3.stage_bytes + 4096 + 1024 + 128;
-#define D2B_LAUNCH_K3(BN)                                                                                              \
-  {                                                                                                                      \
-    D2B_ALLOW_BIG_SMEM(dcn_bwd_weight_tc_kernel<BN>);                                                                  \
-    dcn_bwd_weight_tc_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(xh, offset, mask, gt_oc, d, k3, split, gw_part); \
-  }
-      if (k3.BN == 64) D2B_LAUNCH_K3(64)
-      else D2B_LAUNCH_K3(128)
-#undef D2B_LAUNCH_K3
+      rc = with_tile_width<64, 128>(k3.BN, [&](auto bn) {
+        return launch_big_smem<dcn_bwd_weight_tc_kernel<decltype(bn)::value>>(grid, smem_bytes, stream, xh, offset, mask, gt_oc,
+                                                                               d, k3, P.split, gw_part);
+      });
+    }
+    if (rc) return rc;
+    if (d.KK <= 9) {  // d.ops is a multiple of 16 (shape gate)
+      dcn_gw_reduce_tile_kernel<<<dim3(d.SG * (d.cps / kRedCh), d.ops / kRedOc), 256, 0, stream>>>(gw_part, d, grad_weight);
+    } else {
+      const long long total = (long long)d.SG * d.U * 64 * d.ops;
+      dcn_gw_reduce_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(gw_part, d, grad_weight);
     }
     D2B_CHECK_LAUNCH();
-    {
-      if (d.KK <= 9) {  // d.ops is a multiple of 16 (shape gate)
-        dcn_gw_reduce_tile_kernel<<<dim3(d.SG * (d.cps / kRedCh), d.ops / kRedOc), 256, 0, stream>>>(gw_part, d, grad_weight);
-      } else {
-        const long long total = (long long)d.SG * d.U * 64 * d.ops;
-        dcn_gw_reduce_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(gw_part, d, grad_weight);
-      }
-      D2B_CHECK_LAUNCH();
-    }
   }
   return D2B_OK;
 }
+

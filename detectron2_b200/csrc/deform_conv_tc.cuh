@@ -1,17 +1,14 @@
 // Host entry points of the tensor-core deformable convolution (deform_conv_tc.cu) that the public entry points in
-// deform_conv.cu dispatch to.  Library-internal: not exported from libd2b200.so.
+// deform_conv.cu dispatch to.  Library-internal: not exported from libd2b200.so.  Whether the kernels take a shape is the
+// public d2b_deform_conv_tc_shape_supported; the sizes below are 0 when they do not.
 #pragma once
 #include <stddef.h>
 
 #include "../../include/d2b200.h"
 
-// shape gates: the forward kernel / both backward kernels take the shape
-int d2b_deform_conv_tc_supported(const d2b_dcn_params* p);
-int d2b_deform_conv_tc_bwd_supported(const d2b_dcn_params* p);
-
-size_t d2b_deform_conv_tc_fwd_workspace(const d2b_dcn_params* p, int x_nhwc);
+size_t d2b_deform_conv_tc_fwd_workspace(const d2b_dcn_params* p, int precision, int x_nhwc);
+size_t d2b_deform_conv_tc_bwd_workspace(const d2b_dcn_params* p, int precision, int x_nhwc, int need_data, int need_weight);
 size_t d2b_deform_conv_tc_cols_bytes(const d2b_dcn_params* p, int precision);
-size_t d2b_deform_conv_tc_bwd_workspace(const d2b_dcn_params* p, int x_nhwc, int need_data, int need_weight);
 
 int d2b_deform_conv_forward_tc(const float* x, const float* offset, const float* mask, const float* weight,
                                const float* scale, const float* shift, int relu, const d2b_dcn_params* p, int precision,
