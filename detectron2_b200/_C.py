@@ -24,9 +24,9 @@ class DcnParams(C.Structure):
 
 MAX_LEVELS = 8
 MAX_IMAGES = 64  # D2B_MAX_IMAGES
-ABI_VERSION = 4  # include/d2b200.h D2B_ABI_VERSION
+ABI_VERSION = 5  # include/d2b200.h D2B_ABI_VERSION
 DCN_X_NHWC = 1   # D2B_DCN_X_NHWC
-ROI_ROTATED, ROI_BACKWARD = 1, 2  # D2B_ROI_ROTATED / D2B_ROI_BACKWARD
+ROI_ROTATED, ROI_BACKWARD, ROI_NHWC = 1, 2, 4  # D2B_ROI_ROTATED / D2B_ROI_BACKWARD / D2B_ROI_NHWC
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}  # D2B_F32 / D2B_F16 / D2B_BF16
 MATCH_ROTATED, MATCH_LOW_QUALITY, MATCH_APPEND_GT = 1, 2, 4  # D2B_MATCH_*
 MATCH_MAX_THRESHOLDS = 8  # D2B_MATCH_MAX_THRESHOLDS
@@ -69,28 +69,10 @@ def _declare(lib):
         "d2b_abi_version": (i, []),
         "d2b_cuda_version": (i, []),
         "d2b_arch": (C.c_char_p, []),
-        "d2b_roi_align_forward": (i, [f32p, i, i, i, i, f32p, i, f, i, i, i, i, f32p, vp]),
-        "d2b_roi_align_backward": (i, [f32p, f32p, i, f, i, i, i, i, i, i, i, i, f32p, vp]),
-        "d2b_roi_pooler_forward": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, i, f32p, vp]),
-        "d2b_roi_pooler_backward": (i, [C.POINTER(Pyramid), i, i, f32p, f32p, i, i, i, i, i, vp]),
-        "d2b_roi_align_forward_nhwc": (i, [f32p, i, i, i, i, f32p, i, f, i, i, i, i, f32p, vp]),
-        "d2b_roi_pooler_forward_nhwc": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, i, f32p, vp]),
-        "d2b_pyramid_nchw_to_nhwc": (i, [C.POINTER(Pyramid), i, i, C.POINTER(C.c_void_p), vp]),
-        "d2b_pyramid_nhwc_to_nchw": (i, [C.POINTER(Pyramid), i, i, C.POINTER(C.c_void_p), vp]),
-        "d2b_pyramid_nchw_to_nhwc_t": (i, [C.POINTER(Pyramid), i, i, C.POINTER(C.c_void_p), i, vp]),
-        "d2b_pyramid_nhwc_to_nchw_t": (i, [C.POINTER(Pyramid), i, i, C.POINTER(C.c_void_p), i, vp]),
-        "d2b_roi_pooler_forward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, i, vp, i, vp]),
-        "d2b_roi_pooler_backward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, vp, i, f32p, i, i, i, i, i, vp]),
-        "d2b_roi_align_backward_nhwc": (i, [f32p, f32p, i, f, i, i, i, i, i, i, i, i, f32p, vp]),
-        "d2b_roi_pooler_backward_nhwc": (i, [C.POINTER(Pyramid), i, i, f32p, f32p, i, i, i, i, i, vp]),
-        "d2b_roi_align_rotated_forward": (i, [f32p, i, i, i, i, f32p, i, f, i, i, i, f32p, vp]),
-        "d2b_roi_align_rotated_backward": (i, [f32p, f32p, i, f, i, i, i, i, i, i, i, f32p, vp]),
-        "d2b_roi_align_rotated_forward_nhwc": (i, [f32p, i, i, i, i, f32p, i, f, i, i, i, f32p, vp]),
-        "d2b_roi_align_rotated_backward_nhwc": (i, [f32p, f32p, i, f, i, i, i, i, i, i, i, f32p, vp]),
-        "d2b_roi_pooler_rotated_forward": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, f32p, vp]),
-        "d2b_roi_pooler_rotated_backward": (i, [C.POINTER(Pyramid), i, i, f32p, f32p, i, i, i, i, vp]),
-        "d2b_roi_pooler_rotated_forward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, vp, i, vp]),
-        "d2b_roi_pooler_rotated_backward_nhwc_t": (i, [C.POINTER(Pyramid), i, i, vp, i, f32p, i, i, i, i, vp]),
+        "d2b_roi_pooler_forward": (i, [C.POINTER(Pyramid), i, i, f32p, i, i, i, i, i, i, vp, i, vp]),
+        "d2b_roi_pooler_backward": (i, [C.POINTER(Pyramid), i, i, vp, i, f32p, i, i, i, i, i, i, vp]),
+        "d2b_pyramid_nchw_to_nhwc": (i, [C.POINTER(Pyramid), i, i, C.POINTER(C.c_void_p), i, vp]),
+        "d2b_pyramid_nhwc_to_nchw": (i, [C.POINTER(Pyramid), i, i, C.POINTER(C.c_void_p), i, vp]),
         "d2b_roi_pooler_nhwc_supported": (i, [C.POINTER(Pyramid), i, i, i, i]),
         "d2b_nms_workspace_bytes": (sz, [i64, i, i64]),
         "d2b_nms": (i, [f32p, f32p, i64p, i64, d, i, i64, i64p, i64p, vp, sz, vp]),

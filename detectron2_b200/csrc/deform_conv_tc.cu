@@ -1347,7 +1347,8 @@ int change_layout(const float* src, const TC& d, float* dst, bool to_nhwc, cudaS
   P.W[0] = d.W;
   P.scale[0] = 1.f;
   float* dsts[1] = {dst};
-  return (to_nhwc ? d2b_pyramid_nchw_to_nhwc : d2b_pyramid_nhwc_to_nchw)(&P, d.N, d.Cin, dsts, (void*)stream);
+  return to_nhwc ? d2b_pyramid_nchw_to_nhwc(&P, d.N, d.Cin, dsts, D2B_F32, (void*)stream)
+                 : d2b_pyramid_nhwc_to_nchw(&P, d.N, d.Cin, reinterpret_cast<void* const*>(dsts), D2B_F32, (void*)stream);
 }
 
 // Launches one of the warp-specialised kernels, which need more than 48 KB of dynamic shared memory.  Every kernel is its

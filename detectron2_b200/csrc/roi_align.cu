@@ -1091,13 +1091,8 @@ __global__ void __launch_bounds__(kNhwcThreads, 4) roi_align_nhwc_kernel(const P
   }
 }
 
-static int nhwc_supported(int num_levels, const int* H, const int* W, int C, int PH, int PW, int flags);
-
 static int launch_fwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C, int PH, int PW, int sr, int aligned,
                            void* out, cudaStream_t stream, int out_dt = D2B_F32) {
-  if (int rc = nhwc_supported(P.num_levels, P.H, P.W, C, PH, PW, 0)) return rc;
-  for (int l = 0; l < P.num_levels; ++l)
-    if ((reinterpret_cast<uintptr_t>(P.feat[l]) & 15) != 0) return D2B_EINVAL;
   (void)N;
   const int bins = PH * PW;
   const int slabs = d2b_cdiv(C, kNhwcCh);
@@ -1111,7 +1106,6 @@ static int launch_fwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C,
   const int chunk_pad = chunk | 1;
   const size_t smem = sizeof(float) * 128 * (size_t)chunk_pad;
   dim3 grid(K, slabs, nchunks);  // nchunks <= 65535: chunks hold >= 7 bins (nhwc_supported)
-  // (the per-bin loop alone and a 3-CTA / wider-batch variant were measured against this: profiles/r2_pooler_fwd_ab.md)
   D2B_DISPATCH_DTYPE(out_dt, (roi_align_nhwc_kernel<DT><<<grid, kNhwcThreads, smem, stream>>>(P, rois, C, PH, PW, sr, aligned, chunk,
                                                                                             chunk_pad, out)));
   D2B_CHECK_LAUNCH();
@@ -1125,7 +1119,7 @@ static int launch_fwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C,
 // (lane = 4 channels): it sums the <= few contributing bins from the RoI's gradient tile in shared memory and issues ONE
 // red.global.add.v4.f32 per pixel -- against 4*g*g scalar atomics per output element in the reference
 // (ROIAlignRotated_cuda.cu:311-318 / torchvision roi_align_backward) and one scalar red per pixel and channel in the NCHW
-// kernel above.  Measured ceiling of red.v4 on 256-byte runs: 5.9 TB/s (profiles/r2_microbench.txt).
+// kernel above.
 constexpr int kBwdBand = 64;     // footprint rows per pass
 constexpr int kBwdMaxFw = 96;    // footprint columns with a table (FPN-assigned RoIs span < 60); wider RoIs take the per-sample path
 constexpr int kBwdThreads = 256;
@@ -1378,9 +1372,6 @@ static size_t bwd_nhwc_smem(int rows, int PW) {
 
 static int launch_bwd_nhwc(const Pyr& P, int N, const float* rois, int K, int C, int PH, int PW, int sr, int aligned,
                            const void* gout, cudaStream_t stream, int g_dt = D2B_F32) {
-  if (int rc = nhwc_supported(P.num_levels, P.H, P.W, C, PH, PW, D2B_ROI_BACKWARD)) return rc;
-  for (int l = 0; l < P.num_levels; ++l)
-    if ((reinterpret_cast<uintptr_t>(P.grad[l]) & 15) != 0) return D2B_EINVAL;
   (void)N;
   // bin rows per CTA: all of them, unless that leaves fewer than ~2 CTAs per SM resident (shared memory) AND in the grid
   const int slabs = d2b_cdiv(C, kNhwcCh);
@@ -1504,14 +1495,14 @@ __global__ void __launch_bounds__(kBwdThreads) roi_align_rot_nhwc_kernel(const P
 }
 
 // dt: element type of `out` (forward) / `gout` (backward).  Every level's feature map (forward) or gradient map (backward)
-// must be 16-byte aligned -- checked by the callers.
+// must be 16-byte aligned -- checked by pooler_args.
 template <bool BWD>
 static size_t rot_nhwc_smem(int PH, int PW) {
   return sizeof(float) * 128 * (size_t)(BWD ? PH * PW : ((PH * PW) | 1));
 }
 
-// The shape limits of every channels-last kernel (D2B_OK or D2B_EUNSUPPORTED), stated once: the channels-last launchers and
-// d2b_roi_pooler_nhwc_supported all ask this.  Host-only, no CUDA call.
+// The shape limits of every channels-last kernel (D2B_OK or D2B_EUNSUPPORTED), stated once: pooler_args and
+// d2b_roi_pooler_nhwc_supported both ask this.  Host-only, no CUDA call.
 static int nhwc_supported(int num_levels, const int* H, const int* W, int C, int PH, int PW, int flags) {
   if (C % 4 != 0) return D2B_EUNSUPPORTED;  // lane = 4 channels
   for (int l = 0; l < num_levels; ++l)
@@ -1535,7 +1526,6 @@ static int nhwc_supported(int num_levels, const int* H, const int* W, int C, int
 template <bool BWD>
 static int launch_rot_nhwc(const Pyr& P, const float* rois, int K, int C, int PH, int PW, int sr, const void* gout, void* out,
                            cudaStream_t stream, int dt = D2B_F32) {
-  if (int rc = nhwc_supported(P.num_levels, P.H, P.W, C, PH, PW, D2B_ROI_ROTATED | (BWD ? D2B_ROI_BACKWARD : 0))) return rc;
   const size_t smem = rot_nhwc_smem<BWD>(PH, PW);
   dim3 grid(K, d2b_cdiv(C, kNhwcCh));
   D2B_DISPATCH_DTYPE(dt, {
@@ -1653,18 +1643,6 @@ static bool make_pyr(const d2b_pyramid* pyr, Pyr& P) {
   return true;
 }
 
-// A single-level entry point is a one-level pyramid (pick_level returns 0 for it): same kernels, same launches.
-static d2b_pyramid one_level(const float* feat, float* grad, int H, int W, float scale) {
-  d2b_pyramid p = {};
-  p.num_levels = 1;
-  p.feat[0] = feat;
-  p.grad[0] = grad;
-  p.H[0] = H;
-  p.W[0] = W;
-  p.scale[0] = scale;
-  return p;
-}
-
 // Every backward zero-fills the gradient maps of all levels with one launch before it accumulates into them.
 static int zero_grads(const Pyr& P, int N, int C, cudaStream_t stream) {
   void* zp[D2B_MAX_LEVELS];
@@ -1676,106 +1654,87 @@ static int zero_grads(const Pyr& P, int N, int C, cudaStream_t stream) {
   return d2b_zero_buffers(zp, zb, P.num_levels, stream);
 }
 
+// The argument rule of d2b_roi_pooler_forward / _backward, stated once (include/d2b200.h): every D2B_EINVAL condition comes
+// before any D2B_EUNSUPPORTED one, and the entry points launch nothing until it has passed.  `data` is the forward's out or
+// the backward's grad_out, `dtype` its element type.  On D2B_OK, P holds the pyramid and `idle` says that the call has
+// nothing to write.
+static int pooler_args(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int PH, int PW, int flags,
+                       const void* data, int dtype, bool bwd, Pyr& P, bool& idle) {
+  idle = true;
+  if (!bwd && (K == 0 || C == 0)) return D2B_OK;  // nothing to compute: before any other check
+  const bool nhwc = flags & D2B_ROI_NHWC;
+  if ((flags & ~(D2B_ROI_ROTATED | D2B_ROI_NHWC)) || !make_pyr(pyr, P) || ((flags & D2B_ROI_ROTATED) && P.level_rois))
+    return D2B_EINVAL;
+  if (N < 0 || C < 0 || K < 0 || (N == 0 && K > 0)) return D2B_EINVAL;  // N == 0, K > 0: RoIs of images that do not exist
+  if (!dtype_ok(dtype) || (!nhwc && dtype != D2B_F32)) return D2B_EINVAL;  // the NCHW kernels read and write fp32 only
+  if (N == 0 || C == 0) return D2B_OK;                                     // a backward with no gradient element to write
+  for (int l = 0; l < P.num_levels; ++l) {
+    const void* map = bwd ? static_cast<const void*>(P.grad[l]) : P.feat[l];
+    if (!map || (nhwc && (reinterpret_cast<uintptr_t>(map) & 15) != 0)) return D2B_EINVAL;
+  }
+  if (K > 0 && (!rois || !data || PH < 1 || PW < 1)) return D2B_EINVAL;
+  idle = false;
+  return nhwc && K > 0 ? nhwc_supported(P.num_levels, P.H, P.W, C, PH, PW, flags | (bwd ? D2B_ROI_BACKWARD : 0)) : D2B_OK;
+}
+
 D2B_API int d2b_roi_pooler_nhwc_supported(const d2b_pyramid* pyr, int C, int pooled_h, int pooled_w, int flags) {
   if (!pyr || pyr->num_levels < 1 || pyr->num_levels > D2B_MAX_LEVELS || C < 0 || pooled_h <= 0 || pooled_w <= 0)
     return D2B_EINVAL;
   return nhwc_supported(pyr->num_levels, pyr->H, pyr->W, C, pooled_h, pooled_w, flags);
 }
 
-D2B_API int d2b_roi_align_forward(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                  float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio, int aligned,
-                                  float* out, void* stream) {
-  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
-  return d2b_roi_pooler_forward(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, out, stream);
-}
-
-D2B_API int d2b_roi_align_forward_nhwc(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                       float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
-                                       int aligned, float* out, void* stream) {
-  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
-  return d2b_roi_pooler_forward_nhwc(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, out, stream);
-}
-
-D2B_API int d2b_roi_align_backward(const float* grad_out, const float* rois, int K, float spatial_scale, int pooled_h,
-                                   int pooled_w, int N, int C, int H, int W, int sampling_ratio, int aligned,
-                                   float* grad_in, void* stream) {
-  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
-  if ((size_t)N * C * H * W == 0) return D2B_OK;  // no gradient element to write
-  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
-  return d2b_roi_pooler_backward(&p, N, C, grad_out, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, stream);
-}
-
-D2B_API int d2b_roi_align_backward_nhwc(const float* grad_out, const float* rois, int K, float spatial_scale,
-                                        int pooled_h, int pooled_w, int N, int C, int H, int W, int sampling_ratio,
-                                        int aligned, float* grad_in, void* stream) {
-  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
-  if ((size_t)N * C * H * W == 0) return D2B_OK;
-  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
-  return d2b_roi_pooler_backward_nhwc(&p, N, C, grad_out, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, stream);
-}
-
-D2B_API int d2b_roi_align_rotated_forward(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                          float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
-                                          float* out, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;  // before the pooler's argument checks
-  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
-  return d2b_roi_pooler_rotated_forward(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, out, stream);
-}
-
-D2B_API int d2b_roi_align_rotated_forward_nhwc(const float* input, int N, int C, int H, int W, const float* rois, int K,
-                                               float spatial_scale, int pooled_h, int pooled_w, int sampling_ratio,
-                                               float* out, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;
-  const d2b_pyramid p = one_level(input, nullptr, H, W, spatial_scale);
-  return d2b_roi_pooler_rotated_forward_nhwc_t(&p, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, out, D2B_F32, stream);
-}
-
-D2B_API int d2b_roi_align_rotated_backward(const float* grad_out, const float* rois, int K, float spatial_scale,
-                                           int pooled_h, int pooled_w, int N, int C, int H, int W, int sampling_ratio,
-                                           float* grad_in, void* stream) {
-  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0) return D2B_EINVAL;
-  if ((size_t)N * C * H * W == 0) return D2B_OK;
-  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
-  return d2b_roi_pooler_rotated_backward(&p, N, C, grad_out, rois, K, pooled_h, pooled_w, sampling_ratio, stream);
-}
-
-D2B_API int d2b_roi_align_rotated_backward_nhwc(const float* grad_out, const float* rois, int K, float spatial_scale,
-                                                int pooled_h, int pooled_w, int N, int C, int H, int W,
-                                                int sampling_ratio, float* grad_in, void* stream) {
-  if (!grad_in || N < 0 || C < 0 || H < 0 || W < 0 || (reinterpret_cast<uintptr_t>(grad_in) & 15) != 0) return D2B_EINVAL;
-  if ((size_t)N * C * H * W == 0) return D2B_OK;
-  const d2b_pyramid p = one_level(nullptr, grad_in, H, W, spatial_scale);
-  return d2b_roi_pooler_rotated_backward_nhwc_t(&p, N, C, grad_out, D2B_F32, rois, K, pooled_h, pooled_w, sampling_ratio,
-                                                stream);
-}
-
 D2B_API int d2b_roi_pooler_forward(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
-                                   int pooled_w, int sampling_ratio, int aligned, float* out, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;
+                                   int pooled_w, int sampling_ratio, int aligned, int flags, void* out, int out_dtype,
+                                   void* stream) {
   Pyr P;
-  if (!make_pyr(pyr, P) || !rois || !out || N <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0) return D2B_EINVAL;
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.feat[l]) return D2B_EINVAL;
-  return launch_fwd(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, out, (cudaStream_t)stream);
+  bool idle;
+  if (int rc = pooler_args(pyr, N, C, rois, K, pooled_h, pooled_w, flags, out, out_dtype, false, P, idle)) return rc;
+  if (idle) return D2B_OK;
+  const cudaStream_t s = (cudaStream_t)stream;
+  switch (flags) {
+    case 0:
+      return launch_fwd(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, static_cast<float*>(out), s);
+    case D2B_ROI_NHWC:
+      return launch_fwd_nhwc(P, N, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, out, s, out_dtype);
+    case D2B_ROI_ROTATED | D2B_ROI_NHWC:
+      return launch_rot_nhwc<false>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, nullptr, out, s, out_dtype);
+  }
+  const int cpc = pick_c_per_cta(K, C);  // D2B_ROI_ROTATED
+  dim3 grid(K, d2b_cdiv(C, cpc));
+  roi_align_rot_fwd_kernel<1024><<<grid, kThreads, 0, s>>>(P, rois, C, pooled_h, pooled_w, sampling_ratio, cpc,
+                                                           static_cast<float*>(out));
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
 }
 
-D2B_API int d2b_roi_pooler_forward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
-                                          int pooled_w, int sampling_ratio, int aligned, void* out, int out_dtype, void* stream) {
-  if (K == 0 || C == 0) return D2B_OK;
+D2B_API int d2b_roi_pooler_backward(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
+                                    const float* rois, int K, int pooled_h, int pooled_w, int sampling_ratio, int aligned,
+                                    int flags, void* stream) {
   Pyr P;
-  if (!make_pyr(pyr, P) || !rois || !out || N <= 0 || pooled_h <= 0 || pooled_w <= 0 || K < 0 || !dtype_ok(out_dtype))
-    return D2B_EINVAL;
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.feat[l]) return D2B_EINVAL;
-  return launch_fwd_nhwc(P, N, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, out, (cudaStream_t)stream, out_dtype);
+  bool idle;
+  if (int rc = pooler_args(pyr, N, C, rois, K, pooled_h, pooled_w, flags, grad_out, grad_dtype, true, P, idle)) return rc;
+  if (idle) return D2B_OK;
+  const cudaStream_t s = (cudaStream_t)stream;
+  const int rc = zero_grads(P, N, C, s);
+  if (rc || K == 0) return rc;
+  switch (flags) {
+    case 0:
+      return launch_fwd(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, nullptr, s,
+                        static_cast<const float*>(grad_out));
+    case D2B_ROI_NHWC:
+      return launch_bwd_nhwc(P, N, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, grad_out, s, grad_dtype);
+    case D2B_ROI_ROTATED | D2B_ROI_NHWC:
+      return launch_rot_nhwc<true>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, grad_out, nullptr, s, grad_dtype);
+  }
+  const int cpc = pick_c_per_cta(K, C);  // D2B_ROI_ROTATED
+  dim3 grid(K, d2b_cdiv(C, cpc));
+  roi_align_rot_bwd_kernel<<<grid, kThreads, 0, s>>>(P, static_cast<const float*>(grad_out), rois, C, pooled_h, pooled_w,
+                                                     sampling_ratio, cpc);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
 }
 
-D2B_API int d2b_roi_pooler_forward_nhwc(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
-                                        int pooled_w, int sampling_ratio, int aligned, float* out, void* stream) {
-  return d2b_roi_pooler_forward_nhwc_t(pyr, N, C, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, out, D2B_F32, stream);
-}
-
-D2B_API int d2b_pyramid_nchw_to_nhwc_t(const d2b_pyramid* pyr, int N, int C, float* const* dst, int src_dtype, void* stream) {
+D2B_API int d2b_pyramid_nchw_to_nhwc(const d2b_pyramid* pyr, int N, int C, float* const* dst, int src_dtype, void* stream) {
   if (!pyr || !dst || pyr->num_levels < 1 || pyr->num_levels > D2B_MAX_LEVELS || N < 0 || C < 0 || !dtype_ok(src_dtype))
     return D2B_EINVAL;
   if (N == 0 || C == 0) return D2B_OK;
@@ -1800,11 +1759,7 @@ D2B_API int d2b_pyramid_nchw_to_nhwc_t(const d2b_pyramid* pyr, int N, int C, flo
   return D2B_OK;
 }
 
-D2B_API int d2b_pyramid_nchw_to_nhwc(const d2b_pyramid* pyr, int N, int C, float* const* dst, void* stream) {
-  return d2b_pyramid_nchw_to_nhwc_t(pyr, N, C, dst, D2B_F32, stream);
-}
-
-D2B_API int d2b_pyramid_nhwc_to_nchw_t(const d2b_pyramid* pyr, int N, int C, void* const* dst, int dst_dtype, void* stream) {
+D2B_API int d2b_pyramid_nhwc_to_nchw(const d2b_pyramid* pyr, int N, int C, void* const* dst, int dst_dtype, void* stream) {
   if (!pyr || !dst || pyr->num_levels < 1 || pyr->num_levels > D2B_MAX_LEVELS || N < 0 || C < 0 || !dtype_ok(dst_dtype))
     return D2B_EINVAL;
   if (N == 0 || C == 0) return D2B_OK;
@@ -1827,113 +1782,4 @@ D2B_API int d2b_pyramid_nhwc_to_nchw_t(const d2b_pyramid* pyr, int N, int C, voi
   D2B_DISPATCH_DTYPE(dst_dtype, (nhwc_to_nchw_kernel<DT><<<grid, 256, 0, (cudaStream_t)stream>>>(L, C)));
   D2B_CHECK_LAUNCH();
   return D2B_OK;
-}
-
-D2B_API int d2b_pyramid_nhwc_to_nchw(const d2b_pyramid* pyr, int N, int C, float* const* dst, void* stream) {
-  return d2b_pyramid_nhwc_to_nchw_t(pyr, N, C, reinterpret_cast<void* const*>(dst), D2B_F32, stream);
-}
-
-D2B_API int d2b_roi_pooler_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
-                                           const float* rois, int K, int pooled_h, int pooled_w, int sampling_ratio, int aligned,
-                                           void* stream) {
-  Pyr P;
-  if (!make_pyr(pyr, P) || N < 0 || C < 0 || !dtype_ok(grad_dtype)) return D2B_EINVAL;
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.grad[l]) return D2B_EINVAL;
-  if (int rc = zero_grads(P, N, C, (cudaStream_t)stream)) return rc;
-  if (K == 0 || C == 0 || N == 0) return D2B_OK;
-  if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  return launch_bwd_nhwc(P, N, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, grad_out, (cudaStream_t)stream, grad_dtype);
-}
-
-D2B_API int d2b_roi_pooler_backward_nhwc(const d2b_pyramid* pyr, int N, int C, const float* grad_out, const float* rois,
-                                         int K, int pooled_h, int pooled_w, int sampling_ratio, int aligned, void* stream) {
-  return d2b_roi_pooler_backward_nhwc_t(pyr, N, C, grad_out, D2B_F32, rois, K, pooled_h, pooled_w, sampling_ratio, aligned, stream);
-}
-
-D2B_API int d2b_roi_pooler_backward(const d2b_pyramid* pyr, int N, int C, const float* grad_out, const float* rois,
-                                    int K, int pooled_h, int pooled_w, int sampling_ratio, int aligned, void* stream) {
-  Pyr P;
-  if (!make_pyr(pyr, P) || N < 0 || C < 0) return D2B_EINVAL;
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.grad[l]) return D2B_EINVAL;
-  if (int rc = zero_grads(P, N, C, (cudaStream_t)stream)) return rc;
-  if (K == 0 || C == 0 || N == 0) return D2B_OK;
-  if (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  return launch_fwd(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, aligned, nullptr, (cudaStream_t)stream, grad_out);
-}
-
-// ------------------------------------------------------------------ multi-level rotated pooler
-// ROIPooler(pooler_type="ROIAlignRotated") with several levels: the per-level loop of detectron2/modeling/poolers.py:245-263 as
-// one launch per direction, the level of each RoI picked in-kernel from its w*h.  The reference samples rotated RoIs in fp32
-// whatever the feature dtype (layers/roi_align_rotated.py:81-83), so there are no separate level boxes: level_rois must be
-// NULL.  Every argument is checked before anything is launched.
-static int rot_pooler_args(const d2b_pyramid* pyr, int N, int C, int K, int dtype, Pyr& P) {
-  if (!make_pyr(pyr, P) || P.level_rois || N < 0 || C < 0 || K < 0 || !dtype_ok(dtype)) return D2B_EINVAL;
-  if (N == 0 && K > 0) return D2B_EINVAL;  // RoIs of images that do not exist
-  return D2B_OK;
-}
-
-D2B_API int d2b_roi_pooler_rotated_forward(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
-                                           int pooled_w, int sampling_ratio, float* out, void* stream) {
-  Pyr P;
-  if (rot_pooler_args(pyr, N, C, K, D2B_F32, P)) return D2B_EINVAL;
-  if (K == 0 || C == 0) return D2B_OK;
-  if (!rois || !out || N <= 0 || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.feat[l]) return D2B_EINVAL;
-  int cpc = pick_c_per_cta(K, C);
-  dim3 grid(K, d2b_cdiv(C, cpc));
-  roi_align_rot_fwd_kernel<1024><<<grid, kThreads, 0, (cudaStream_t)stream>>>(P, rois, C, pooled_h, pooled_w, sampling_ratio,
-                                                                               cpc, out);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
-}
-
-D2B_API int d2b_roi_pooler_rotated_forward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const float* rois, int K, int pooled_h,
-                                                  int pooled_w, int sampling_ratio, void* out, int out_dtype, void* stream) {
-  Pyr P;
-  if (rot_pooler_args(pyr, N, C, K, out_dtype, P)) return D2B_EINVAL;
-  if (K == 0 || C == 0) return D2B_OK;
-  if (!rois || !out || N <= 0 || pooled_h <= 0 || pooled_w <= 0) return D2B_EINVAL;
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.feat[l] || (reinterpret_cast<uintptr_t>(P.feat[l]) & 15) != 0) return D2B_EINVAL;
-  return launch_rot_nhwc<false>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, nullptr, out, (cudaStream_t)stream,
-                                out_dtype);
-}
-
-D2B_API int d2b_roi_pooler_rotated_backward(const d2b_pyramid* pyr, int N, int C, const float* grad_out, const float* rois,
-                                            int K, int pooled_h, int pooled_w, int sampling_ratio, void* stream) {
-  Pyr P;
-  if (rot_pooler_args(pyr, N, C, K, D2B_F32, P)) return D2B_EINVAL;
-  if (N == 0 || C == 0) return D2B_OK;  // no gradient element to write
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.grad[l]) return D2B_EINVAL;
-  if (K > 0 && (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0)) return D2B_EINVAL;
-  int rc = zero_grads(P, N, C, (cudaStream_t)stream);
-  if (rc || K == 0) return rc;
-  int cpc = pick_c_per_cta(K, C);
-  dim3 grid(K, d2b_cdiv(C, cpc));
-  roi_align_rot_bwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(P, grad_out, rois, C, pooled_h, pooled_w,
-                                                                        sampling_ratio, cpc);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
-}
-
-D2B_API int d2b_roi_pooler_rotated_backward_nhwc_t(const d2b_pyramid* pyr, int N, int C, const void* grad_out, int grad_dtype,
-                                                   const float* rois, int K, int pooled_h, int pooled_w, int sampling_ratio,
-                                                   void* stream) {
-  Pyr P;
-  if (rot_pooler_args(pyr, N, C, K, grad_dtype, P)) return D2B_EINVAL;
-  if (N == 0 || C == 0) return D2B_OK;
-  for (int l = 0; l < P.num_levels; ++l)
-    if (!P.grad[l] || (reinterpret_cast<uintptr_t>(P.grad[l]) & 15) != 0) return D2B_EINVAL;
-  if (K > 0 && (!grad_out || !rois || pooled_h <= 0 || pooled_w <= 0)) return D2B_EINVAL;
-  if (int rc = K > 0 ? nhwc_supported(P.num_levels, P.H, P.W, C, pooled_h, pooled_w, D2B_ROI_ROTATED | D2B_ROI_BACKWARD)
-                     : D2B_OK)
-    return rc;  // before the zero-fill
-  int rc = zero_grads(P, N, C, (cudaStream_t)stream);
-  if (rc || K == 0) return rc;
-  return launch_rot_nhwc<true>(P, rois, K, C, pooled_h, pooled_w, sampling_ratio, grad_out, nullptr, (cudaStream_t)stream,
-                               grad_dtype);
 }

@@ -92,7 +92,7 @@ def _to_nhwc(fs, P, n: int, c: int, device):
     fp32 NHWC buffers; returns them.  For half-precision levels the layout change is also the up-cast."""
     bufs = [torch.empty((t.shape[0], t.shape[2], t.shape[3], t.shape[1]), dtype=torch.float32, device=device) for t in fs]
     dst = (C.c_void_p * len(bufs))(*[b.data_ptr() for b in bufs])
-    check(_C.lib().d2b_pyramid_nchw_to_nhwc_t(C.byref(P), n, c, dst, _C.DTYPE_CODE[fs[0].dtype], stream_ptr(device)),
+    check(_C.lib().d2b_pyramid_nchw_to_nhwc(C.byref(P), n, c, dst, _C.DTYPE_CODE[fs[0].dtype], stream_ptr(device)),
           "pyramid_nchw_to_nhwc")
     return bufs
 
@@ -107,7 +107,7 @@ def _from_nhwc(bufs, n: int, c: int, device, dtype=torch.float32):
         P.feat[l] = b.data_ptr()
         P.H[l], P.W[l] = b.shape[1], b.shape[2]
     dst = (C.c_void_p * len(outs))(*[o.data_ptr() for o in outs])
-    check(_C.lib().d2b_pyramid_nhwc_to_nchw_t(C.byref(P), n, c, dst, _C.DTYPE_CODE[dtype], stream_ptr(device)),
+    check(_C.lib().d2b_pyramid_nhwc_to_nchw(C.byref(P), n, c, dst, _C.DTYPE_CODE[dtype], stream_ptr(device)),
           "pyramid_nhwc_to_nchw")
     return outs
 
@@ -187,24 +187,20 @@ def _roi_forward(feats, rois, scales, pooled_h: int, pooled_w: int, sampling_rat
     out_dt = feats[0].dtype if (layout != "nchw" and feats[0].dtype in _C.DTYPE_CODE) else torch.float32
     out = torch.empty((k, c, pooled_h, pooled_w), dtype=out_dt, device=r.device)
     if numel:
-        lib = _C.lib()
-        what = "roi_pooler_rotated_forward" if rotated else "roi_pooler_forward"
+        flags = (_C.ROI_ROTATED if rotated else 0) | (_C.ROI_NHWC if layout != "nchw" else 0)
         with torch.cuda.device(r.device):
             if layout != "cl":
                 fs = [t.contiguous() for t in fs]
             # channels_last tensors: same logical shape, NHWC storage -- _pyramid only takes pointers and H, W
             P = _pyramid(fs, None, scales, *levels, lr)
-            args = (C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w, sampling_ratio) + (() if rotated else (int(aligned),))
-            if layout == "nchw":
-                fn = lib.d2b_roi_pooler_rotated_forward if rotated else lib.d2b_roi_pooler_forward
-                check(fn(*args, ptr(out), stream_ptr(r.device)), what)
-            else:
-                if layout == "xpose":
-                    bufs = _to_nhwc(fs, P, n, c, r.device)
-                    for l, b in enumerate(bufs):
-                        P.feat[l] = b.data_ptr()
-                fn = lib.d2b_roi_pooler_rotated_forward_nhwc_t if rotated else lib.d2b_roi_pooler_forward_nhwc_t
-                check(fn(*args, ptr(out), _C.DTYPE_CODE[out_dt], stream_ptr(r.device)), what + "_nhwc")
+            if layout == "xpose":
+                bufs = _to_nhwc(fs, P, n, c, r.device)
+                for l, b in enumerate(bufs):
+                    P.feat[l] = b.data_ptr()
+            check(_C.lib().d2b_roi_pooler_forward(C.byref(P), n, c, ptr(r), k, pooled_h, pooled_w, sampling_ratio,
+                                                  int(aligned), flags, ptr(out), _C.DTYPE_CODE[out_dt],
+                                                  stream_ptr(r.device)),
+                  "roi_pooler_forward")
     return out if out.dtype == feats[0].dtype else out.to(feats[0].dtype)
 
 
@@ -221,25 +217,19 @@ def _roi_backward(grad, rois, shapes, scales, pooled_h: int, pooled_w: int, samp
                            channels_last) if n * c else "nchw")
     # the channels-last kernels read fp16 / bf16 gradients in place; the NCHW kernels take fp32
     g = grad.contiguous() if (layout != "nchw" and grad.dtype in _C.DTYPE_CODE) else _f32c(grad)
-    lib = _C.lib()
-    what = "roi_pooler_rotated_backward" if rotated else "roi_pooler_backward"
-    args = (ptr(r), r.shape[0], pooled_h, pooled_w, sampling_ratio) + (() if rotated else (int(aligned),))
+    flags = (_C.ROI_ROTATED if rotated else 0) | (_C.ROI_NHWC if layout != "nchw" else 0)
     with torch.cuda.device(g.device):
         if layout == "nchw":
             grads = [torch.empty((n, c, h, w), dtype=torch.float32, device=g.device) for (h, w) in hw]
-            P = _pyramid(grads, grads, scales, *levels, lr)
-            fn = lib.d2b_roi_pooler_rotated_backward if rotated else lib.d2b_roi_pooler_backward
-            check(fn(C.byref(P), n, c, ptr(g), *args, stream_ptr(g.device)), what)
         else:
             bufs = [torch.empty((n, h, w, c), dtype=torch.float32, device=g.device) for (h, w) in hw]
-            views = [b.permute(0, 3, 1, 2) for b in bufs]  # logical NCHW shape: _pyramid reads H, W from dims 2, 3
-            P = _pyramid(views, views, scales, *levels, lr)
-            fn = lib.d2b_roi_pooler_rotated_backward_nhwc_t if rotated else lib.d2b_roi_pooler_backward_nhwc_t
-            check(fn(C.byref(P), n, c, ptr(g), _C.DTYPE_CODE[g.dtype], *args, stream_ptr(g.device)), what + "_nhwc")
-            if layout == "cl":
-                grads = views
-            else:
-                grads = _from_nhwc(bufs, n, c, g.device, grad.dtype if (half_grads and grad.dtype in _HALF) else torch.float32)
+            grads = [b.permute(0, 3, 1, 2) for b in bufs]  # logical NCHW shape: _pyramid reads H, W from dims 2, 3
+        P = _pyramid(grads, grads, scales, *levels, lr)
+        check(_C.lib().d2b_roi_pooler_backward(C.byref(P), n, c, ptr(g), _C.DTYPE_CODE[g.dtype], ptr(r), r.shape[0], pooled_h,
+                                               pooled_w, sampling_ratio, int(aligned), flags, stream_ptr(g.device)),
+              "roi_pooler_backward")
+        if layout == "xpose":
+            grads = _from_nhwc(bufs, n, c, g.device, grad.dtype if (half_grads and grad.dtype in _HALF) else torch.float32)
     if half_grads and grad.dtype in _HALF:
         grads = [t if t.dtype == grad.dtype else t.to(grad.dtype) for t in grads]
     return grads

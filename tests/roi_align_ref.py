@@ -18,17 +18,17 @@ import numpy as np
 from test_roi_align_column_walk import sample_pos, tap_list
 
 # roi_align.cu constants
-K_MAXE, K_MAXP, K_CAPPX, K_ROWOFF = 32, 16, 448, 1536  # :327-333
-K_COLCAP = 192                                          # :846
-K_NHWC_CH, K_NHWC_CHUNK = 128, 64                       # :774-775
-K_BWD_BAND, K_BWD_MAXFW, K_BWD_WARPS = 64, 96, 8        # :1161-1163
+K_MAXE, K_MAXP, K_CAPPX, K_ROWOFF = 32, 16, 448, 1536  # :295-301
+K_COLCAP = 192                                          # :814
+K_NHWC_CH, K_NHWC_CHUNK = 128, 64                       # :742-743
+K_BWD_BAND, K_BWD_MAXFW, K_BWD_WARPS = 64, 96, 8        # :1123-1125
 EPS32 = 2.0 ** -24
 
 Geom = namedtuple("Geom", "b start_h start_w bin_h bin_w gh gw count raw_h raw_w")
 
 
 def geom(roi, scale, ph, pw, sr, aligned):
-    """load_geom<false> (:107-148) in fp32.  raw_h / raw_w: the box sides before the aligned=False clamp to one pixel."""
+    """load_geom<false> (:80-122) in fp32.  raw_h / raw_w: the box sides before the aligned=False clamp to one pixel."""
     f = np.float32
     s, off = f(scale), f(0.5 if aligned else 0.0)
     sw, sh = f(f(roi[1]) * s) - off, f(f(roi[2]) * s) - off
@@ -42,7 +42,7 @@ def geom(roi, scale, ph, pw, sr, aligned):
 
 
 def lists(g, ph, pw, h, w):
-    """The per-bin-row and per-bin-column tap lists (add_tap, :340-354) without the kMaxE cap: [(index, weight)] each."""
+    """The per-bin-row and per-bin-column tap lists (add_tap, :308-322) without the kMaxE cap: [(index, weight)] each."""
     ys = [tap_list(g.start_h, g.bin_h, g.gh, p, h, fp32=True) for p in range(ph)]
     xs = [tap_list(g.start_w, g.bin_w, g.gw, p, w, fp32=True) for p in range(pw)]
     return ys, xs
@@ -182,7 +182,7 @@ def cdiv(a, b):
 
 
 def launch_fwd_nhwc(k, c, ph, pw, sms):
-    """launch_fwd_nhwc (:1134-1142): (nchunks, chunk) of the channels-last forward's grid.z."""
+    """launch_fwd_nhwc (:1101-1105): (nchunks, chunk) of the channels-last forward's grid.z."""
     bins, slabs = ph * pw, cdiv(c, K_NHWC_CH)
     want = cdiv(8 * sms, k * slabs)
     nchunks = max(cdiv(bins, K_NHWC_CHUNK), min(want, cdiv(bins, 8)))
@@ -192,12 +192,12 @@ def launch_fwd_nhwc(k, c, ph, pw, sms):
     return cdiv(bins, chunk), chunk
 
 
-def bwd_nhwc_smem(rows, pw):  # :1407-1409
+def bwd_nhwc_smem(rows, pw):  # :1369-1371
     return 4 * K_NHWC_CH * (rows * pw + K_BWD_WARPS * pw)
 
 
 def launch_bwd_nhwc(k, c, ph, pw, sms):
-    """launch_bwd_nhwc (:1418-1423): bin rows per CTA of the channels-last backward."""
+    """launch_bwd_nhwc (:1378-1382): bin rows per CTA of the channels-last backward."""
     slabs, rows = cdiv(c, K_NHWC_CH), ph
     while (rows > 4 and (bwd_nhwc_smem(rows, pw) > 100 * 1024 or k * slabs * cdiv(ph, rows) < 4 * sms)
            and bwd_nhwc_smem(rows, pw) > 56 * 1024):
@@ -206,7 +206,7 @@ def launch_bwd_nhwc(k, c, ph, pw, sms):
 
 
 def nhwc_bwd_supported(ph, pw):
-    """nhwc_supported's backward branch (:1555-1560): the tile at the deepest split launch_bwd_nhwc may take fits 180 KB."""
+    """nhwc_supported's backward branch (:1514-1519): the tile at the deepest split launch_bwd_nhwc may take fits 180 KB."""
     rows = ph
     while rows > 4 and bwd_nhwc_smem(rows, pw) > 100 * 1024:
         rows = (rows + 1) // 2
@@ -214,7 +214,7 @@ def nhwc_bwd_supported(ph, pw):
 
 
 def launch_fwd(k, c, sms):
-    """launch_fwd (:750-753): channel groups of 4 per CTA of the NCHW kernel."""
+    """launch_fwd (:718-721): channel groups of 4 per CTA of the NCHW kernel."""
     ngroup = cdiv(c, 4)
     gpc = ngroup
     while gpc > 8 and k * cdiv(ngroup, gpc) < 24 * sms:
@@ -227,12 +227,12 @@ def slabs(c):
     return [(c0, min(K_NHWC_CH, c - c0)) for c0 in range(0, c, K_NHWC_CH)]
 
 
-def _padded_x(n):  # :1014 (table) and :1043 (per-bin loop): lists padded to 4, or to a multiple of 8 when longer
+def _padded_x(n):  # :982 (table) and :1011 (per-bin loop): lists padded to 4, or to a multiple of 8 when longer
     return 0 if n == 0 else (4 if n <= 4 else (n + 7) & ~7)
 
 
 def walk_refusals(R, chunk):
-    """Why roi_align_nhwc_kernel does not take the column walk for this RoI (:1002-1018, :1055): a subset of
+    """Why roi_align_nhwc_kernel does not take the column walk for this RoI (:970-986, :1023): a subset of
     {three_bins, colcap, profit, nymax, pw7}; empty = the walk runs."""
     xl, pw = R.xlists, R.pw
     why = set()
@@ -259,7 +259,7 @@ def walk_refusals(R, chunk):
 
 
 def nhwc_fwd_labels(R, chunk, nchunks):
-    """Paths of roi_align_nhwc_kernel for one RoI (:1049-1114)."""
+    """Paths of roi_align_nhwc_kernel for one RoI (:1017-1082)."""
     bins = R.ph * R.pw
     if R.ph > K_MAXP or R.pw > K_MAXP:
         return {"fwd_onfly_pooled"}
@@ -277,7 +277,7 @@ def nhwc_fwd_labels(R, chunk, nchunks):
                 if ny == 0:
                     out.add("walk_empty_row")
                     continue
-                out.add("walk_ry%d" % ny)  # ny <= 6: one chunk of ny tap rows (:1070)
+                out.add("walk_ry%d" % ny)  # ny <= 6: one chunk of ny tap rows (:1038)
                 if pw0 > 0:
                     out.add("walk_carry_in")
         return out
@@ -294,13 +294,13 @@ def nhwc_fwd_labels(R, chunk, nchunks):
                 continue
             form = "bin42" if _padded_x(nx) <= 4 else "bin81"
             out.add(form)
-            if ny % 2 and nx % (4 if form == "bin42" else 8):  # padding taps on both axes (:966, :1043)
+            if ny % 2 and nx % (4 if form == "bin42" else 8):  # padding taps on both axes (:934, :1011)
                 out.add(form + "_padded")
     return out
 
 
 def nhwc_bwd_labels(R, rows):
-    """Paths of roi_align_bwd_nhwc_kernel for one RoI, over its grid.z CTAs of `rows` bin rows (:1219-1403)."""
+    """Paths of roi_align_bwd_nhwc_kernel for one RoI, over its grid.z CTAs of `rows` bin rows (:1181-1365)."""
     if R.ph > K_MAXP or R.pw > K_MAXP:
         return {"bwd_per_sample_pooled"}
     out = set()
@@ -309,11 +309,11 @@ def nhwc_bwd_labels(R, rows):
         yl = R.ylists[ph0:ph0 + rows]
         yrows = [i for l in yl for i, _ in l]
         if not xcols or not yrows:
-            out.add("bwd_empty")  # :1266
+            out.add("bwd_empty")  # :1228
             continue
         fw = max(xcols) - min(xcols) + 1
         if fw > K_BWD_MAXFW:
-            out.add("bwd_per_sample_wide")  # :1267
+            out.add("bwd_per_sample_wide")  # :1229
             continue
         ymin, ymax = min(yrows), max(yrows)
         nb = cdiv(ymax - ymin + 1, K_BWD_BAND)
@@ -324,12 +324,12 @@ def nhwc_bwd_labels(R, rows):
                 out.add("bwd_band_edge_in_bin_row")
         colcnt = max(sum(any(i == x for i, _ in l) for l in R.xlists) for x in set(xcols))
         rowcnt = max(sum(any(i == y for i, _ in l) for l in yl) for y in set(yrows))
-        out.add("bwd_general" if max(colcnt, rowcnt) > 2 else "bwd_separable")  # s_wide (:1304, :1337)
+        out.add("bwd_general" if max(colcnt, rowcnt) > 2 else "bwd_separable")  # s_wide (:1266, :1299)
     return out
 
 
 def v3_labels(R):
-    """Mode of roi_align_v3_kernel for one RoI (:385-496): the same in the forward and the backward."""
+    """Mode of roi_align_v3_kernel for one RoI (:353-464): the same in the forward and the backward."""
     if R.ph > K_MAXP or R.pw > K_MAXP or any(len(l) > K_MAXE for l in R.ylists + R.xlists):
         return {"v3_onfly"}
     xs = [i for l in R.xlists for i, _ in l]
@@ -341,7 +341,7 @@ def v3_labels(R):
     if (ymax - ymin + 1) * fw > K_ROWOFF:
         return {"v3_direct_rowoff"}
     nb, ph0 = 0, 0
-    while ph0 < R.ph:  # greedy bands of bin rows (:443-465)
+    while ph0 < R.ph:  # greedy bands of bin rows (:411-433)
         yb, ye, ph1 = 1 << 30, -1, ph0
         while ph1 < R.ph:
             l = R.ylists[ph1]

@@ -19,7 +19,10 @@ def test_header_symbols_exported():
     for name in declared:
         assert hasattr(lib, name), name
     assert set(_C.EXPORTED) == declared
-    assert lib.d2b_abi_version() == _C.ABI_VERSION == 4
+    assert {n for n in declared if n.startswith(("d2b_roi_", "d2b_pyramid_"))} == {
+        "d2b_roi_pooler_forward", "d2b_roi_pooler_backward", "d2b_roi_pooler_nhwc_supported", "d2b_pyramid_nchw_to_nhwc",
+        "d2b_pyramid_nhwc_to_nchw"}
+    assert lib.d2b_abi_version() == _C.ABI_VERSION == 5
     assert lib.d2b_arch() == b"sm_90a"
     assert _C.get_cuda_version().startswith("CUDA 12")
 
@@ -199,10 +202,9 @@ def test_pooler_layout_policy_host_logic(monkeypatch):
         ops.pyramid_to_channels_last(nchw)
 
 
-def test_channels_last_limits_and_single_level_entry_points_without_a_gpu(monkeypatch):
+def test_channels_last_limits_without_a_gpu(monkeypatch):
     """d2b_roi_pooler_nhwc_supported is the one statement of the channels-last kernels' shape limits; the layout chooser
-    sends every shape it refuses to the NCHW kernels.  The single-level entry points are one-level pyramid calls with the
-    status codes they always had.  Every call here returns before any CUDA call."""
+    sends every shape it refuses to the NCHW kernels.  Every call here is host-only."""
     import ctypes as C
 
     from detectron2_b200 import _C, ops
@@ -244,39 +246,97 @@ def test_channels_last_limits_and_single_level_entry_points_without_a_gpu(monkey
     assert ops._pick_layout([x], 1, (20, 20), rotated=True) == "nchw"
     assert ops._pick_layout([tuple(x.shape)], 1, (20, 20), rotated=True, backward=True, channels_last=False) == "nchw"
 
-    # single-level entry points (the pointers are never dereferenced: each call below fails or returns before a launch).
-    # Forwards: (input, N, C, H, W, rois, K, scale, PH, PW, sr[, aligned], out, stream), in the order
-    # axis-aligned NCHW, axis-aligned channels-last, rotated NCHW, rotated channels-last.
-    def fwd(which=range(4), inp=0x1000, n=2, c=8, h=16, w=16, rois=0x2000, k=3, ph=7, pw=7, out=0x3000):
-        calls = (lambda: lib.d2b_roi_align_forward(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, 1, out, None),
-                 lambda: lib.d2b_roi_align_forward_nhwc(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, 1, out, None),
-                 lambda: lib.d2b_roi_align_rotated_forward(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, out, None),
-                 lambda: lib.d2b_roi_align_rotated_forward_nhwc(inp, n, c, h, w, rois, k, 0.25, ph, pw, 0, out, None))
-        return tuple(calls[i]() for i in which)
 
-    assert fwd(k=0) == fwd(c=0) == fwd(k=0, n=-1, inp=None) == (0, 0, 0, 0)  # nothing to compute: before any check
-    for bad in (dict(inp=None), dict(rois=None), dict(out=None), dict(n=0), dict(h=0), dict(w=-1), dict(ph=0), dict(k=-2)):
-        assert fwd(**bad) == (EINVAL,) * 4, bad
-    assert fwd((1, 3), inp=0x1004) == (EINVAL, EINVAL)          # the channels-last forms need a 16-byte aligned map
-    assert fwd((1, 3), c=6) == (UNSUPPORTED, UNSUPPORTED)
-    assert fwd((3,), ph=20, pw=20) == (UNSUPPORTED,)
+# The argument rule of d2b_roi_pooler_forward / _backward (include/d2b200.h), one row per fault: (what, arguments changed
+# from a valid call, expected status).  The expected status is a number, or a function of the call's kind that returns None
+# where the call is valid (it would launch, so it is not made).  `flag` is a bit added to the call's flags; pyramid keys:
+# `h` / `w` / `map` set H, W and feat = grad of the last level, `num_levels`, `max_level` and `level_rois` the fields of the
+# same name.
+EINVAL, UNSUPPORTED = -1, -3
+_ROI_FAULTS = [
+    ("no RoIs", dict(k=0), lambda t: None if t.bwd else 0),  # the backward zero-fills its gradient maps
+    ("no RoIs, nothing else valid", dict(k=0, n=-1, map=None), lambda t: EINVAL if t.bwd else 0),
+    ("no RoIs, no images", dict(k=0, n=0), 0),
+    ("no channels", dict(c=0), 0),
+    ("no channels, no data", dict(c=0, data=None), 0),
+    ("no images", dict(n=0), EINVAL),  # RoIs of images that do not exist
+    ("n < 0", dict(n=-1), EINVAL),
+    ("c < 0", dict(c=-4), EINVAL),
+    ("k < 0", dict(k=-1), EINVAL),
+    ("k < 0, no images", dict(k=-2, n=0), EINVAL),
+    ("pooled_h < 1", dict(ph=0), EINVAL),
+    ("pooled_w < 1", dict(pw=-1), EINVAL),
+    ("no rois", dict(rois=None), EINVAL),
+    ("no out / grad_out", dict(data=None), EINVAL),
+    ("no feature / gradient map", dict(map=None), EINVAL),
+    ("empty level", dict(h=0), EINVAL),
+    ("negative level height", dict(h=-1), EINVAL),
+    ("negative level width", dict(w=-3), EINVAL),
+    ("no levels", dict(num_levels=0), EINVAL),
+    ("too many levels", dict(num_levels=9), EINVAL),
+    ("levels do not match min_level..max_level", dict(max_level=6), lambda t: EINVAL if t.levels > 1 else None),
+    ("level boxes of rotated RoIs", dict(level_rois=0x30), lambda t: EINVAL if t.rot else None),
+    ("flag D2B_ROI_BACKWARD", dict(flag=2), EINVAL),
+    ("unknown flag", dict(flag=8), EINVAL),
+    ("dtype code 3", dict(dt=3), EINVAL),
+    ("dtype code -1", dict(dt=-1), EINVAL),
+    ("dtype code 9", dict(dt=9), EINVAL),
+    ("fp16 data", dict(dt=1), lambda t: None if t.nhwc else EINVAL),  # the NCHW kernels read and write fp32 only
+    ("bf16 data", dict(dt=2), lambda t: None if t.nhwc else EINVAL),
+    ("fp16 data, no rois", dict(dt=1, rois=None), EINVAL),
+    ("bf16 data, no out / grad_out", dict(dt=2, data=None), EINVAL),
+    ("misaligned map", dict(map=0x1004), lambda t: EINVAL if t.nhwc else None),
+    ("misaligned empty map", dict(map=0x1004, h=0), EINVAL),
+    ("misaligned map, c % 4 != 0", dict(map=0x1004, c=6), lambda t: EINVAL if t.nhwc else None),  # EINVAL first
+    ("c % 4 != 0", dict(c=6), lambda t: UNSUPPORTED if t.nhwc else None),
+    ("rotated tile > 150 KB", dict(ph=20, pw=20), lambda t: UNSUPPORTED if t.nhwc and t.rot else None),
+    ("tile of the backward > 180 KB", dict(ph=32, pw=32), lambda t: UNSUPPORTED if t.nhwc and (t.rot or t.bwd) else None),
+]
 
-    # Backwards: (grad_out, rois, K, scale, PH, PW, N, C, H, W, sr[, aligned], grad_in, stream), same order.  A backward
-    # with a non-empty gradient and valid arguments zero-fills it, so only the empty and the invalid cases are called here.
-    def bwd(which=range(4), go=0x1000, rois=0x2000, k=3, ph=7, pw=7, n=2, c=8, h=16, w=16, gin=0x3000):
-        calls = (lambda: lib.d2b_roi_align_backward(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, 1, gin, None),
-                 lambda: lib.d2b_roi_align_backward_nhwc(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, 1, gin, None),
-                 lambda: lib.d2b_roi_align_rotated_backward(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, gin, None),
-                 lambda: lib.d2b_roi_align_rotated_backward_nhwc(go, rois, k, 0.25, ph, pw, n, c, h, w, 0, gin, None))
-        return tuple(calls[i]() for i in which)
 
-    for bad in (dict(gin=None), dict(n=-1), dict(c=-4), dict(h=-1), dict(w=-3)):
-        assert bwd(**bad) == (EINVAL,) * 4, bad
-    assert bwd(h=0) == bwd(n=0) == bwd(c=0, go=None) == (0, 0, 0, 0)  # empty gradient: nothing to write
-    assert bwd((3,), gin=0x3004) == bwd((3,), gin=0x3004, h=0) == (EINVAL,)
-    # the rotated backwards check their arguments before the zero-fill launch
-    assert bwd((2, 3), go=None) == bwd((2, 3), rois=None) == bwd((2, 3), ph=0) == (EINVAL, EINVAL)
-    assert bwd((3,), c=6) == bwd((3,), ph=20, pw=20) == (UNSUPPORTED,)
+def _roi_pooler_call(lib, bwd, flags, levels, n=2, c=8, k=3, ph=7, pw=7, rois=0x10, data=0x20, dt=0, **pyr):
+    """One call on a one-level (a single-level op: 16x16 at scale 1/4) or four-level (64x96 .. 8x12) pyramid whose maps are
+    16-byte aligned pointers that are never dereferenced."""
+    import ctypes as C
+
+    from detectron2_b200 import _C
+
+    P = _C.Pyramid()
+    P.num_levels = levels
+    for l in range(levels):
+        P.H[l], P.W[l] = (16, 16) if levels == 1 else (64 >> l, 96 >> l)
+        P.scale[l] = 0.25 / 2 ** l
+        P.feat[l] = P.grad[l] = 0x1000 * (l + 1)
+    P.min_level, P.max_level, P.canonical_level, P.canonical_box_size = 2, 1 + levels, 4, 224.0
+    last = levels - 1
+    P.H[last], P.W[last] = pyr.get("h", P.H[last]), pyr.get("w", P.W[last])
+    P.feat[last] = P.grad[last] = pyr.get("map", P.feat[last])
+    P.num_levels, P.max_level = pyr.get("num_levels", levels), pyr.get("max_level", P.max_level)
+    P.level_rois = pyr.get("level_rois")
+    if bwd:
+        return lib.d2b_roi_pooler_backward(C.byref(P), n, c, data, dt, rois, k, ph, pw, 0, 1, flags, None)
+    return lib.d2b_roi_pooler_forward(C.byref(P), n, c, rois, k, ph, pw, 0, 1, flags, data, dt, None)
+
+
+def test_roi_pooler_entry_points_validate_arguments_without_a_gpu():
+    """Every fault gets its status before anything is launched, in each of the eight forward / backward x axis-aligned /
+    rotated x NCHW / channels-last kinds of call.  Without a GPU a launch attempt returns a positive CUDA error, so a negative
+    status here also shows that no launch came first (the gradient maps were not written)."""
+    import itertools
+    import types
+
+    from detectron2_b200 import _C
+
+    lib = _C.lib()
+    for bwd, rot, nhwc, levels in itertools.product((False, True), (False, True), (False, True), (1, 4)):
+        flags = (_C.ROI_ROTATED if rot else 0) | (_C.ROI_NHWC if nhwc else 0)
+        kind = types.SimpleNamespace(bwd=bwd, rot=rot, nhwc=nhwc, levels=levels)
+        for what, args, want in _ROI_FAULTS:
+            want = want(kind) if callable(want) else want
+            if want is not None:
+                a = dict(args)
+                got = _roi_pooler_call(lib, bwd, flags | a.pop("flag", 0), levels, **a)
+                assert got == want, (what, "bwd" if bwd else "fwd", flags, levels, got)
 
 
 def test_roi_pooler_no_images():  # /root/reference/tests/modeling/test_roi_pooler.py:107-115
@@ -342,10 +402,8 @@ def test_new_entry_points_validate_arguments_without_a_gpu():
     P.num_levels = 1
     P.H[0], P.W[0] = 8, 8
     dst = (C.c_void_p * 1)(None)
-    assert lib.d2b_pyramid_nchw_to_nhwc_t(C.byref(P), 1, 4, dst, 7, None) == EINVAL
-    assert lib.d2b_pyramid_nhwc_to_nchw_t(C.byref(P), 1, 4, dst, -1, None) == EINVAL
-    assert lib.d2b_roi_pooler_forward_nhwc_t(C.byref(P), 1, 4, None, 3, 7, 7, 0, 1, None, 5, None) == EINVAL
-    assert lib.d2b_roi_pooler_backward_nhwc_t(C.byref(P), 1, 4, None, 9, None, 3, 7, 7, 0, 1, None) == EINVAL
+    assert lib.d2b_pyramid_nchw_to_nhwc(C.byref(P), 1, 4, dst, 7, None) == EINVAL
+    assert lib.d2b_pyramid_nhwc_to_nchw(C.byref(P), 1, 4, dst, -1, None) == EINVAL
     assert _C.DTYPE_CODE == {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
     # bit-packed paste: boolean output only
     assert lib.d2b_paste_masks_packed(None, None, 3, 28, 10, 10, -1.0, None, None) == EINVAL

@@ -15,7 +15,7 @@ GEO = ([1, 1], [1, 1], [1, 1], 1, 1)  # stride, padding, dilation, groups, defor
 # d2b_dcn_params of the two shapes: N, Cin, H, W, Cout, kh, kw, stride, padding, dilation (h, w each), groups, dg
 PARAMS = {(2, c, 10, 12, c, 3, 3, 1, 1, 1, 1, 1, 1, 1, 1): "P%d" % c for c in (64, 48)}
 _SHORT = {"d2b_deform_conv_forward": "fwd", "d2b_deform_conv_backward": "bwd", "d2b_deform_conv_fused_forward": "ffwd",
-          "d2b_deform_conv_fused_backward": "fbwd", "d2b_pyramid_nchw_to_nhwc_t": "to_nhwc"}
+          "d2b_deform_conv_fused_backward": "fbwd", "d2b_pyramid_nchw_to_nhwc": "to_nhwc"}
 
 
 def _describe(name, args):

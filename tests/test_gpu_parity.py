@@ -177,6 +177,19 @@ def test_roi_align_rotated_kats(L):
     assert torch.allclose(xa.grad, xr.grad, atol=1e-5)
 
 
+def test_roi_align_backward_ops_with_nothing_to_write():
+    # a single-level backward whose gradient has no element (h == 0, or no images while there are three RoIs) returns the
+    # empty gradient without a native call: the pooler entry points refuse such a pyramid
+    from detectron2_b200 import ops
+
+    grad = torch.randn(3, 8, 7, 7, device=DEV)
+    for n, h in ((2, 0), (0, 16)):
+        gx = ops.roi_align_backward_op(grad, torch.zeros(3, 5, device=DEV), 0.25, 7, 7, n, 8, h, 16, 0, True)
+        gr = ops.roi_align_rotated_backward_op(grad, torch.zeros(3, 6, device=DEV), 0.25, 7, 7, n, 8, h, 16, 0)
+        for g in (gx, gr):
+            assert g.shape == (n, 8, h, 16) and g.dtype == grad.dtype and g.device == grad.device, (n, h)
+
+
 # ------------------------------------------------------------------------------- NMS
 def test_nms_golden_bit_exact(L, golden):
     d = golden("nms")
