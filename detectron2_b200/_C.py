@@ -24,12 +24,13 @@ class DcnParams(C.Structure):
 
 MAX_LEVELS = 8
 MAX_IMAGES = 64  # D2B_MAX_IMAGES
-ABI_VERSION = 5  # include/d2b200.h D2B_ABI_VERSION
+ABI_VERSION = 6  # include/d2b200.h D2B_ABI_VERSION
 DCN_X_NHWC = 1   # D2B_DCN_X_NHWC
 ROI_ROTATED, ROI_BACKWARD, ROI_NHWC = 1, 2, 4  # D2B_ROI_ROTATED / D2B_ROI_BACKWARD / D2B_ROI_NHWC
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}  # D2B_F32 / D2B_F16 / D2B_BF16
 MATCH_ROTATED, MATCH_LOW_QUALITY, MATCH_APPEND_GT = 1, 2, 4  # D2B_MATCH_*
 MATCH_MAX_THRESHOLDS = 8  # D2B_MATCH_MAX_THRESHOLDS
+SELECT_ROTATED, SELECT_SEG_PER_IMAGE, SELECT_NO_OFFSETS, SELECT_LINEAR = 1, 2, 4, 8  # D2B_SELECT_*
 
 
 class Pyramid(C.Structure):
@@ -77,16 +78,11 @@ def _declare(lib):
         "d2b_nms_workspace_bytes": (sz, [i64, i, i64]),
         "d2b_nms": (i, [f32p, f32p, i64p, i64, d, i, i64, i64p, i64p, vp, sz, vp]),
         "d2b_rpn_prepare": (i, [C.POINTER(RpnLevels), i, f32p, f, i, f32p, f32p, f32p, f32p, i64p, vp, vp]),
-        "d2b_rpn_select": (i, [i64p, i64p, i, i, i, f32p, f32p, i64p, f32p, f32p, i64p, i64p, vp]),
-        "d2b_frcnn_prepare": (i, [f32p, f32p, C.POINTER(C.c_int), i, i, i, f32p, f, i, f32p, f32p, f32p, f32p, i64p, i64p,
+        "d2b_rpn_select": (i, [i64p, i64p, i, i, i, i, f32p, f32p, i64p, f32p, f32p, i64p, i64p, vp]),
+        "d2b_frcnn_prepare": (i, [f32p, f32p, C.POINTER(C.c_int), i, i, i, f32p, f, i, i, f32p, f32p, f32p, f32p, i64p, i64p,
                                   i64p, i64p, vp]),
-        "d2b_dense_prepare": (i, [C.POINTER(DenseLevels), i, i, C.POINTER(C.c_float), f, f32p, f32p, f32p, f32p, i64p, i64p,
-                                  vp]),
-        "d2b_dense_prepare_linear": (i, [C.POINTER(DenseLevels), i, i, f32p, f32p, f32p, f32p, i64p, i64p, vp]),
-        "d2b_rrpn_prepare": (i, [C.POINTER(RpnLevels), i, f32p, f, i, f32p, f32p, f32p, f32p, i64p, vp, vp]),
-        "d2b_frcnn_rotated_prepare": (i, [f32p, f32p, C.POINTER(C.c_int), i, i, i, f32p, f, i, i, f32p, f32p, f32p, f32p, i64p,
-                                          i64p, i64p, i64p, vp]),
-        "d2b_rpn_select_rotated": (i, [i64p, i64p, i, i, i, f32p, f32p, i64p, f32p, f32p, i64p, i64p, vp]),
+        "d2b_dense_prepare": (i, [C.POINTER(DenseLevels), i, i, C.POINTER(C.c_float), f, i, f32p, f32p, f32p, f32p, i64p,
+                                  i64p, vp]),
         "d2b_mask_loss_forward": (i, [f32p, i, i, i, u8p, i, i, i, f32p, i64p, i64p, f32p, u8p, vp]),
         "d2b_mask_loss_backward": (i, [f32p, i, i, i, u8p, i64p, f32p, f32p, vp]),
         "d2b_keypoints_workspace_bytes": (sz, [i, i]),
@@ -98,7 +94,6 @@ def _declare(lib):
                                        C.POINTER(C.c_float), f32p, f32p, i64p, i64p, vp, vp, sz, vp]),
         "d2b_dense_loss_backward": (i, [C.POINTER(DenseLossLevels), i, i, i, i, f32p, f32p, vp, i, f, f, f, i, f,
                                         C.POINTER(C.c_float), f32p, f32p, vp]),
-        "d2b_fcos_loss_workspace_bytes": (sz, [C.POINTER(DenseLossLevels), i, i, i]),
         "d2b_fcos_loss_forward": (i, [C.POINTER(DenseLossLevels), C.POINTER(C.c_void_p), i, i, i, f32p, f32p, i64p, f, f, f32p,
                                       f32p, f32p, i64p, vp, vp, sz, vp]),
         "d2b_fcos_loss_backward": (i, [C.POINTER(DenseLossLevels), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), i, i, i,

@@ -41,7 +41,7 @@ def topk_levels(proposals, logits, pre_nms_topk: int):
 
 def nms_select(nms_boxes, nms_scores, cat_ids, flat_boxes, raw_scores, n: int, t: int, topk: int, nms_thresh: float,
                rotated: bool, max_segment: int):
-    """ONE `ops.nms_fixed` over the n * t candidates (category -1 = ignored), then `d2b_rpn_select[_rotated]`: every image
+    """ONE `ops.nms_fixed` over the n * t candidates (category -1 = ignored), then `d2b_rpn_select`: every image
     gets the first `topk` of its survivors.  Returns (out_boxes [n, topk, 4 or 5], out_scores [n, topk], out_index
     [n, topk] into the candidates, counts [n]); rows past counts[i] are zero.  Static shapes: capturable."""
     from . import _C
@@ -60,10 +60,11 @@ def nms_select(nms_boxes, nms_scores, cat_ids, flat_boxes, raw_scores, n: int, t
         return out_boxes, out_scores, out_index, counts
     keep, num_keep = ops.nms_fixed(nms_boxes, nms_scores, cat_ids, float(nms_thresh), rotated, apply_offsets=False,
                                    max_segment=max_segment)
-    select = _C.lib().d2b_rpn_select_rotated if rotated else _C.lib().d2b_rpn_select
+    flags = _C.SELECT_ROTATED if rotated else 0
     with torch.cuda.device(device):
-        check(select(ptr(keep), ptr(num_keep), n, t, int(topk), ptr(flat_boxes), ptr(raw_scores), ptr(cat_ids),
-                     ptr(out_boxes), ptr(out_scores), ptr(out_index), ptr(counts), stream_ptr(device)), "rpn_select")
+        check(_C.lib().d2b_rpn_select(ptr(keep), ptr(num_keep), n, t, int(topk), flags, ptr(flat_boxes), ptr(raw_scores),
+                                      ptr(cat_ids), ptr(out_boxes), ptr(out_scores), ptr(out_index), ptr(counts),
+                                      stream_ptr(device)), "rpn_select")
     return out_boxes, out_scores, out_index, counts
 
 

@@ -795,10 +795,6 @@ D2B_API int d2b_dense_loss_backward(const d2b_dense_loss_levels* lv, int N, int 
   return dense_dispatch<true>(blocks, dtype, box_dim, label_kind, P, A, (cudaStream_t)stream);
 }
 
-D2B_API size_t d2b_fcos_loss_workspace_bytes(const d2b_dense_loss_levels* lv, int N, int K, int dtype) {
-  return d2b_dense_loss_workspace_bytes(lv, N, K, dtype);
-}
-
 D2B_API int d2b_fcos_loss_forward(const d2b_dense_loss_levels* lv, const void* const* ctr, int N, int K, int dtype,
                                   const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma,
                                   float alpha, float* cls_sum, float* reg_sum, float* ctr_sum, int64_t* num_pos,

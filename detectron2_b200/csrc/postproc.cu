@@ -2,12 +2,12 @@
 // detectron2/modeling/proposal_generator/proposal_utils.py:22-135 (find_top_rpn_proposals) and rrpn.py:20-127
 // (find_top_rrpn_proposals) as fixed-capacity kernels, one CTA per image.
 //
-//   d2b_rpn_prepare / d2b_rrpn_prepare   gather the per-level top-k candidates, clip them to the image (Boxes.clip, :112 /
+//   d2b_rpn_prepare   gather the per-level top-k candidates, clip them to the image (Boxes.clip, :112 /
 //                     RotatedBoxes.clip), mark non-finite (:104-110) and too-small (:115-119) boxes as IGNORED (category -1)
 //                     instead of removing them, and apply the batched-NMS coordinate offsets per image -- torchvision's
 //                     level * (max coordinate + 1), or batched_nms_rotated's level * (max - min + 1) on the centres, over
 //                     that image's surviving boxes, fp32 -- so that every IoU rounds like the reference's;
-//   d2b_rpn_select[_rotated]   walks the score-ordered keep list of ONE NMS over all images and hands every image its first
+//   d2b_rpn_select    walks the score-ordered keep list of ONE NMS over all images and hands every image its first
 //                     post_nms_topk survivors (:129) in a fixed [N, post_nms_topk] layout + a count.
 //
 // Together with d2b_nms (category = image * L + level, per-category bound = pre_nms_topk) the whole selection is a
@@ -15,8 +15,8 @@
 // with boolean indexing and one `.item()` per image.  Compiled with -fmad=false like nms.cu (bit-exact clip / offsets).
 //
 // The box type is a template policy (XyxyBox / RotBox, boxes.cuh) of every candidate and selection kernel in this file:
-// rpn_prepare_kernel, frcnn_prepare_kernel (d2b_frcnn_prepare / d2b_frcnn_rotated_prepare) and rpn_select_kernel; the
-// rotated calls run d2b_nms with D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET.
+// rpn_prepare_kernel, frcnn_prepare_kernel and rpn_select_kernel.  Each entry point picks the instantiation from its
+// D2B_SELECT_* flags; the rotated calls run d2b_nms with D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET.
 #include <climits>
 #include <type_traits>
 
@@ -37,7 +37,7 @@ struct RpnLevels {
 
 __device__ __forceinline__ bool finitef(float v) { return fabsf(v) <= 3.402823466e38f; }  // false for inf and NaN
 
-// D = 4: xyxy boxes (d2b_rpn_select), D = 5: rotated boxes (d2b_rpn_select_rotated).
+// D = 4: xyxy boxes, D = 5: rotated boxes (D2B_SELECT_ROTATED).
 template <int D>
 __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* __restrict__ keep,
                                                               const long long* __restrict__ num_keep, int T, int post_topk,
@@ -84,11 +84,21 @@ __global__ void __launch_bounds__(kThreads) rpn_select_kernel(const long long* _
 
 namespace {
 
-template <int D>
-int rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk, const float* flat_boxes,
-               const float* raw_scores, const int64_t* cat_ids, float* out_boxes, float* out_scores, int64_t* out_index,
-               int64_t* counts, void* stream) {
-  if (N < 0 || T < 0 || post_nms_topk < 0) return D2B_EINVAL;
+// A flag bit the entry point does not take (`allowed`), SEG_PER_IMAGE without ROTATED, or NO_OFFSETS with it.
+bool bad_flags(int flags, int allowed) {
+  const bool rot = (flags & D2B_SELECT_ROTATED) != 0;
+  return (flags & ~allowed) != 0 || ((flags & D2B_SELECT_SEG_PER_IMAGE) && !rot) || ((flags & D2B_SELECT_NO_OFFSETS) && rot);
+}
+
+bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }  // xyxy boxes: float4 access
+
+}  // namespace
+
+D2B_API int d2b_rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk, int flags,
+                           const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
+                           float* out_scores, int64_t* out_index, int64_t* counts, void* stream) {
+  const bool rot = (flags & D2B_SELECT_ROTATED) != 0;
+  if (bad_flags(flags, D2B_SELECT_ROTATED) || N < 0 || T < 0 || post_nms_topk < 0) return D2B_EINVAL;
   if (N == 0) return D2B_OK;
   if (!counts) return D2B_EINVAL;
   if (T == 0 || post_nms_topk == 0) {
@@ -96,28 +106,13 @@ int rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int p
     return D2B_OK;
   }
   if (!keep || !num_keep || !flat_boxes || !raw_scores || !cat_ids || !out_boxes || !out_scores || !out_index) return D2B_EINVAL;
-  rpn_select_kernel<D><<<N, kThreads, 0, (cudaStream_t)stream>>>((const long long*)keep, (const long long*)num_keep, T,
-                                                                 post_nms_topk, flat_boxes, raw_scores,
-                                                                 (const long long*)cat_ids, out_boxes, out_scores,
-                                                                 (long long*)out_index, (long long*)counts);
+  if (!rot && (misaligned16(flat_boxes) || misaligned16(out_boxes))) return D2B_EINVAL;
+  const auto kernel = rot ? rpn_select_kernel<5> : rpn_select_kernel<4>;
+  kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>((const long long*)keep, (const long long*)num_keep, T, post_nms_topk,
+                                                   flat_boxes, raw_scores, (const long long*)cat_ids, out_boxes, out_scores,
+                                                   (long long*)out_index, (long long*)counts);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
-}
-
-}  // namespace
-
-D2B_API int d2b_rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
-                           const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
-                           float* out_scores, int64_t* out_index, int64_t* counts, void* stream) {
-  return rpn_select<4>(keep, num_keep, N, T, post_nms_topk, flat_boxes, raw_scores, cat_ids, out_boxes, out_scores, out_index,
-                       counts, stream);
-}
-
-D2B_API int d2b_rpn_select_rotated(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
-                                   const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
-                                   float* out_scores, int64_t* out_index, int64_t* counts, void* stream) {
-  return rpn_select<5>(keep, num_keep, N, T, post_nms_topk, flat_boxes, raw_scores, cat_ids, out_boxes, out_scores, out_index,
-                       counts, stream);
 }
 
 // ================================================================================================ Fast R-CNN / dense-head candidates
@@ -131,8 +126,8 @@ D2B_API int d2b_rpn_select_rotated(const int64_t* keep, const int64_t* num_keep,
 //                       with their box clipped to the image (:146-147) and torchvision's batched-NMS coordinate offsets.
 //   d2b_dense_prepare   DenseDetector._decode_per_level_predictions (meta_arch/dense_detector.py:186-235) after the per-level
 //                       top-k: Box2BoxTransform.apply_deltas (box_regression.py:78-116, same fp32 expression order) on the
-//                       selected (anchor, class) pairs only, class ids, coordinate offsets.
-//   d2b_dense_prepare_linear  the same for FCOS (meta_arch/fcos.py:253-301): Box2BoxTransformLinear.apply_deltas
+//                       selected (anchor, class) pairs only, class ids, coordinate offsets.  With D2B_SELECT_LINEAR the
+//                       same for FCOS (meta_arch/fcos.py:253-301): Box2BoxTransformLinear.apply_deltas
 //                       (box_regression.py:275-307) as the decode.
 namespace {
 
@@ -156,8 +151,8 @@ __device__ __forceinline__ float block_max(float v, float* s_red, float* s_out) 
   return *s_out;
 }
 
-// Box = XyxyBox: d2b_frcnn_prepare; RotBox: d2b_frcnn_rotated_prepare (rotated_fast_rcnn.py:84-122, the same steps on
-// RotatedBoxes, with `seg_per_image` for thresholds that IoU 0 passes: every candidate of the image in one NMS segment).
+// Box = RotBox: rotated_fast_rcnn.py:84-122, the same steps on RotatedBoxes, with `seg_per_image` for thresholds that IoU 0
+// passes: every candidate of the image in one NMS segment.
 template <class Box>
 __global__ void __launch_bounds__(kThreads) frcnn_prepare_kernel(const FrcnnImages I, const float* __restrict__ boxes,
                                                                  const float* __restrict__ scores, int K, int kreg,
@@ -385,49 +380,20 @@ __global__ void __launch_bounds__(kThreads) dense_prepare_kernel(const DenseLeve
 
 }  // namespace
 
-namespace {
-
-template <class Box>
-int frcnn_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes, int kreg,
-                  const float* image_hw, float score_thresh, int cap, int seg_per_image, float* cand_boxes, float* nms_boxes,
-                  float* nms_scores, float* raw_scores, int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand, int64_t* row_map,
-                  void* stream) {
-  if (N < 0 || N > D2B_MAX_IMAGES || num_classes <= 0 || (kreg != 1 && kreg != num_classes) || cap < 0 || !row_start)
+D2B_API int d2b_rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int flags,
+                            float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
+                            int* nonfinite, void* stream) {
+  const bool rot = (flags & D2B_SELECT_ROTATED) != 0;
+  if (bad_flags(flags, D2B_SELECT_ROTATED | D2B_SELECT_SEG_PER_IMAGE | D2B_SELECT_NO_OFFSETS) || !lv || lv->num_levels < 1 ||
+      lv->num_levels > D2B_MAX_LEVELS || N < 0 || !nonfinite)
     return D2B_EINVAL;
-  if (N == 0) return D2B_OK;
-  FrcnnImages I = {};
-  I.N = N;
-  for (int i = 0; i <= N; ++i) {
-    I.row_start[i] = row_start[i];
-    if (i && row_start[i] < row_start[i - 1]) return D2B_EINVAL;
-  }
-  if (!image_hw || !n_cand) return D2B_EINVAL;
-  if (row_start[N] > row_start[0] && (!boxes || !scores || !row_map)) return D2B_EINVAL;
-  if (cap > 0 && (!cand_boxes || !nms_boxes || !nms_scores || !raw_scores || !cand_flat || !cat_ids)) return D2B_EINVAL;
-  if (Box::D == 4 &&
-      ((reinterpret_cast<uintptr_t>(cand_boxes) & 15) != 0 || (reinterpret_cast<uintptr_t>(nms_boxes) & 15) != 0))
-    return D2B_EINVAL;
-  frcnn_prepare_kernel<Box><<<N, kThreads, 0, (cudaStream_t)stream>>>(I, boxes, scores, num_classes, kreg, image_hw,
-                                                                      score_thresh, cap, seg_per_image, cand_boxes, nms_boxes,
-                                                                      nms_scores, raw_scores, (long long*)cand_flat,
-                                                                      (long long*)cat_ids, (long long*)n_cand,
-                                                                      (long long*)row_map);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
-}
-
-template <class Box>
-int rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int use_offsets, int seg_per_image,
-                float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids, int* nonfinite,
-                void* stream) {
-  if (!lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0 || !nonfinite) return D2B_EINVAL;
   RpnLevels P = {};
   P.L = lv->num_levels;
   long long T = 0;
   for (int l = 0; l < P.L; ++l) {
     if (lv->A[l] < 0 || lv->k[l] < 0 || lv->k[l] > lv->A[l]) return D2B_EINVAL;
     if (N > 0 && lv->k[l] > 0 && (!lv->proposals[l] || !lv->topk_idx[l] || !lv->topk_scores[l])) return D2B_EINVAL;
-    if (Box::D == 4 && (reinterpret_cast<uintptr_t>(lv->proposals[l]) & 15) != 0) return D2B_EINVAL;  // float4 loads
+    if (!rot && misaligned16(lv->proposals[l])) return D2B_EINVAL;
     P.proposals[l] = lv->proposals[l];
     P.topk_idx[l] = lv->topk_idx[l];
     P.topk_scores[l] = lv->topk_scores[l];
@@ -439,101 +405,82 @@ int rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float mi
   if (T > INT_MAX) return D2B_EINVAL;
   P.t0[P.L] = (int)T;
   if (N > 0 && T > 0 && (!image_hw || !flat_boxes || !nms_boxes || !nms_scores || !raw_scores || !cat_ids)) return D2B_EINVAL;
-  if (Box::D == 4 &&
-      ((reinterpret_cast<uintptr_t>(flat_boxes) & 15) != 0 || (reinterpret_cast<uintptr_t>(nms_boxes) & 15) != 0))
-    return D2B_EINVAL;
+  if (!rot && (misaligned16(flat_boxes) || misaligned16(nms_boxes))) return D2B_EINVAL;
   D2B_CUDA(cudaMemsetAsync(nonfinite, 0, sizeof(int), (cudaStream_t)stream));
   if (N == 0 || T == 0) return D2B_OK;
-  rpn_prepare_kernel<Box><<<N, kThreads, 0, (cudaStream_t)stream>>>(P, (int)T, image_hw, min_box_size, use_offsets,
-                                                                    seg_per_image, flat_boxes, nms_boxes, nms_scores,
-                                                                    raw_scores, (long long*)cat_ids, nonfinite);
+  const auto kernel = rot ? rpn_prepare_kernel<RotBox> : rpn_prepare_kernel<XyxyBox>;
+  kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(P, (int)T, image_hw, min_box_size, (flags & D2B_SELECT_NO_OFFSETS) ? 0 : 1,
+                                                   (flags & D2B_SELECT_SEG_PER_IMAGE) ? 1 : 0, flat_boxes, nms_boxes,
+                                                   nms_scores, raw_scores, (long long*)cat_ids, nonfinite);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }
 
-}  // namespace
-
 D2B_API int d2b_frcnn_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes, int kreg,
-                              const float* image_hw, float score_thresh, int cap, float* cand_boxes, float* nms_boxes,
-                              float* nms_scores, float* raw_scores, int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand,
-                              int64_t* row_map, void* stream) {
-  return frcnn_prepare<XyxyBox>(boxes, scores, row_start, N, num_classes, kreg, image_hw, score_thresh, cap, 0, cand_boxes,
-                                nms_boxes, nms_scores, raw_scores, cand_flat, cat_ids, n_cand, row_map, stream);
+                              const float* image_hw, float score_thresh, int cap, int flags, float* cand_boxes,
+                              float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cand_flat, int64_t* cat_ids,
+                              int64_t* n_cand, int64_t* row_map, void* stream) {
+  const bool rot = (flags & D2B_SELECT_ROTATED) != 0;
+  if (bad_flags(flags, D2B_SELECT_ROTATED | D2B_SELECT_SEG_PER_IMAGE) || N < 0 || N > D2B_MAX_IMAGES || num_classes <= 0 ||
+      (kreg != 1 && kreg != num_classes) || cap < 0 || !row_start)
+    return D2B_EINVAL;
+  if (N == 0) return D2B_OK;
+  FrcnnImages I = {};
+  I.N = N;
+  for (int i = 0; i <= N; ++i) {
+    I.row_start[i] = row_start[i];
+    if (i ? row_start[i] < row_start[i - 1] : row_start[0] < 0) return D2B_EINVAL;  // a row before boxes[0]
+  }
+  if (!image_hw || !n_cand) return D2B_EINVAL;
+  if (row_start[N] > row_start[0] && (!boxes || !scores || !row_map)) return D2B_EINVAL;
+  if (cap > 0 && (!cand_boxes || !nms_boxes || !nms_scores || !raw_scores || !cand_flat || !cat_ids)) return D2B_EINVAL;
+  if (!rot && (misaligned16(cand_boxes) || misaligned16(nms_boxes))) return D2B_EINVAL;
+  const auto kernel = rot ? frcnn_prepare_kernel<RotBox> : frcnn_prepare_kernel<XyxyBox>;
+  kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(I, boxes, scores, num_classes, kreg, image_hw, score_thresh, cap,
+                                                   (flags & D2B_SELECT_SEG_PER_IMAGE) ? 1 : 0, cand_boxes, nms_boxes,
+                                                   nms_scores, raw_scores, (long long*)cand_flat, (long long*)cat_ids,
+                                                   (long long*)n_cand, (long long*)row_map);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
 }
 
-D2B_API int d2b_frcnn_rotated_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes,
-                                      int kreg, const float* image_hw, float score_thresh, int cap, int seg_per_image,
-                                      float* cand_boxes, float* nms_boxes, float* nms_scores, float* raw_scores,
-                                      int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand, int64_t* row_map, void* stream) {
-  return frcnn_prepare<RotBox>(boxes, scores, row_start, N, num_classes, kreg, image_hw, score_thresh, cap, seg_per_image,
-                               cand_boxes, nms_boxes, nms_scores, raw_scores, cand_flat, cat_ids, n_cand, row_map, stream);
-}
-
-D2B_API int d2b_rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int use_offsets,
-                            float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
-                            int* nonfinite, void* stream) {
-  return rpn_prepare<XyxyBox>(lv, N, image_hw, min_box_size, use_offsets, 0, flat_boxes, nms_boxes, nms_scores, raw_scores,
-                              cat_ids, nonfinite, stream);
-}
-
-D2B_API int d2b_rrpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int seg_per_image,
-                             float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
-                             int* nonfinite, void* stream) {
-  return rpn_prepare<RotBox>(lv, N, image_hw, min_box_size, 1, seg_per_image, flat_boxes, nms_boxes, nms_scores, raw_scores,
-                             cat_ids, nonfinite, stream);
-}
-
-namespace {
-
-template <bool kLinear>
-int dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
-                  float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
-                  int64_t* cat_ids, void* stream) {
-  if (!lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0 || num_classes <= 0 || !weights) return D2B_EINVAL;
+D2B_API int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
+                              int flags, float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores,
+                              int64_t* classes, int64_t* cat_ids, void* stream) {
+  const bool linear = (flags & D2B_SELECT_LINEAR) != 0;
+  if (bad_flags(flags, D2B_SELECT_LINEAR) || !lv || lv->num_levels < 1 || lv->num_levels > D2B_MAX_LEVELS || N < 0 ||
+      num_classes <= 0 || (!weights && !linear))
+    return D2B_EINVAL;
   if (N == 0) return D2B_OK;
   DenseLevels P = {};
   P.L = lv->num_levels;
-  int T = 0;
+  long long T = 0;
   for (int l = 0; l < P.L; ++l) {
     if (lv->R[l] < 0 || lv->k[l] < 0) return D2B_EINVAL;
     if (lv->k[l] > 0 && (!lv->anchors[l] || !lv->deltas[l] || !lv->topk_idx[l] || !lv->topk_scores[l])) return D2B_EINVAL;
-    if ((reinterpret_cast<uintptr_t>(lv->anchors[l]) & 15) != 0 || (reinterpret_cast<uintptr_t>(lv->deltas[l]) & 15) != 0)
-      return D2B_EINVAL;
+    if (misaligned16(lv->anchors[l]) || misaligned16(lv->deltas[l])) return D2B_EINVAL;
     P.anchors[l] = lv->anchors[l];
     P.deltas[l] = lv->deltas[l];
     P.topk_idx[l] = lv->topk_idx[l];
     P.topk_scores[l] = lv->topk_scores[l];
     P.R[l] = lv->R[l];
     P.k[l] = lv->k[l];
-    P.t0[l] = T;
+    P.t0[l] = (int)T;
     T += lv->k[l];
   }
-  P.t0[P.L] = T;
+  if (T > INT_MAX) return D2B_EINVAL;
+  P.t0[P.L] = (int)T;
   if (T == 0) return D2B_OK;
   if (!flat_boxes || !nms_boxes || !nms_scores || !raw_scores || !classes || !cat_ids) return D2B_EINVAL;
-  dense_prepare_kernel<kLinear><<<N, kThreads, 0, (cudaStream_t)stream>>>(P, T, num_classes, weights[0], weights[1],
-                                                                          weights[2], weights[3], scale_clamp, flat_boxes,
-                                                                          nms_boxes, nms_scores, raw_scores,
-                                                                          (long long*)classes, (long long*)cat_ids);
+  if (misaligned16(flat_boxes) || misaligned16(nms_boxes)) return D2B_EINVAL;
+  const float unused[4] = {1.f, 1.f, 1.f, 1.f};
+  const float* w = linear ? unused : weights;
+  const auto kernel = linear ? dense_prepare_kernel<true> : dense_prepare_kernel<false>;
+  kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(P, (int)T, num_classes, w[0], w[1], w[2], w[3], scale_clamp, flat_boxes,
+                                                   nms_boxes, nms_scores, raw_scores, (long long*)classes,
+                                                   (long long*)cat_ids);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
-}
-
-}  // namespace
-
-D2B_API int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
-                              float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
-                              int64_t* cat_ids, void* stream) {
-  return dense_prepare<false>(lv, N, num_classes, weights, scale_clamp, flat_boxes, nms_boxes, nms_scores, raw_scores,
-                              classes, cat_ids, stream);
-}
-
-D2B_API int d2b_dense_prepare_linear(const d2b_dense_levels* lv, int N, int num_classes, float* flat_boxes,
-                                     float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
-                                     int64_t* cat_ids, void* stream) {
-  const float unused[4] = {1.f, 1.f, 1.f, 1.f};
-  return dense_prepare<true>(lv, N, num_classes, unused, 0.f, flat_boxes, nms_boxes, nms_scores, raw_scores, classes,
-                             cat_ids, stream);
 }
 
 // ================================================================================================ mask targets + loss

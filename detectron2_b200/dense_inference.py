@@ -96,7 +96,7 @@ def dense_detector_inference_fixed(anchors: List[torch.Tensor], pred_scores: Lis
     (library), then d2b_dense_prepare (decode + class ids + NMS offsets of ALL levels and images), memset + 3 NMS kernels,
     d2b_rpn_select, one gather.  Static shapes: capturable in a CUDA graph.
     transform: "delta" decodes with Box2BoxTransform(box2box_weights, scale_clamp) (RetinaNet), "linear" with
-    Box2BoxTransformLinear(normalize_by_size=True) (FCOS; weights and scale_clamp unused)."""
+    Box2BoxTransformLinear(normalize_by_size=True) (FCOS, D2B_SELECT_LINEAR; weights and scale_clamp unused)."""
     import ctypes as C
 
     from . import _C
@@ -134,15 +134,11 @@ def dense_detector_inference_fixed(anchors: List[torch.Tensor], pred_scores: Lis
     classes, cat_ids = torch.empty((m,), **i64), torch.empty((m,), **i64)
     _check_transform(transform)
     w = (C.c_float * 4)(*[float(x) for x in box2box_weights])
+    flags = _C.SELECT_LINEAR if transform == "linear" else 0
     with torch.cuda.device(device):
-        if transform == "linear":
-            check(_C.lib().d2b_dense_prepare_linear(C.byref(lv), n, ncls, ptr(flat_boxes), ptr(nms_boxes), ptr(nms_scores),
-                                                    ptr(raw_scores), ptr(classes), ptr(cat_ids), stream_ptr(device)),
-                  "dense_prepare_linear")
-        else:
-            check(_C.lib().d2b_dense_prepare(C.byref(lv), n, ncls, w, float(scale_clamp), ptr(flat_boxes), ptr(nms_boxes),
-                                             ptr(nms_scores), ptr(raw_scores), ptr(classes), ptr(cat_ids),
-                                             stream_ptr(device)), "dense_prepare")
+        check(_C.lib().d2b_dense_prepare(C.byref(lv), n, ncls, w, float(scale_clamp), flags, ptr(flat_boxes), ptr(nms_boxes),
+                                         ptr(nms_scores), ptr(raw_scores), ptr(classes), ptr(cat_ids), stream_ptr(device)),
+              "dense_prepare")
     out_boxes, out_scores, out_index, counts = nms_select(nms_boxes, nms_scores, cat_ids, flat_boxes, raw_scores, n, t, topk,
                                                           nms_thresh, False, max(t, 1))
     out_classes = classes[out_index.reshape(-1)].reshape(n, topk) if m else out_index

@@ -17,10 +17,10 @@ Launch sequence for the whole batch: prepare, memset + 3 NMS kernels, select, tw
 same selection written with torch ops (`_fast_rcnn_inference_host`, the host-logic restatement pinned by the CPU tests).
 
 With `rotated=True` the same functions are rotated Fast R-CNN inference (detectron2/modeling/roi_heads/rotated_fast_rcnn.py:
-46-132, whose public names live in `rotated_fast_rcnn.py`): 5-wide boxes, `d2b_frcnn_rotated_prepare` (RotatedBoxes.clip and
-batched_nms_rotated's offsets class * (max - min + 1) on the centres), `D2B_NMS_ROTATED`, `d2b_rpn_select_rotated`, and for a
-threshold <= 0, which IoU 0 passes, one NMS segment per image (the reference's one NMS per image then suppresses across
-classes too).
+46-132, whose public names live in `rotated_fast_rcnn.py`): 5-wide boxes, `D2B_SELECT_ROTATED` for `d2b_frcnn_prepare`
+(RotatedBoxes.clip and batched_nms_rotated's offsets class * (max - min + 1) on the centres) and `d2b_rpn_select`,
+`D2B_NMS_ROTATED`, and for a threshold <= 0, which IoU 0 passes, `D2B_SELECT_SEG_PER_IMAGE`: one NMS segment per image (the
+reference's one NMS per image then suppresses across classes too).
 """
 from typing import List, Tuple
 
@@ -57,49 +57,35 @@ def _clip(boxes: torch.Tensor, h: float, w: float) -> torch.Tensor:  # Boxes.cli
     return torch.stack([x1, y1, x2, y2], dim=1)
 
 
-def _single_image_exact(boxes, scores, image_shape, score_thresh, nms_thresh, topk_per_image):
-    """Reference structure (fast_rcnn.py:117-173) on top of our NMS; data-dependent shapes, hence host syncs.
-    Used only for images whose candidate count exceeds CANDIDATE_CAP."""
+def _single_image_exact(boxes, scores, image_shape, score_thresh, nms_thresh, topk_per_image, rotated=False):
+    """Reference structure (fast_rcnn.py:117-173, rotated_fast_rcnn.py:98-132) on top of our NMS; data-dependent shapes,
+    hence host syncs.  Used only for images whose candidate count exceeds the candidate slots."""
     valid = torch.isfinite(boxes).all(dim=1) & torch.isfinite(scores).all(dim=1)
     if not bool(valid.all()):
         boxes, scores = boxes[valid], scores[valid]
     scores = scores[:, :-1]
-    k = boxes.shape[1] // 4
-    boxes = _clip(boxes, float(image_shape[0]), float(image_shape[1])).view(-1, k, 4)
+    d = 5 if rotated else 4
+    k = boxes.shape[1] // d
+    h, w = float(image_shape[0]), float(image_shape[1])
+    boxes = (clip_rotated(boxes.reshape(-1, 5).float(), h, w) if rotated else _clip(boxes, h, w)).view(-1, k, d)
     filter_mask = scores > score_thresh
     filter_inds = filter_mask.nonzero()
     boxes = boxes[filter_inds[:, 0], 0] if k == 1 else boxes[filter_mask]
     scores = scores[filter_mask]
-    from .layers import batched_nms
-
-    keep = batched_nms(boxes, scores, filter_inds[:, 1], nms_thresh)
-    if topk_per_image >= 0:
-        keep = keep[:topk_per_image]
-    return Detections(image_shape, boxes[keep], scores[keep], filter_inds[keep, 1]), filter_inds[keep, 0]
-
-
-def _single_image_exact_rotated(boxes, scores, image_shape, score_thresh, nms_thresh, topk_per_image):
-    """Reference structure (rotated_fast_rcnn.py:98-132) on top of our NMS; data-dependent shapes, hence host syncs.
-    Used only for images whose candidate count exceeds the candidate slots."""
-    valid = torch.isfinite(boxes).all(dim=1) & torch.isfinite(scores).all(dim=1)
-    if not bool(valid.all()):
-        boxes, scores = boxes[valid], scores[valid]
-    scores = scores[:, :-1]
-    k = boxes.shape[1] // 5
-    boxes = clip_rotated(boxes.reshape(-1, 5).float(), float(image_shape[0]), float(image_shape[1])).view(-1, k, 5)
-    filter_mask = scores > score_thresh
-    filter_inds = filter_mask.nonzero()
-    boxes = boxes[filter_inds[:, 0], 0] if k == 1 else boxes[filter_mask]
-    scores = scores[filter_mask]
-    # batched_nms_rotated with the offsets applied here, as the batched path does: one segment per class, or one for the
-    # whole image when IoU 0 passes the threshold
     cls = filter_inds[:, 1]
-    live = torch.ones_like(scores, dtype=torch.bool)
-    off = cls.to(torch.float32) * rotated_offset_scale(boxes[None], live[None])[0]
-    nms_boxes = torch.cat([boxes[:, :2] + off[:, None], boxes[:, 2:]], dim=1)
-    seg = torch.zeros_like(cls) if float(nms_thresh) <= 0.0 else cls
-    keep, num_keep = ops.nms_fixed(nms_boxes, scores, seg, float(nms_thresh), True, apply_offsets=False)
-    keep = keep[: int(num_keep.item())]
+    if rotated:
+        # batched_nms_rotated with the offsets applied here, as the batched path does: one segment per class, or one for
+        # the whole image when IoU 0 passes the threshold
+        live = torch.ones_like(scores, dtype=torch.bool)
+        off = cls.to(torch.float32) * rotated_offset_scale(boxes[None], live[None])[0]
+        nms_boxes = torch.cat([boxes[:, :2] + off[:, None], boxes[:, 2:]], dim=1)
+        seg = torch.zeros_like(cls) if float(nms_thresh) <= 0.0 else cls
+        keep, num_keep = ops.nms_fixed(nms_boxes, scores, seg, float(nms_thresh), True, apply_offsets=False)
+        keep = keep[: int(num_keep.item())]
+    else:
+        from .layers import batched_nms
+
+        keep = batched_nms(boxes, scores, cls, nms_thresh)
     if topk_per_image >= 0:
         keep = keep[:topk_per_image]
     return Detections(image_shape, boxes[keep], scores[keep], filter_inds[keep, 1]), filter_inds[keep, 0]
@@ -143,14 +129,11 @@ def fast_rcnn_inference_fixed(boxes: List[torch.Tensor], scores: List[torch.Tens
     row_map = torch.empty((starts[-1],), **i64)
     rs = (C.c_int * (n + 1))(*starts)
     per_image = rotated and float(nms_thresh) <= 0.0
-    head = (ptr(all_b), ptr(all_s), rs, n, ncls, kreg, ptr(hw), float(score_thresh), cap)
-    tail = (ptr(cand_boxes), ptr(nms_boxes), ptr(nms_scores), ptr(raw_scores), ptr(cand_flat), ptr(cat_ids), ptr(n_cand),
-            ptr(row_map), stream_ptr(device))
+    flags = (_C.SELECT_ROTATED if rotated else 0) | (_C.SELECT_SEG_PER_IMAGE if per_image else 0)
     with torch.cuda.device(device):
-        if rotated:
-            check(_C.lib().d2b_frcnn_rotated_prepare(*head, int(per_image), *tail), "frcnn_rotated_prepare")
-        else:
-            check(_C.lib().d2b_frcnn_prepare(*head, *tail), "frcnn_prepare")
+        check(_C.lib().d2b_frcnn_prepare(ptr(all_b), ptr(all_s), rs, n, ncls, kreg, ptr(hw), float(score_thresh), cap, flags,
+                                         ptr(cand_boxes), ptr(nms_boxes), ptr(nms_scores), ptr(raw_scores), ptr(cand_flat),
+                                         ptr(cat_ids), ptr(n_cand), ptr(row_map), stream_ptr(device)), "frcnn_prepare")
     # an (image, class) category holds at most one candidate per proposal row; an image segment at most `cap`
     max_segment = cap if per_image else max(min(cap, max(rcounts + [0])), 1)
     out_boxes, out_scores, out_index, counts = nms_select(nms_boxes, nms_scores, cat_ids, cand_boxes, raw_scores, n, cap,
@@ -176,7 +159,6 @@ def fast_rcnn_inference(boxes: List[torch.Tensor], scores: List[torch.Tensor], i
                                          rotated=rotated)
     from . import _C
 
-    exact = _single_image_exact_rotated if rotated else _single_image_exact
     results, kept_rows = [], []
     for i0 in range(0, len(boxes), _C.MAX_IMAGES):  # chunks of the ABI's image bound
         sl = slice(i0, i0 + _C.MAX_IMAGES)
@@ -187,7 +169,8 @@ def fast_rcnn_inference(boxes: List[torch.Tensor], scores: List[torch.Tensor], i
         for j, (c, n_cand) in enumerate(stats):
             i = i0 + j
             if n_cand > out["cap"]:  # candidate list was truncated: redo this image exactly (rare)
-                det, rows_i = exact(boxes[i], scores[i], image_shapes[i], score_thresh, nms_thresh, topk_per_image)
+                det, rows_i = _single_image_exact(boxes[i], scores[i], image_shapes[i], score_thresh, nms_thresh,
+                                                  topk_per_image, rotated)
             else:
                 det = Detections(image_shapes[i], out["boxes"][j, :c], out["scores"][j, :c].to(dt), out["classes"][j, :c])
                 rows_i = out["rows"][j, :c]
@@ -262,12 +245,12 @@ def _fast_rcnn_inference_host(boxes: List[torch.Tensor], scores: List[torch.Tens
 
     stats = torch.stack([counts, torch.stack(n_cand_l).to(counts.dtype)], dim=1).tolist()  # the one host sync
     flat_all = torch.cat(cand_flat, dim=0)
-    exact = _single_image_exact_rotated if rotated else _single_image_exact
     results, kept_rows = [], []
     for i in range(num_images):
         c, n_cand = stats[i]
         if n_cand > caps[i]:  # candidate list was truncated: redo this image exactly (rare)
-            det, rows_i = exact(boxes[i], scores[i], image_shapes[i], score_thresh, nms_thresh, topk_per_image)
+            det, rows_i = _single_image_exact(boxes[i], scores[i], image_shapes[i], score_thresh, nms_thresh, topk_per_image,
+                                              rotated)
             results.append(det)
             kept_rows.append(rows_i)
             continue

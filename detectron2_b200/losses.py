@@ -196,7 +196,7 @@ def fcos_loss_op(logits: List[Tensor], deltas: List[Tensor], ctr: List[Tensor], 
     status = torch.empty((), dtype=torch.int32, device=dev)
     lib = _C.lib()
     code = _C.DTYPE_CODE[dt]
-    ws_bytes = int(lib.d2b_fcos_loss_workspace_bytes(C.byref(lv), n, num_classes, code))
+    ws_bytes = int(lib.d2b_dense_loss_workspace_bytes(C.byref(lv), n, num_classes, code))
     ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
         check(lib.d2b_fcos_loss_forward(C.byref(lv), _ptr_array(cs), n, num_classes, code, ptr(an), ptr(gt), ptr(lab),

@@ -54,8 +54,8 @@ def find_top_rpn_proposals_fixed(proposals: List[torch.Tensor], pred_objectness_
     """Sync-free, fixed-capacity form (CUDA tensors only): returns (boxes [N, post_nms_topk, 4], or 5 with `rotated`,
     objectness logits [N, post_nms_topk], counts [N] int64, nonfinite [1] int32) -- rows beyond counts[i] are zero.
     `image_sizes` is a list of (h, w) or an [N, 2] CUDA tensor (needed inside a CUDA-graph capture).  The launch sequence
-    (torch.topk per level, d2b_[r]rpn_prepare, d2b_nms, d2b_rpn_select[_rotated]) has static shapes: it can be captured
-    in a CUDA graph."""
+    (torch.topk per level, d2b_rpn_prepare, d2b_nms, d2b_rpn_select; D2B_SELECT_ROTATED with `rotated`) has static shapes:
+    it can be captured in a CUDA graph."""
     import ctypes as C
 
     from . import _C
@@ -74,13 +74,13 @@ def find_top_rpn_proposals_fixed(proposals: List[torch.Tensor], pred_objectness_
     nonfinite = torch.empty((1,), dtype=torch.int32, device=device)
     # IoU 0 passes a rotated threshold <= 0: the reference's one NMS per image then suppresses across levels as well
     per_image = rotated and float(nms_thresh) <= 0.0
-    if rotated:
-        prepare, flag = _C.lib().d2b_rrpn_prepare, int(per_image)
-    else:  # torchvision's batched_nms applies the coordinate trick per image only up to 100 000 coordinates (25 000 boxes)
-        prepare, flag = _C.lib().d2b_rpn_prepare, int(t * 4 <= 100_000)
+    flags = (_C.SELECT_ROTATED if rotated else 0) | (_C.SELECT_SEG_PER_IMAGE if per_image else 0)
+    if not rotated and t * 4 > 100_000:  # torchvision's batched_nms offsets at most 100 000 coordinates (25 000 boxes)
+        flags |= _C.SELECT_NO_OFFSETS
     with torch.cuda.device(device):
-        check(prepare(C.byref(lv), n, ptr(hw), float(min_box_size), flag, ptr(flat_boxes), ptr(nms_boxes), ptr(nms_scores),
-                      ptr(raw_scores), ptr(cat_ids), ptr(nonfinite), stream_ptr(device)), "rpn_prepare")
+        check(_C.lib().d2b_rpn_prepare(C.byref(lv), n, ptr(hw), float(min_box_size), flags, ptr(flat_boxes), ptr(nms_boxes),
+                                       ptr(nms_scores), ptr(raw_scores), ptr(cat_ids), ptr(nonfinite), stream_ptr(device)),
+              "rpn_prepare")
     out_boxes, out_scores, _, counts = nms_select(nms_boxes, nms_scores, cat_ids, flat_boxes, raw_scores, n, t,
                                                   int(post_nms_topk), nms_thresh, rotated, t if per_image else max(ks))
     del keepalive

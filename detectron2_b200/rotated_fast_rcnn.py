@@ -7,11 +7,12 @@ sync), `nonzero()` on the R x K score matrix (another sync), one `batched_nms_ro
 batch goes through ONE rotated NMS: the functions below are `fast_rcnn_inference.fast_rcnn_inference[_fixed]` with
 `rotated=True`:
 
-  * `d2b_frcnn_rotated_prepare` (one CTA per image) drops the non-finite rows, compacts the (row, class) pairs with
-    score > score_thresh IN ROW-MAJOR ORDER into `CAP` slots per image, normalises the angles and clips the boxes, and adds
-    batched_nms_rotated's offsets class * (max - min + 1) over the image's candidates to the centres;
+  * `d2b_frcnn_prepare` with `D2B_SELECT_ROTATED` (one CTA per image) drops the non-finite rows, compacts the (row, class)
+    pairs with score > score_thresh IN ROW-MAJOR ORDER into `CAP` slots per image, normalises the angles and clips the boxes,
+    and adds batched_nms_rotated's offsets class * (max - min + 1) over the image's candidates to the centres;
   * one `d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET)` with category image * (K + 1) + class, empty slots -1 (ignored);
-  * `d2b_rpn_select_rotated` hands every image the first `topk_per_image` entries of the score-ordered keep list.
+  * `d2b_rpn_select` with `D2B_SELECT_ROTATED` hands every image the first `topk_per_image` entries of the score-ordered
+    keep list.
 An image whose candidates overflow `fast_rcnn_inference.CANDIDATE_CAP` is recomputed with the exact (synchronising)
 candidate list.  CPU tensors take the same selection written with torch ops.
 """

@@ -6,12 +6,14 @@ boxes (`RotatedBoxes.clip`, whose `torch.where(...)[0]` is a host sync), drops e
 one `batched_nms_rotated`.  Here all images go through ONE rotated NMS: the functions below are
 `proposal_utils.find_top_rpn_proposals[_fixed]` with `rotated=True`:
 
-  * `d2b_rrpn_prepare` (one CTA per image) gathers the per-level top-k, normalises the angles and clips, and moves removed
-    boxes (non-finite, or not larger than `min_box_size` after clipping) to the ignored category -1 instead of removing them;
-    it adds batched_nms_rotated's offsets -- level * (max - min + 1) over THAT image's surviving boxes, fp32 -- to the centres;
+  * `d2b_rpn_prepare` with `D2B_SELECT_ROTATED` (one CTA per image) gathers the per-level top-k, normalises the angles and
+    clips, and moves removed boxes (non-finite, or not larger than `min_box_size` after clipping) to the ignored category -1
+    instead of removing them; it adds batched_nms_rotated's offsets -- level * (max - min + 1) over THAT image's surviving
+    boxes, fp32 -- to the centres;
   * one `d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET)` with category image * L + level (image alone for a threshold <= 0,
-    which IoU 0 passes: the reference's one NMS per image then suppresses across levels too);
-  * `d2b_rpn_select_rotated` hands every image the first `post_nms_topk` survivors of the score-ordered keep list.
+    which IoU 0 passes: the reference's one NMS per image then suppresses across levels too; `D2B_SELECT_SEG_PER_IMAGE`);
+  * `d2b_rpn_select` with `D2B_SELECT_ROTATED` hands every image the first `post_nms_topk` survivors of the score-ordered
+    keep list.
 The only host synchronisation is the final read of the N output lengths.  `clip_rotated` and `rotated_offset_scale` are
 the torch-op forms of the clip and the offsets that the host restatements use.
 """
@@ -54,8 +56,8 @@ def find_top_rrpn_proposals_fixed(proposals: List[torch.Tensor], pred_objectness
                                   min_box_size: float):
     """Sync-free, fixed-capacity form (CUDA tensors only): returns (boxes [N, post_nms_topk, 5], objectness logits
     [N, post_nms_topk], counts [N] int64, nonfinite [1] int32) -- rows beyond counts[i] are zero.  `image_sizes` is a list
-    of (h, w) or an [N, 2] CUDA tensor.  The launch sequence (torch.topk per level, d2b_rrpn_prepare, d2b_nms,
-    d2b_rpn_select_rotated) has static shapes: it can be captured in a CUDA graph."""
+    of (h, w) or an [N, 2] CUDA tensor.  The launch sequence (torch.topk per level, d2b_rpn_prepare, d2b_nms, d2b_rpn_select,
+    with D2B_SELECT_ROTATED) has static shapes: it can be captured in a CUDA graph."""
     return find_top_rpn_proposals_fixed(proposals, pred_objectness_logits, image_sizes, nms_thresh, pre_nms_topk,
                                         post_nms_topk, min_box_size, rotated=True)
 

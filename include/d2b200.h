@@ -31,7 +31,7 @@ extern "C" {
 #define D2B_EWORKSPACE (-2)  /* workspace too small */
 #define D2B_EUNSUPPORTED (-3)
 
-#define D2B_ABI_VERSION 5
+#define D2B_ABI_VERSION 6
 int d2b_abi_version(void);
 /* compile-time facts, replaces detectron2._C.get_cuda_version / has_cuda (csrc/vision.cpp:23-49,86-88) */
 int d2b_cuda_version(void);
@@ -151,22 +151,80 @@ int d2b_nms(const float* boxes, const float* scores, const int64_t* idxs, int64_
             double iou_threshold, int flags, int64_t max_segment, int64_t* keep, int64_t* num_keep,
             void* workspace, size_t workspace_bytes, void* stream);
 
-/* ---- Batched RPN proposal selection around the NMS (SURVEY 8f-2) ----------------------------------------
- * Replaces the per-image Python loop of detectron2/modeling/proposal_generator/proposal_utils.py:96-133 (boolean filtering,
- * `.item()` sync, per-image batched_nms, slicing) by a fixed-capacity launch sequence for ALL images:
- *   torch.topk per level (library)  ->  d2b_rpn_prepare  ->  d2b_nms(category = image*L + level, D2B_NMS_NO_OFFSET,
- *   max_segment = pre_nms_topk)  ->  d2b_rpn_select.
- * d2b_rpn_prepare: lv->proposals[l] [N,A_l,4] decoded boxes, lv->topk_idx[l] / topk_scores[l] [N,k_l] (the per-level top-k of
+/* ---- Inference candidate selection around the NMS (SURVEY 8f-2) -------------------------------------------------------
+ * Replaces the per-image Python loops of detectron2/modeling/proposal_generator/proposal_utils.py:96-133 and rrpn.py:20-127
+ * (find_top_rpn_proposals / find_top_rrpn_proposals: boolean filtering, `.item()` sync, per-image batched_nms, slicing),
+ * of modeling/roi_heads/fast_rcnn.py:46-173 and rotated_fast_rcnn.py:46-132 (fast_rcnn_inference[_rotated]: boolean
+ * filtering, `nonzero()` sync, per-image batched_nms, slicing) and of meta_arch/dense_detector.py:186-258 +
+ * meta_arch/retinanet.py:256-308 / fcos.py:253-301 (per-level filter / top-k / apply_deltas, per-image batched_nms) by a
+ * fixed-capacity launch sequence for ALL images:
+ *   d2b_rpn_prepare | d2b_frcnn_prepare | (torch.topk per level ->) d2b_dense_prepare  ->  d2b_nms(D2B_NMS_NO_OFFSET, and
+ *   D2B_NMS_ROTATED for rotated boxes; category = image*L + level | image*(K+1) + class, -1 = removed; max_segment =
+ *   pre_nms_topk for the RPN)  ->  d2b_rpn_select (the same per-image first-topk selection for all three).
+ * flags, one namespace for the four entry points:
+ *   D2B_SELECT_ROTATED (rpn, frcnn, select): boxes are (cx, cy, w, h, angle_deg), D = 5 floats per box, no alignment
+ *     requirement.  The prepares apply RotatedBoxes.clip(image, clip_angle_threshold = 1) -- every angle normalised to
+ *     (a + 180) % 360 - 180 (torch's float remainder), boxes with |angle| <= 1 clipped as xyxy boxes -- and
+ *     batched_nms_rotated's per-image offsets category * (max - min + 1) on the centre (layers/nms.py:137-146).  Without it
+ *     boxes are xyxy, D = 4, and the box arrays must be 16-byte aligned (float4 access); the offsets are torchvision's
+ *     category * (max coordinate + 1).  Offsets are computed over the image's surviving boxes, in fp32.
+ *   D2B_SELECT_SEG_PER_IMAGE (rpn, frcnn; with ROTATED only): every surviving candidate of image n gets NMS category n,
+ *     offsets unchanged.  Pass it for iou_threshold <= 0, which IoU 0 passes (the reference's single NMS then suppresses
+ *     across categories too); the NMS max_segment must then bound the image's slot count.
+ *   D2B_SELECT_NO_OFFSETS (rpn, without ROTATED only): nms_boxes are not shifted, as torchvision's batched_nms past 25 000
+ *     boxes per image.  The rotated offsets are always applied.
+ *   D2B_SELECT_LINEAR (dense only): the Box2BoxTransformLinear.apply_deltas decode of FCOS (box_regression.py:275-307,
+ *     normalize_by_size): relu(deltas) times the anchor's (width, height), then the centre minus (l, t), plus (r, b);
+ *     weights and scale_clamp are unused and weights may be NULL.
+ * d2b_rpn_prepare: lv->proposals[l] [N,A_l,D] decoded boxes, lv->topk_idx[l] / topk_scores[l] [N,k_l] (the per-level top-k of
  *   the objectness logits), image_hw [N,2] (h, w) on the device.  T = sum_l k_l candidates per image.  Writes, for all N*T
- *   candidates: flat_boxes (clipped to the image; zeros for removed ones), nms_boxes (+ torchvision's per-image
- *   level offsets when use_offsets), nms_scores (-inf for removed), raw_scores, cat_ids (image*L + level, or -1 = removed:
- *   non-finite or not larger than min_box_size after clipping), nonfinite[1] (1 if any candidate was non-finite).
- *   Arguments (the same rules for d2b_rrpn_prepare, checked before the first CUDA call): 1 <= num_levels <= D2B_MAX_LEVELS,
- *   N >= 0, nonfinite non-NULL; per level 0 <= k_l <= A_l, and the level's three pointers non-NULL when N > 0 and k_l > 0;
- *   T <= INT_MAX; image_hw and the five output arrays non-NULL when N > 0 and T > 0.  proposals[l], flat_boxes and
- *   nms_boxes must be 16-byte aligned (float4 access).  nonfinite is zeroed even when there is no candidate.
- * d2b_rpn_select: keep / num_keep as returned by d2b_nms over the N*T candidates; out_boxes [N,post_nms_topk,4],
- *   out_scores / out_index [N,post_nms_topk] (0-padded), counts [N] int64. */
+ *   candidates: flat_boxes [N*T,D] (clipped to the image; zeros for removed ones), nms_boxes [N*T,D] (+ the per-image level
+ *   offsets), nms_scores (-inf for removed), raw_scores, cat_ids (image*L + level, or -1 = removed: non-finite, or width or
+ *   height not larger than min_box_size after clipping), nonfinite[1] (1 if any candidate was non-finite).
+ * d2b_frcnn_prepare: boxes [Rtot, kreg*D] predicted boxes (kreg = 1 class-agnostic or K), scores [Rtot, K+1] (last column =
+ *   background) of N <= D2B_MAX_IMAGES images concatenated; row_start [N+1] HOST array of the images' first rows;
+ *   image_hw [N,2] on the device.  Per image the (row, class) pairs with score > score_thresh of the rows whose box and
+ *   score entries are all finite are written in row-major order into `cap` slots: cand_boxes [N*cap,D] (clipped), nms_boxes
+ *   (+ the class offsets), nms_scores (-inf in dead slots), raw_scores, cand_flat (row_in_image * K + class), cat_ids
+ *   (image*(K+1) + class, -1 = dead); n_cand [N] = the image's candidate count (larger than cap: the list was truncated and
+ *   the caller must redo that image); row_map [Rtot] = index of a row among its image's valid rows (-1 for dropped rows) --
+ *   what the reference returns as kept row indices.
+ * d2b_dense_prepare: per level l anchors [R_l,4], deltas [N,R_l,4], and the batched top-k of the thresholded scores
+ *   (topk_idx [N,k_l] = anchor*K + class, topk_scores [N,k_l] with -inf in dead slots); weights[4] (HOST) and scale_clamp of
+ *   Box2BoxTransform.  Writes for all N*T candidates (T = sum k_l): flat_boxes (decoded), nms_boxes (+ offsets while the
+ *   image has <= 25 000 live candidates, as torchvision), nms_scores, raw_scores, classes, cat_ids.  xyxy boxes only.
+ * d2b_rpn_select: keep / num_keep as returned by d2b_nms over the N*T candidates (T = cap after d2b_frcnn_prepare),
+ *   flat_boxes [N*T,D]; out_boxes [N,post_nms_topk,D], out_scores / out_index [N,post_nms_topk] (0-padded), counts [N] int64.
+ * Arguments are checked in this order, and nothing is launched or written before every check has passed:
+ *   all four:  1. D2B_EINVAL: a flag bit the entry point does not take, SEG_PER_IMAGE without ROTATED, NO_OFFSETS with it.
+ *   rpn_prepare:  2. D2B_EINVAL: lv or nonfinite NULL, num_levels outside 1..D2B_MAX_LEVELS, N < 0; per level A_l < 0,
+ *                    k_l < 0 or k_l > A_l, a level pointer NULL when N > 0 and k_l > 0, or (xyxy) proposals[l] not 16-byte
+ *                    aligned; T > INT_MAX; when N > 0 and T > 0, image_hw or an output NULL; (xyxy) flat_boxes or
+ *                    nms_boxes not 16-byte aligned.
+ *                 3. nonfinite is zeroed, even when there is no candidate; N == 0 or T == 0: D2B_OK.
+ *   frcnn_prepare: 2. D2B_EINVAL: N < 0 or N > D2B_MAX_IMAGES, num_classes < 1, kreg neither 1 nor num_classes, cap < 0,
+ *                    row_start NULL.
+ *                 3. N == 0: D2B_OK.
+ *                 4. D2B_EINVAL: row_start[0] < 0 or row_start decreasing; image_hw or n_cand NULL; when the images have
+ *                    rows, boxes, scores or row_map NULL; when cap > 0, an output NULL; (xyxy) cand_boxes or nms_boxes not
+ *                    16-byte aligned.
+ *   dense_prepare: 2. D2B_EINVAL: lv NULL, num_levels outside 1..D2B_MAX_LEVELS, N < 0, num_classes < 1, weights NULL
+ *                    without LINEAR.
+ *                 3. N == 0: D2B_OK.
+ *                 4. D2B_EINVAL: per level R_l < 0 or k_l < 0, a level pointer NULL when k_l > 0, or anchors[l] or
+ *                    deltas[l] not 16-byte aligned; T > INT_MAX.
+ *                 5. T == 0: D2B_OK.
+ *                 6. D2B_EINVAL: an output NULL, or flat_boxes or nms_boxes not 16-byte aligned.
+ *   rpn_select:    2. D2B_EINVAL: N, T or post_nms_topk below 0.
+ *                 3. N == 0: D2B_OK.
+ *                 4. D2B_EINVAL: counts NULL; when T > 0 and post_nms_topk > 0, another pointer NULL, or (xyxy)
+ *                    flat_boxes or out_boxes not 16-byte aligned.
+ *                 5. T == 0 or post_nms_topk == 0: counts zeroed, D2B_OK. */
+#define D2B_SELECT_ROTATED 1
+#define D2B_SELECT_SEG_PER_IMAGE 2
+#define D2B_SELECT_NO_OFFSETS 4
+#define D2B_SELECT_LINEAR 8
+#define D2B_MAX_IMAGES 64
 typedef struct {
   int num_levels;
   const float* proposals[D2B_MAX_LEVELS];
@@ -174,32 +232,6 @@ typedef struct {
   const float* topk_scores[D2B_MAX_LEVELS];
   int A[D2B_MAX_LEVELS], k[D2B_MAX_LEVELS];
 } d2b_rpn_levels;
-int d2b_rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int use_offsets,
-                    float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
-                    int* nonfinite, void* stream);
-int d2b_rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
-                   const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
-                   float* out_scores, int64_t* out_index, int64_t* counts, void* stream);
-
-/* ---- Fast R-CNN and dense-head (RetinaNet) inference candidates around the NMS (SURVEY 8f-2) -----------------
- * Replace the per-image Python loops of detectron2/modeling/roi_heads/fast_rcnn.py:46-173 (`fast_rcnn_inference`:
- * boolean filtering, `nonzero()` sync, per-image batched_nms, slicing) and of meta_arch/dense_detector.py:186-258 +
- * meta_arch/retinanet.py:256-308 (per-level filter / top-k / apply_deltas, per-image batched_nms) by
- *   d2b_frcnn_prepare | (torch.topk per level ->) d2b_dense_prepare  ->  d2b_nms(category = image*(K+1) + class,
- *   D2B_NMS_NO_OFFSET)  ->  d2b_rpn_select (the same per-image first-topk selection).
- * d2b_frcnn_prepare: boxes [Rtot, kreg*4] predicted boxes (kreg = 1 class-agnostic or K), scores [Rtot, K+1] (last column =
- *   background) of N <= D2B_MAX_IMAGES images concatenated; row_start [N+1] HOST array of the images' first rows;
- *   image_hw [N,2] on the device.  Per image the (row, class) pairs with score > score_thresh of the rows whose box and
- *   score entries are all finite are written in row-major order into `cap` slots: cand_boxes (clipped), nms_boxes
- *   (+ torchvision's class * (max coordinate + 1) offsets), nms_scores (-inf in dead slots), raw_scores, cand_flat
- *   (row_in_image * K + class), cat_ids (image*(K+1) + class, -1 = dead); n_cand [N] = the image's candidate count (larger
- *   than cap: the list was truncated and the caller must redo that image); row_map [Rtot] = index of a row among its image's
- *   valid rows (-1 for dropped rows) -- what the reference returns as kept row indices.
- * d2b_dense_prepare: per level l anchors [R_l,4], deltas [N,R_l,4], and the batched top-k of the thresholded scores
- *   (topk_idx [N,k_l] = anchor*K + class, topk_scores [N,k_l] with -inf in dead slots); weights[4] (HOST) and scale_clamp of
- *   Box2BoxTransform.  Writes for all N*T candidates (T = sum k_l): flat_boxes (decoded), nms_boxes (+ offsets while the
- *   image has <= 25 000 live candidates, as torchvision), nms_scores, raw_scores, classes, cat_ids. */
-#define D2B_MAX_IMAGES 64
 typedef struct {
   int num_levels;
   const float* anchors[D2B_MAX_LEVELS];
@@ -208,47 +240,18 @@ typedef struct {
   const float* topk_scores[D2B_MAX_LEVELS];
   int R[D2B_MAX_LEVELS], k[D2B_MAX_LEVELS];
 } d2b_dense_levels;
+int d2b_rpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int flags, float* flat_boxes,
+                    float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids, int* nonfinite, void* stream);
 int d2b_frcnn_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes, int kreg,
-                      const float* image_hw, float score_thresh, int cap, float* cand_boxes, float* nms_boxes,
+                      const float* image_hw, float score_thresh, int cap, int flags, float* cand_boxes, float* nms_boxes,
                       float* nms_scores, float* raw_scores, int64_t* cand_flat, int64_t* cat_ids, int64_t* n_cand,
                       int64_t* row_map, void* stream);
-int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp,
+int d2b_dense_prepare(const d2b_dense_levels* lv, int N, int num_classes, const float* weights, float scale_clamp, int flags,
                       float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* classes,
                       int64_t* cat_ids, void* stream);
-/* d2b_dense_prepare_linear: d2b_dense_prepare for FCOS (meta_arch/fcos.py:253-301), the same arguments without weights and
- *   scale_clamp: the boxes are decoded by Box2BoxTransformLinear.apply_deltas (box_regression.py:275-307,
- *   normalize_by_size): relu(deltas) times the anchor's (width, height), then the centre minus (l, t), plus (r, b). */
-int d2b_dense_prepare_linear(const d2b_dense_levels* lv, int N, int num_classes, float* flat_boxes, float* nms_boxes,
-                             float* nms_scores, float* raw_scores, int64_t* classes, int64_t* cat_ids, void* stream);
-
-/* ---- Rotated RRPN proposal selection and rotated Fast R-CNN inference around the NMS -----------------------------
- * Replace the per-image Python loops of detectron2/modeling/proposal_generator/rrpn.py:20-127 (find_top_rrpn_proposals)
- * and modeling/roi_heads/rotated_fast_rcnn.py:46-132 (fast_rcnn_inference_rotated) by
- *   d2b_rrpn_prepare | d2b_frcnn_rotated_prepare  ->  d2b_nms(D2B_NMS_ROTATED | D2B_NMS_NO_OFFSET, category =
- *   image*L + level | image*(K+1) + class, -1 = removed)  ->  d2b_rpn_select_rotated.
- * Boxes are (cx, cy, w, h, angle_deg) fp32, 5 floats per box, no alignment requirement.  Both prepares apply
- * RotatedBoxes.clip(image, clip_angle_threshold = 1): every angle is normalised to (a + 180) % 360 - 180 (torch's float
- * remainder), boxes with |angle| <= 1 are clipped as xyxy boxes; and batched_nms_rotated's per-image offsets
- * category * (max - min + 1) on the centre (layers/nms.py:137-146), over the image's surviving boxes.
- * seg_per_image != 0 (pass it for iou_threshold <= 0, which IoU 0 passes: the reference's single NMS then suppresses
- * across categories too): every surviving candidate of image n gets category n instead, offsets unchanged; the NMS
- * max_segment must then bound the image's slot count.
- * d2b_rrpn_prepare: as d2b_rpn_prepare (same argument rules, no alignment requirement) with lv->proposals[l] [N,A_l,5];
- *   removed = non-finite or w / h not larger than min_box_size after clipping (RotatedBoxes.nonempty); flat_boxes /
- *   nms_boxes [N*T,5]; the offsets are always applied.
- * d2b_frcnn_rotated_prepare: as d2b_frcnn_prepare with boxes [Rtot, kreg*5]; cand_boxes / nms_boxes [N*cap,5].
- * d2b_rpn_select_rotated: as d2b_rpn_select with flat_boxes [N*T,5] and out_boxes [N,post_nms_topk,5].
- * All arguments are checked before the first CUDA call. */
-int d2b_rrpn_prepare(const d2b_rpn_levels* lv, int N, const float* image_hw, float min_box_size, int seg_per_image,
-                     float* flat_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cat_ids,
-                     int* nonfinite, void* stream);
-int d2b_frcnn_rotated_prepare(const float* boxes, const float* scores, const int* row_start, int N, int num_classes,
-                              int kreg, const float* image_hw, float score_thresh, int cap, int seg_per_image,
-                              float* cand_boxes, float* nms_boxes, float* nms_scores, float* raw_scores, int64_t* cand_flat,
-                              int64_t* cat_ids, int64_t* n_cand, int64_t* row_map, void* stream);
-int d2b_rpn_select_rotated(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk,
-                           const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
-                           float* out_scores, int64_t* out_index, int64_t* counts, void* stream);
+int d2b_rpn_select(const int64_t* keep, const int64_t* num_keep, int N, int T, int post_nms_topk, int flags,
+                   const float* flat_boxes, const float* raw_scores, const int64_t* cat_ids, float* out_boxes,
+                   float* out_scores, int64_t* out_index, int64_t* counts, void* stream);
 
 /* ---- Anchor / proposal matching for the training targets -------------------------------------------------------
  * Replaces the per-image pairwise_iou + Matcher loops of RPN / RRPN.label_and_sample_anchors, RetinaNet.label_anchors,
@@ -446,10 +449,9 @@ int d2b_dense_loss_backward(const d2b_dense_loss_levels* lv, int N, int K, int b
  *   ctr_sum = binary_cross_entropy_with_logits of ctr[l] [N,R_l] (`dtype`, read in place) over the positive rows against
  *   sqrt((min(l,r) / max(l,r)) * (min(t,b) / max(t,b))), (l,t,r,b) = Box2BoxTransformLinear.get_deltas(anchor, gt box).
  *   num_pos = the positive rows.  ctr / grad_ctr: HOST arrays of lv->num_levels device pointers.  workspace:
- *   d2b_fcos_loss_workspace_bytes(lv, N, K, dtype) bytes, 16-byte aligned.  Backward: grad_cls / grad_reg / grad_ctr_sum
+ *   d2b_dense_loss_workspace_bytes(lv, N, K, dtype) bytes, 16-byte aligned.  Backward: grad_cls / grad_reg / grad_ctr_sum
  *   (device scalars); lv->grad_logits, lv->grad_deltas and grad_ctr are fully written (0 on non-positive rows for the
  *   deltas and the centerness, sigmoid(x) - t times grad_ctr_sum on the positive ones). */
-size_t d2b_fcos_loss_workspace_bytes(const d2b_dense_loss_levels* lv, int N, int K, int dtype);
 int d2b_fcos_loss_forward(const d2b_dense_loss_levels* lv, const void* const* ctr, int N, int K, int dtype,
                           const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma, float alpha,
                           float* cls_sum, float* reg_sum, float* ctr_sum, int64_t* num_pos, int* status, void* workspace,

@@ -9,7 +9,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_header_symbols_exported():
+def test_header_symbols_and_abi_version():
     from detectron2_b200 import _C
 
     lib = _C.lib()
@@ -22,7 +22,13 @@ def test_header_symbols_exported():
     assert {n for n in declared if n.startswith(("d2b_roi_", "d2b_pyramid_"))} == {
         "d2b_roi_pooler_forward", "d2b_roi_pooler_backward", "d2b_roi_pooler_nhwc_supported", "d2b_pyramid_nchw_to_nhwc",
         "d2b_pyramid_nhwc_to_nchw"}
-    assert lib.d2b_abi_version() == _C.ABI_VERSION == 5
+    # one entry point per selection stage, the box type and the decode as D2B_SELECT_* flags
+    assert {n for n in declared if re.search(r"_(prepare|select)", n)} == {
+        "d2b_rpn_prepare", "d2b_frcnn_prepare", "d2b_dense_prepare", "d2b_rpn_select"}
+    # the FCOS loss sizes its workspace with d2b_dense_loss_workspace_bytes
+    assert {n for n in declared if n.startswith("d2b_fcos_")} == {
+        "d2b_fcos_assign", "d2b_fcos_loss_forward", "d2b_fcos_loss_backward"}
+    assert lib.d2b_abi_version() == _C.ABI_VERSION == 6
     assert lib.d2b_arch() == b"sm_90a"
     assert _C.get_cuda_version().startswith("CUDA 12")
 
@@ -339,6 +345,130 @@ def test_roi_pooler_entry_points_validate_arguments_without_a_gpu():
                 assert got == want, (what, "bwd" if bwd else "fwd", flags, levels, got)
 
 
+# The inference selection entry points.  Each row is one fault in an otherwise valid call whose pointers are dummy addresses,
+# never dereferenced: (entry point, fault, arguments that differ, expected status or a function of the call's flags giving
+# it, None where the row does not apply).  A flag set with ROT runs the rotated box type, one without it xyxy.
+ROT, SEG, NOOFF, LIN = 1, 2, 4, 8  # D2B_SELECT_ROTATED / _SEG_PER_IMAGE / _NO_OFFSETS / _LINEAR
+_SELECT_KINDS = {  # every flag set each entry point takes
+    "d2b_rpn_prepare": (0, NOOFF, ROT, ROT | SEG),
+    "d2b_frcnn_prepare": (0, ROT, ROT | SEG),
+    "d2b_dense_prepare": (0, LIN),
+    "d2b_rpn_select": (0, ROT),
+}
+_P = 0x1000  # a 16-byte aligned dummy address
+_SELECT_PARAMS = {  # every parameter in order, with its value in a valid call (lv: the levels built by _select_call)
+    "d2b_rpn_prepare": dict(lv=None, N=2, image_hw=_P, min_box_size=0.0, flags=0, flat_boxes=_P, nms_boxes=_P, nms_scores=_P,
+                            raw_scores=_P, cat_ids=_P, nonfinite=_P),
+    "d2b_frcnn_prepare": dict(boxes=_P, scores=_P, row_start=(0, 4, 9), N=2, num_classes=3, kreg=3, image_hw=_P,
+                              score_thresh=0.05, cap=16, flags=0, cand_boxes=_P, nms_boxes=_P, nms_scores=_P, raw_scores=_P,
+                              cand_flat=_P, cat_ids=_P, n_cand=_P, row_map=_P),
+    "d2b_dense_prepare": dict(lv=None, N=2, num_classes=80, weights=(1.0, 1.0, 1.0, 1.0), scale_clamp=4.135, flags=0,
+                              flat_boxes=_P, nms_boxes=_P, nms_scores=_P, raw_scores=_P, classes=_P, cat_ids=_P),
+    "d2b_rpn_select": dict(keep=_P, num_keep=_P, N=2, T=10, post_nms_topk=5, flags=0, flat_boxes=_P, raw_scores=_P,
+                           cat_ids=_P, out_boxes=_P, out_scores=_P, out_index=_P, counts=_P),
+}
+_MISALIGNED = 0x1004
+_XYXY_ONLY = lambda f: EINVAL if not f & ROT else None  # noqa: E731  (rotated boxes have no alignment requirement)
+_SELECT_FAULTS = [
+    ("d2b_rpn_prepare", "no level struct", dict(lv=None), EINVAL),
+    ("d2b_rpn_prepare", "nonfinite NULL", dict(nonfinite=None), EINVAL),
+    ("d2b_rpn_prepare", "N < 0", dict(N=-1), EINVAL),
+    ("d2b_rpn_prepare", "no level", dict(num_levels=0), EINVAL),
+    ("d2b_rpn_prepare", "9 levels", dict(num_levels=9), EINVAL),
+    ("d2b_rpn_prepare", "k > A", dict(k=[11]), EINVAL),
+    ("d2b_rpn_prepare", "top-k indices NULL", dict(topk_idx=[None]), EINVAL),
+    ("d2b_rpn_prepare", "T > INT_MAX", dict(num_levels=2, A=[2 ** 30] * 2, k=[2 ** 30] * 2), EINVAL),
+    ("d2b_rpn_prepare", "image_hw NULL", dict(image_hw=None), EINVAL),
+    ("d2b_rpn_prepare", "nms_boxes NULL", dict(nms_boxes=None), EINVAL),
+    ("d2b_rpn_prepare", "proposals misaligned", dict(proposals=[_MISALIGNED]), _XYXY_ONLY),
+    ("d2b_rpn_prepare", "flat_boxes misaligned", dict(flat_boxes=_MISALIGNED), _XYXY_ONLY),
+    ("d2b_frcnn_prepare", "more images than D2B_MAX_IMAGES", dict(N=65), EINVAL),
+    ("d2b_frcnn_prepare", "N < 0", dict(N=-1), EINVAL),
+    ("d2b_frcnn_prepare", "no class", dict(num_classes=0), EINVAL),
+    ("d2b_frcnn_prepare", "kreg neither 1 nor K", dict(kreg=2), EINVAL),
+    ("d2b_frcnn_prepare", "cap < 0", dict(cap=-1), EINVAL),
+    ("d2b_frcnn_prepare", "row_start NULL", dict(row_start=None), EINVAL),
+    ("d2b_frcnn_prepare", "row_start decreasing", dict(row_start=(0, 4, 3)), EINVAL),
+    ("d2b_frcnn_prepare", "row_start[0] < 0: rows before boxes[0]", dict(row_start=(-1, 4, 9)), EINVAL),
+    ("d2b_frcnn_prepare", "image_hw NULL", dict(image_hw=None), EINVAL),
+    ("d2b_frcnn_prepare", "n_cand NULL", dict(n_cand=None), EINVAL),
+    ("d2b_frcnn_prepare", "boxes NULL", dict(boxes=None), EINVAL),
+    ("d2b_frcnn_prepare", "row_map NULL", dict(row_map=None), EINVAL),
+    ("d2b_frcnn_prepare", "cand_boxes NULL", dict(cand_boxes=None), EINVAL),
+    ("d2b_frcnn_prepare", "cat_ids NULL", dict(cat_ids=None), EINVAL),
+    ("d2b_frcnn_prepare", "cand_boxes misaligned", dict(cand_boxes=_MISALIGNED), _XYXY_ONLY),
+    ("d2b_frcnn_prepare", "nms_boxes misaligned", dict(nms_boxes=_MISALIGNED), _XYXY_ONLY),
+    ("d2b_frcnn_prepare", "no images: nothing to do", dict(N=0, image_hw=None, n_cand=None), 0),
+    ("d2b_dense_prepare", "no level struct", dict(lv=None), EINVAL),
+    ("d2b_dense_prepare", "no level", dict(num_levels=0), EINVAL),
+    ("d2b_dense_prepare", "9 levels", dict(num_levels=9), EINVAL),
+    ("d2b_dense_prepare", "N < 0", dict(N=-1), EINVAL),
+    ("d2b_dense_prepare", "no class", dict(num_classes=0), EINVAL),
+    ("d2b_dense_prepare", "weights NULL", dict(weights=None), lambda f: None if f & LIN else EINVAL),
+    ("d2b_dense_prepare", "weights NULL, no images", dict(weights=None, N=0), lambda f: 0 if f & LIN else EINVAL),
+    ("d2b_dense_prepare", "no images: nothing to do", dict(N=0, flat_boxes=None), 0),
+    ("d2b_dense_prepare", "R < 0", dict(R=[-1]), EINVAL),
+    ("d2b_dense_prepare", "k < 0", dict(k=[-1]), EINVAL),
+    ("d2b_dense_prepare", "anchors NULL", dict(anchors=[None]), EINVAL),
+    ("d2b_dense_prepare", "deltas misaligned", dict(deltas=[_MISALIGNED]), EINVAL),
+    ("d2b_dense_prepare", "T > INT_MAX", dict(num_levels=2, k=[2 ** 30] * 2), EINVAL),
+    ("d2b_dense_prepare", "no candidate: nothing to do", dict(k=[0], flat_boxes=None), 0),
+    ("d2b_dense_prepare", "classes NULL", dict(classes=None), EINVAL),
+    ("d2b_dense_prepare", "flat_boxes misaligned", dict(flat_boxes=_MISALIGNED), EINVAL),
+    ("d2b_dense_prepare", "nms_boxes misaligned", dict(nms_boxes=_MISALIGNED), EINVAL),
+    ("d2b_rpn_select", "N < 0", dict(N=-1), EINVAL),
+    ("d2b_rpn_select", "T < 0", dict(T=-1), EINVAL),
+    ("d2b_rpn_select", "post_nms_topk < 0", dict(post_nms_topk=-1), EINVAL),
+    ("d2b_rpn_select", "no images: nothing to do", dict(N=0, counts=None), 0),
+    ("d2b_rpn_select", "counts NULL", dict(counts=None), EINVAL),
+] + [("d2b_rpn_select", name + " NULL", {name: None}, EINVAL)
+     for name in ("keep", "num_keep", "flat_boxes", "raw_scores", "cat_ids", "out_boxes", "out_scores", "out_index")] + [
+    ("d2b_rpn_select", "flat_boxes misaligned", dict(flat_boxes=_MISALIGNED), _XYXY_ONLY),
+    ("d2b_rpn_select", "out_boxes misaligned", dict(out_boxes=_MISALIGNED), _XYXY_ONLY),
+]
+
+
+def _select_call(lib, entry, flags, **over):
+    import ctypes as C
+
+    from detectron2_b200 import _C
+
+    args = dict(_SELECT_PARAMS[entry], flags=flags)
+    if "lv" in args:  # levels of 10 boxes with a top-k of 5 each
+        lv = _C.RpnLevels() if entry == "d2b_rpn_prepare" else _C.DenseLevels()
+        lv.num_levels = over.pop("num_levels", 1)
+        for name, _ in lv._fields_[1:]:
+            default = 10 if name in ("A", "R") else 5 if name == "k" else _P
+            for l, v in enumerate(over.pop(name, [default] * _C.MAX_LEVELS)):
+                getattr(lv, name)[l] = v
+        args["lv"] = C.byref(lv)
+    args.update(over)
+    if args.get("row_start") is not None:
+        args["row_start"] = (C.c_int * 3)(*args["row_start"])
+    if args.get("weights") is not None:
+        args["weights"] = (C.c_float * 4)(*args["weights"])
+    return getattr(lib, entry)(*args.values(), None)
+
+
+def test_selection_entry_points_validate_arguments_without_a_gpu():
+    """Every fault of the four selection entry points gets its status before anything is launched, for each flag set the
+    entry point takes; every other flag value is D2B_EINVAL.  Without a GPU a launch attempt returns a positive CUDA error,
+    so a status <= 0 here also shows that nothing was launched or written (not even rpn_prepare's zeroing of nonfinite)."""
+    from detectron2_b200 import _C
+
+    lib = _C.lib()
+    assert (_C.SELECT_ROTATED, _C.SELECT_SEG_PER_IMAGE, _C.SELECT_NO_OFFSETS, _C.SELECT_LINEAR) == (ROT, SEG, NOOFF, LIN)
+    for entry, kinds in _SELECT_KINDS.items():
+        for flags in [f for f in range(32) if f not in kinds] + [-1, 1 << 30]:
+            assert _select_call(lib, entry, flags) == EINVAL, (entry, flags)
+    for entry, what, args, want in _SELECT_FAULTS:
+        for flags in _SELECT_KINDS[entry]:
+            w = want(flags) if callable(want) else want
+            if w is not None:
+                got = _select_call(lib, entry, flags, **args)
+                assert got == w, (entry, what, flags, got)
+
+
 def test_roi_pooler_no_images():  # /root/reference/tests/modeling/test_roi_pooler.py:107-115
     from detectron2_b200.poolers import ROIPooler
 
@@ -374,29 +504,15 @@ def _nms_rotated_fn(boxes: torch.Tensor, scores: torch.Tensor, threshold: float)
     return torch.ops.detectron2.nms_rotated(boxes, scores, threshold)
 
 
-def test_new_entry_points_validate_arguments_without_a_gpu():
-    """Status codes of the round-2 entry points on invalid arguments (checked before anything is launched): negative =
-    d2b error (include/d2b200.h), what the Python host turns into RuntimeError."""
+def test_layout_change_and_packed_paste_validate_arguments_without_a_gpu():
+    """Status codes of the pyramid layout changes and the bit-packed paste on invalid arguments (checked before anything is
+    launched): negative = d2b error (include/d2b200.h), what the Python host turns into RuntimeError."""
     import ctypes as C
 
     from detectron2_b200 import _C
 
     lib = _C.lib()
     EINVAL = -1
-    # Fast R-CNN candidates: too many images for one call, class-specific boxes that do not match the class count, no row table
-    rs = (C.c_int * 3)(0, 4, 8)
-    assert lib.d2b_frcnn_prepare(None, None, rs, _C.MAX_IMAGES + 1, 80, 80, None, 0.05, 16, *([None] * 8), None) == EINVAL
-    assert lib.d2b_frcnn_prepare(None, None, rs, 2, 80, 3, None, 0.05, 16, *([None] * 8), None) == EINVAL
-    assert lib.d2b_frcnn_prepare(None, None, None, 2, 80, 80, None, 0.05, 16, *([None] * 8), None) == EINVAL
-    assert lib.d2b_frcnn_prepare(None, None, rs, 0, 80, 80, None, 0.05, 16, *([None] * 8), None) == 0  # no images: nothing to do
-    # dense head: level count out of range, missing weights
-    lv = _C.DenseLevels()
-    lv.num_levels = 0
-    w = (C.c_float * 4)(1, 1, 1, 1)
-    assert lib.d2b_dense_prepare(C.byref(lv), 2, 80, w, 4.135, *([None] * 6), None) == EINVAL
-    lv.num_levels = 1
-    assert lib.d2b_dense_prepare(C.byref(lv), 2, 80, None, 4.135, *([None] * 6), None) == EINVAL
-    assert lib.d2b_dense_prepare(C.byref(lv), 0, 80, w, 4.135, *([None] * 6), None) == 0
     # dtype codes of the half-precision variants
     P = _C.Pyramid()
     P.num_levels = 1

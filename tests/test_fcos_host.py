@@ -62,7 +62,7 @@ def test_linear_decode_inverts_get_deltas():
     assert torch.equal(apply_deltas_linear(torch.tensor([[-1.0, 0.0, -0.5, 0.0]]), an[:1]), torch.tensor([[4.0, 4, 4, 4]]))
 
 
-def test_fcos_entry_points_validate_arguments_without_a_gpu():
+def test_fcos_assign_and_loss_validate_arguments_without_a_gpu():
     from detectron2_b200 import _C
 
     lib = _C.lib()
@@ -107,15 +107,8 @@ def test_fcos_entry_points_validate_arguments_without_a_gpu():
     assert fwd(alpha=math.nan) == EINVAL
     assert fwd(out=None) == EINVAL
     assert fwd() == -2  # workspace too small (checked after the arguments)
-    assert lib.d2b_fcos_loss_workspace_bytes(C.byref(lv), 2, 80, 0) == lib.d2b_dense_loss_workspace_bytes(C.byref(lv), 2,
-                                                                                                            80, 0)
     assert lib.d2b_fcos_loss_backward(C.byref(lv), ctr, None, 2, 80, 0, dummy, dummy, dummy, 2.0, 0.25, dummy, dummy,
                                       dummy, None) == EINVAL  # no centerness gradient buffers
-    dl = _C.DenseLevels()
-    dl.num_levels = 0
-    assert lib.d2b_dense_prepare_linear(C.byref(dl), 2, 80, dummy, dummy, dummy, dummy, dummy, dummy, None) == EINVAL
-    dl.num_levels = 1
-    assert lib.d2b_dense_prepare_linear(C.byref(dl), 2, 0, dummy, dummy, dummy, dummy, dummy, dummy, None) == EINVAL
 
 
 def test_fake_kernels_trace_shapes():

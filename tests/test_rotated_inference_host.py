@@ -1,8 +1,6 @@
 """Rotated RRPN proposal selection and rotated Fast R-CNN inference, on CPU: the oracle restatements and the product's host
 logic against the fixtures from the REAL reference functions (tests/golden/make_golden_rotated.py), the training failure
-mode, thresholds that IoU 0 passes, and the argument checks of the new C entry points (no GPU needed)."""
-import ctypes as C
-
+mode and thresholds that IoU 0 passes."""
 import pytest
 import torch
 
@@ -155,76 +153,3 @@ def test_clip_rotated_matches_reference_clip():
     ref = rref.clip_(b.clone(), (150, 200))
     assert torch.equal(clip_rotated(b, 150.0, 200.0), ref)
     assert ref[3, 4] == 180.0  # -180.00002 normalises to +180
-
-
-def _lib():
-    from detectron2_b200 import _C
-
-    return _C, _C.lib()
-
-
-def _check_rpn_prepare_rejects_bad_arguments(prepare):
-    """The argument checks that d2b_rpn_prepare and d2b_rrpn_prepare share: D2B_EINVAL before the first CUDA call."""
-    _C, lib = _lib()
-    EINVAL = -1
-    fn = getattr(lib, prepare)
-    p = C.c_void_p(16)  # never dereferenced: the checks fail first
-    lv = _C.RpnLevels()
-    lv.num_levels = 1
-    lv.proposals[0], lv.topk_idx[0], lv.topk_scores[0] = 16, 16, 16
-    lv.A[0], lv.k[0] = 10, 5
-    args = lambda lv_, n=2, nf=p: (C.byref(lv_), n, p, 0.0, 0, p, p, p, p, p, nf, None)  # noqa: E731
-    assert fn(None, 2, p, 0.0, 0, p, p, p, p, p, p, None) == EINVAL
-    assert fn(*args(lv, nf=None)) == EINVAL
-    assert fn(*args(lv, n=-1)) == EINVAL
-    for field, value in (("num_levels", 0), ("num_levels", 9)):
-        bad = _C.RpnLevels.from_buffer_copy(lv)
-        setattr(bad, field, value)
-        assert fn(*args(bad)) == EINVAL, (field, value)
-    bad = _C.RpnLevels.from_buffer_copy(lv)
-    bad.k[0] = 11  # k > A
-    assert fn(*args(bad)) == EINVAL
-    bad = _C.RpnLevels.from_buffer_copy(lv)
-    bad.topk_idx[0] = None
-    assert fn(*args(bad)) == EINVAL
-    assert fn(C.byref(lv), 2, None, 0.0, 0, p, p, p, p, p, p, None) == EINVAL
-    assert fn(C.byref(lv), 2, p, 0.0, 0, p, None, p, p, p, p, None) == EINVAL
-
-
-def test_rpn_prepare_rejects_bad_arguments():
-    """d2b_rpn_prepare checks its arguments by the same rules as d2b_rrpn_prepare (one shared host check)."""
-    _check_rpn_prepare_rejects_bad_arguments("d2b_rpn_prepare")
-
-
-def test_rotated_entry_points_reject_bad_arguments():
-    """Every argument is checked before the first CUDA call: these return D2B_EINVAL without a GPU."""
-    _check_rpn_prepare_rejects_bad_arguments("d2b_rrpn_prepare")
-    _C, lib = _lib()
-    EINVAL = -1
-    p = C.c_void_p(16)  # never dereferenced: the checks fail first
-
-    rs = (C.c_int * 3)(0, 4, 9)
-    good = [p, p, rs, 2, 3, 3, p, 0.05, 16, 0, p, p, p, p, p, p, p, p, None]
-
-    def frcnn(**over):
-        a = list(good)
-        names = ["boxes", "scores", "row_start", "N", "K", "kreg", "hw", "thr", "cap", "seg", "cand_boxes", "nms_boxes",
-                 "nms_scores", "raw_scores", "cand_flat", "cat_ids", "n_cand", "row_map"]
-        for k, v in over.items():
-            a[names.index(k)] = v
-        return lib.d2b_frcnn_rotated_prepare(*a)
-
-    for over in (dict(N=65), dict(N=-1), dict(K=0), dict(kreg=2), dict(cap=-1), dict(row_start=None),
-                 dict(row_start=(C.c_int * 3)(0, 4, 3)), dict(hw=None), dict(n_cand=None), dict(boxes=None),
-                 dict(row_map=None), dict(cand_boxes=None), dict(cat_ids=None)):
-        assert frcnn(**over) == EINVAL, over
-
-    sel = [p, p, 2, 10, 5, p, p, p, p, p, p, p, None]
-    for i, v in ((2, -1), (3, -1), (4, -1), (11, None)):
-        a = list(sel)
-        a[i] = v
-        assert lib.d2b_rpn_select_rotated(*a) == EINVAL, (i, v)
-    for i in (0, 1, 5, 6, 7, 8, 9, 10):
-        a = list(sel)
-        a[i] = None
-        assert lib.d2b_rpn_select_rotated(*a) == EINVAL, i
