@@ -63,6 +63,18 @@ class DenseLossLevels(C.Structure):
                 ("R", C.c_int * MAX_LEVELS)]
 
 
+class SemSegImages(C.Structure):
+    _fields_ = [("h", C.c_int * MAX_IMAGES), ("w", C.c_int * MAX_IMAGES), ("H", C.c_int * MAX_IMAGES),
+                ("W", C.c_int * MAX_IMAGES), ("labels", C.c_void_p * MAX_IMAGES)]
+
+
+class PanopticImages(C.Structure):
+    _fields_ = [("R", C.c_int * MAX_IMAGES), ("H", C.c_int * MAX_IMAGES), ("W", C.c_int * MAX_IMAGES),
+                ("scores", C.c_void_p * MAX_IMAGES), ("classes", C.c_void_p * MAX_IMAGES),
+                ("masks", C.c_void_p * MAX_IMAGES), ("labels", C.c_void_p * MAX_IMAGES),
+                ("panoptic", C.c_void_p * MAX_IMAGES)]
+
+
 def _declare(lib):
     vp, f32p, i64p, u8p = C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p
     i, f, d, sz, i64 = C.c_int, C.c_float, C.c_double, C.c_size_t, C.c_int64
@@ -121,6 +133,9 @@ def _declare(lib):
                                               vp]),
         "d2b_deform_conv_fused_backward": (i, [f32p, f32p, f32p, f32p, i, f32p, f32p, C.POINTER(DcnParams), i, i, vp, f32p,
                                                f32p, f32p, vp, sz, vp]),
+        "d2b_sem_seg_labels": (i, [vp, i, i, i, i, i, C.POINTER(SemSegImages), vp]),
+        "d2b_panoptic_workspace_bytes": (sz, [C.POINTER(PanopticImages), i, i]),
+        "d2b_panoptic_combine": (i, [C.POINTER(PanopticImages), i, i, i64p, d, d, d, i64p, i64p, f32p, vp, vp, sz, vp]),
         "d2b_paste_masks": (i, [f32p, f32p, i, i, i, i, f, u8p, vp]),
         "d2b_paste_masks_packed": (i, [f32p, f32p, i, i, i, i, f, vp, vp]),
     }

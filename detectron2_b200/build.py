@@ -27,6 +27,7 @@ SOURCES = {
     "match.cu": ["-fmad=false"],
     "sampling.cu": [],
     "keypoints.cu": ["-fmad=false"],
+    "panoptic.cu": ["-fmad=false"],
     "losses.cu": ["-fmad=false"],
     "deform_conv.cu": [],
     "deform_conv_tc.cu": [],

@@ -386,6 +386,74 @@ int d2b_keypoint_loss_forward(const void* logits, int dtype, int N, int K, int S
 int d2b_keypoint_loss_backward(const void* logits, int dtype, int N, int K, int S, const int64_t* target,
                                const uint8_t* valid, const float* grad_scale, void* grad_logits, void* stream);
 
+/* ---- Panoptic FPN inference: semantic labels and the thing / stuff combine --------------------------------------------
+ * Replace the per-image loop of PanopticFPN.inference (modeling/meta_arch/panoptic_fpn.py:159-179): sem_seg_postprocess
+ * (modeling/postprocessing.py:77-100) + argmax(dim=0), and combine_semantic_and_instance_outputs (panoptic_fpn.py:184-269),
+ * for N <= D2B_MAX_IMAGES images of different sizes, without host reads.  Images are described per image (pointers and
+ * sizes), so a batch of differently sized detector_postprocess outputs needs no concatenation.
+ *
+ * d2b_sem_seg_labels: logits [N,C,Hp,Wp] of `dtype` (D2B_F32 / D2B_F16 / D2B_BF16, read in place); per image the crop
+ *   (h[n], w[n]) <= (Hp, Wp) of the top-left corner and the output size (H[n], W[n]); labels[n] [H[n],W[n]] int64 out =
+ *   argmax over the channels of the bilinear resize of the crop (align_corners = False, no scale factor: PyTorch's CUDA
+ *   upsample_bilinear2d arithmetic, a plain copy when the sizes are equal), each channel's value rounded to `dtype` before
+ *   the comparison.  Argmax as torch.argmax on CUDA: the first maximal channel wins; a NaN beats every number and the first
+ *   NaN wins; -0.0 == +0.0.  The C x H x W map is never stored.  One launch.
+ *   Checks, in order (nothing is launched before all pass):
+ *     1. D2B_EINVAL: img NULL, N < 0 or N > D2B_MAX_IMAGES, dtype not a D2B_F* code, C < 1, Hp < 1 or Wp < 1.
+ *     2. N == 0: D2B_OK.
+ *     3. D2B_EINVAL: logits NULL; per image h outside 1..Hp, w outside 1..Wp, H or W below 1, H * W > INT_MAX, labels NULL.
+ *
+ * d2b_panoptic_combine: per image n, R[n] instances: scores[n] [R] fp32, classes[n] [R] int64, masks[n] [R,H,W] uint8 (any
+ *   nonzero byte is "in"); labels[n] [H,W] int64 in [0, C); num_instances [N] int64 (device, NULL = R[n]; clamped to
+ *   [0, R[n]]: rows at or past it are ignored).  Per image, restating panoptic_fpn.py:206-267:
+ *     1. the instances ordered by ascending -score: a NaN (either sign) goes last, ties to the lower index (the reference's
+ *        argsort is not stable; this is the documented tie rule).  Not the NMS order, where NaN comes first;
+ *     2. walked in that order, stopping at the first with (double)score < instances_score_thresh (a NaN never stops it);
+ *     3. area = the instance's nonzero pixels; area == 0: skipped, no id consumed;
+ *     4. inter = its pixels already painted; (double)inter / (double)area > overlap_threshold: skipped;
+ *     5. otherwise the next id (from 1) paints its unpainted pixels, and the record (id, isthing 1, classes[i], instance i,
+ *        area = the pixels painted; score = scores[i]) is written;
+ *     6. then every label present anywhere in labels[n], ascending, label 0 skipped: a = its still unpainted pixels;
+ *        (double)a < stuff_area_thresh: skipped; otherwise the next id paints them, record (id, isthing 0, label, -1, a;
+ *        score 0).  With stuff_area_thresh <= 0 a present but fully covered label becomes a zero-area segment.
+ *   Outputs: panoptic[n] [H,W] int32, every pixel written (0 = unassigned); num_segments [N] int64; seg_info [N,S,5] int64
+ *   (id, isthing, category, instance, area) and seg_score [N,S] fp32, S = max_n R[n] + C slots, those past num_segments[n]
+ *   zero; status [N] int32: D2B_PANOPTIC_STATUS_BAD_LABEL when a label of the image is outside [0, C) (the image's other
+ *   outputs are then unspecified).  Integer decisions, double threshold comparisons: bitwise reproducible.
+ *   workspace: d2b_panoptic_workspace_bytes(img, N, C) bytes, 256-byte aligned, no initialisation needed (0 for an invalid
+ *   description).  Four launches: bit-packing of the masks, one CTA per image for the ordered walk (the instances are ranked
+ *   by counting, hence R[n] <= D2B_PANOPTIC_MAX_INSTANCES), the stuff histogram of the unpainted pixels, the stuff ids.
+ *   Checks, in order (nothing is launched before all pass):
+ *     1. D2B_EINVAL: img NULL, N < 0 or N > D2B_MAX_IMAGES, C < 1 or C > D2B_PANOPTIC_MAX_CLASSES.
+ *     2. N == 0: D2B_OK.
+ *     3. D2B_EINVAL: per image H or W below 1, H * W > INT_MAX, R < 0 or R > D2B_PANOPTIC_MAX_INSTANCES, labels or panoptic
+ *        NULL, or, when R > 0, scores, classes or masks NULL; num_segments, seg_info, seg_score, status or workspace NULL;
+ *        workspace not 256-byte aligned.
+ *     4. D2B_EWORKSPACE: workspace_bytes below d2b_panoptic_workspace_bytes(img, N, C). */
+#define D2B_PANOPTIC_MAX_INSTANCES 4096
+#define D2B_PANOPTIC_MAX_CLASSES 1024
+#define D2B_PANOPTIC_STATUS_BAD_LABEL 1
+typedef struct {
+  int h[D2B_MAX_IMAGES], w[D2B_MAX_IMAGES];  /* crop of the logits */
+  int H[D2B_MAX_IMAGES], W[D2B_MAX_IMAGES];  /* output size */
+  int64_t* labels[D2B_MAX_IMAGES];
+} d2b_sem_seg_images;
+typedef struct {
+  int R[D2B_MAX_IMAGES], H[D2B_MAX_IMAGES], W[D2B_MAX_IMAGES];
+  const float* scores[D2B_MAX_IMAGES];
+  const int64_t* classes[D2B_MAX_IMAGES];
+  const uint8_t* masks[D2B_MAX_IMAGES];
+  const int64_t* labels[D2B_MAX_IMAGES];
+  int32_t* panoptic[D2B_MAX_IMAGES];
+} d2b_panoptic_images;
+int d2b_sem_seg_labels(const void* logits, int dtype, int N, int C, int Hp, int Wp, const d2b_sem_seg_images* img,
+                       void* stream);
+size_t d2b_panoptic_workspace_bytes(const d2b_panoptic_images* img, int N, int C);
+int d2b_panoptic_combine(const d2b_panoptic_images* img, int N, int C, const int64_t* num_instances,
+                         double overlap_threshold, double stuff_area_thresh, double instances_score_thresh,
+                         int64_t* num_segments, int64_t* seg_info, float* seg_score, int* status, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 /* ---- Box-branch training losses: RPN / RRPN, RetinaNet, Fast R-CNN ------------------------------------------------
  * Replace RPN.losses (proposal_generator/rpn.py:366-429), RetinaNet.losses (meta_arch/retinanet.py:160-210) and
  * FastRCNNOutputLayers.losses / box_reg_loss / _log_classification_stats (roi_heads/fast_rcnn.py:88-115, 307-352, 424-463)
