@@ -52,6 +52,10 @@ constexpr int kLaunchRegs = (65536 / kThreads) & ~7;
 constexpr int kWorkerRegs = 112, kSideRegs = 24;
 static_assert(kWorkers * kWorkerRegs + (kThreads - kWorkers) * kSideRegs <= kThreads * kLaunchRegs,
               "register budget exceeds the launch allocation");
+// what the workers leave of the launch allocation: the side warpgroup of the fused backward (dcn_bwd_fused_kernel), whose
+// producer lane does not fit the K3c part of it in kSideRegs
+constexpr int kSideRegsMax = ((kThreads * kLaunchRegs - kWorkers * kWorkerRegs) / (kThreads - kWorkers)) & ~7;
+static_assert(kSideRegsMax >= kSideRegs, "register budget exceeds the launch allocation");
 constexpr int kMaxBN = 128;                  // widest output-channel tile: 64 accumulator columns (32 registers) per warpgroup
 constexpr int kRowsPerHalf = 128 / (2 * kWorkerWarps);  // pixel rows of a 128-row tile owned by one half-warp: 4
 constexpr int kTile = 16384;                 // [128 rows][128 B]
@@ -80,8 +84,9 @@ struct Epi {
 };
 
 // noct: output-channel tiles of a super-group; goct: those of them the launch computes (noct, or 1 when the column-fed K1c
-// computes the others); red: k-split partial sums meet through red.add
-struct K1P { int BN, noct, goct, nkp, ksplit, S, tap_bytes, stage_bytes, red; };
+// computes the others); uper: units of the reduction per k-split part (the last part may have fewer); red: k-split partial
+// sums meet through red.add
+struct K1P { int BN, noct, goct, uper, ksplit, S, tap_bytes, stage_bytes, red; };
 struct K2P { int mper, msplit, tap_bytes; };
 struct K3P { int BN, noct, sper, nsplit, S, stage_bytes; };
 
@@ -157,6 +162,12 @@ int best_split(long long base, int work, int max_split, int overhead) {
   return best;
 }
 
+// kernel points whose taps a range of `units` consecutive units may touch, wherever the range starts inside a kernel point
+int k1_tap_points(const TC& d, int units) { return std::min(d.KK, (units + d.cbs - 2) / d.cbs + 1); }
+
+// The reduction is split by units, not by whole kernel points, so that the parts can fill the SMs where a kernel point holds
+// many channel blocks (res5: 8 units per kernel point).  A CTA's fixed cost (taps, pipeline fill, the red.add epilogue) is
+// counted as one kernel point's units.
 // colfed: the gathering K1 runs output-channel tile 0 only and K1c the others (plan_k1c)
 bool plan_k1(const TC& d, K1P& k, bool colfed = false) {
   k.BN = largest_tile(d.ops);
@@ -164,28 +175,28 @@ bool plan_k1(const TC& d, K1P& k, bool colfed = false) {
   k.noct = d.ops / k.BN;
   k.goct = colfed ? 1 : k.noct;
   const int base = d.N * d.tiles_img * d.SG * k.goct;
-  k.ksplit = best_split(base, d.KK, d.KK, 1);
-  k.nkp = d2b_cdiv(d.KK, k.ksplit);
-  k.ksplit = d2b_cdiv(d.KK, k.nkp);
+  k.ksplit = best_split(base, d.U, d.U, d.cbs);
+  k.uper = d2b_cdiv(d.U, k.ksplit);
+  k.ksplit = d2b_cdiv(d.U, k.uper);
   k.red = k.ksplit > 1;
   const int ndg = d.DG == 1 ? 1 : std::min(d.DG, d2b_cdiv(d.cps, d.cpdg) + 1);
-  k.tap_bytes = ndg * k.nkp * 128 * 16;
+  k.tap_bytes = ndg * k1_tap_points(d, k.uper) * 128 * 16;
   k.stage_bytes = 2 * kTile + 2 * k.BN * 128;
   k.S = 3;
   while (k.S > 1 && k.S * k.stage_bytes + k.tap_bytes + 1024 + 128 > kMaxSmem) --k.S;
   return k.S >= 2;
 }
 
-// K1c: output-channel tiles 1..noct-1 of a column-fed forward, split over kernel points on its own grid.  Both launches
-// write the same output: if either splits, both add their partials (k1.red and kc.red are set together).
+// K1c: output-channel tiles 1..noct-1 of a column-fed forward, split over units on its own grid.  Both launches write the
+// same output: if either splits, both add their partials (k1.red and kc.red are set together).
 bool plan_k1c(const TC& d, K1P& k1, K1P& kc) {
   const long long base = (long long)d.N * d.tiles_img * d.SG * (k1.noct - 1);
   if (k1.goct != 1 || k1.noct < 2 || (long long)d.N * d.tiles_img * (k1.noct - 1) > 0x7fffffffLL) return false;
   kc = k1;
   kc.goct = k1.noct - 1;
-  kc.ksplit = best_split(base, d.KK, d.KK, 1);
-  kc.nkp = d2b_cdiv(d.KK, kc.ksplit);
-  kc.ksplit = d2b_cdiv(d.KK, kc.nkp);
+  kc.ksplit = best_split(base, d.U, d.U, d.cbs);
+  kc.uper = d2b_cdiv(d.U, kc.ksplit);
+  kc.ksplit = d2b_cdiv(d.U, kc.uper);
   kc.tap_bytes = 0;
   kc.S = 3;
   while (kc.S > 1 && kc.S * kc.stage_bytes + 1024 + 128 > kMaxSmem) --kc.S;
@@ -448,12 +459,13 @@ __device__ __forceinline__ void fwd_epilogue(const float (&acc)[BN / 4], const E
 }
 
 // ================================================================================================ K1: forward
-// grid (N * tiles_img, SG * k.goct, k splits).  Warp 17 is the SAVER, which (when the caller keeps the
-// sampled columns for the weight gradient) copies every finished A stage -- already bf16 hi | lo in the tensor core's
-// swizzled tile layout -- to global memory with one bulk store, so that the backward streams the tiles back instead of
-// sampling x a second time (dcn_bwd_weight_cols_kernel).  Column tile of (image tile, super-group, unit): 16 KB hi [+ 16 KB lo].
-// The workers issue the MMAs of stage t right after gathering it and release stage t - 1 once its MMAs are done, so the
-// gather of a stage overlaps the MMAs of the previous one.
+// grid (N * tiles_img, SG * k.goct, k splits); split z reduces over units [z * k.uper, +k.uper), which may begin and end
+// inside a kernel point's channel blocks: the tap table holds the kernel points the range touches.  Warp 17 is the SAVER,
+// which (when the caller keeps the sampled columns for the weight gradient) copies every finished A stage -- already bf16
+// hi | lo in the tensor core's swizzled tile layout -- to global memory with one bulk store, so that the backward streams
+// the tiles back instead of sampling x a second time (dcn_bwd_weight_cols_kernel).  Column tile of (image tile,
+// super-group, unit): 16 KB hi [+ 16 KB lo].  The workers issue the MMAs of stage t right after gathering it and release
+// stage t - 1 once its MMAs are done, so the gather of a stage overlaps the MMAs of the previous one.
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __restrict__ xh,
                                                                    const float* __restrict__ offset,
@@ -471,8 +483,8 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.x / d.tiles_img, p0 = (blockIdx.x - b * d.tiles_img) * 128;
   const int sg = blockIdx.y / k.goct, oct = blockIdx.y - sg * k.goct;
-  const int kp0 = blockIdx.z * k.nkp, nkp = min(d.KK, kp0 + k.nkp) - kp0;
-  const int nt = nkp * d.cbs;
+  const int u0 = blockIdx.z * k.uper, nt = min(d.U, u0 + k.uper) - u0;
+  const int kp0 = u0 / d.cbs, nkp = (u0 + nt - 1) / d.cbs - kp0 + 1;
   const int dg0 = (sg * d.cps) / d.cpdg;
   const bool saving = cols != nullptr && oct == 0;  // CTAs of the other output-channel tiles build the same columns
 
@@ -503,7 +515,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
     float acc[BN / 4];
 #pragma unroll
     for (int i = 0; i < BN / 4; ++i) acc[i] = 0.f;
-    int kpl = 0, cb = 0;
+    int kpl = 0, cb = u0 - kp0 * d.cbs;
     // gather stage t, then issue its MMAs (one wgmma group)
     auto stage = [&](int t) {
       const int s = t % k.S;
@@ -554,7 +566,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
         const int s = t % k.S;
         const uint32_t par = (uint32_t)((t / k.S) & 1);
         mbar_wait(&empty_bar[s], par ^ 1u);
-        const size_t tile = ((size_t)(sg * k.noct + oct) * d.U + (size_t)kp0 * d.cbs + t);
+        const size_t tile = ((size_t)(sg * k.noct + oct) * d.U + u0 + t);
         mbar_arrive_expect_tx(&full_bar[s], bytes);
         bulk_g2s(smem + s * k.stage_bytes + 2 * kTile, wt + tile * (size_t)(2 * k.BN * 128), bytes, &full_bar[s]);
       }
@@ -567,7 +579,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
         const int s = t % k.S;
         const uint32_t par = (uint32_t)((t / k.S) & 1);
         mbar_wait(&full_bar[s], par);  // the workers' writes are fenced to the async proxy before they arrive
-        const size_t tile = ((size_t)blockIdx.x * d.SG + sg) * d.U + (size_t)kp0 * d.cbs + t;
+        const size_t tile = ((size_t)blockIdx.x * d.SG + sg) * d.U + u0 + t;
         bulk_s2g(cols + tile * tile_bytes, smem + s * k.stage_bytes, tile_bytes);
         bulk_commit();
         bulk_wait_read0();
@@ -582,7 +594,8 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_tc_kernel(const float* __
 // Output-channel tiles 1..noct-1 of a forward that saves its columns: K1 gathers and saves them once (tile 0), and this kernel
 // streams each stage's column tile back with one bulk copy (hi [+ lo], already in K1's swizzled A layout) next to K1's weight
 // tile of its output-channel tile: a pure TMA -> wgmma pipeline like K3c, with K1's epilogue.  grid ((N * tiles_img) *
-// (noct - 1), SG, k splits), the output-channel tile fastest: the CTAs that read one column tile run together and share it in L2.
+// (noct - 1), SG, k splits over units as in K1), the output-channel tile fastest: the CTAs that read one column tile run
+// together and share it in L2.
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_cols_kernel(const uint8_t* __restrict__ cols,
                                                                    const uint8_t* __restrict__ wt, const Epi ep, const TC d,
@@ -597,8 +610,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_cols_kernel(const uint8_t
   const int tile = blockIdx.x / k.goct, oct = 1 + (blockIdx.x - tile * k.goct);
   const int b = tile / d.tiles_img, p0 = (tile - b * d.tiles_img) * 128;
   const int sg = blockIdx.y;
-  const int kp0 = blockIdx.z * k.nkp, nkp = min(d.KK, kp0 + k.nkp) - kp0;
-  const int nt = nkp * d.cbs;
+  const int u0 = blockIdx.z * k.uper, nt = min(d.U, u0 + k.uper) - u0;
 
   if (tid == 0) {
     for (int s = 0; s < k.S; ++s) {
@@ -636,7 +648,6 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_cols_kernel(const uint8_t
       const uint32_t parts = split ? 2u : 1u;
       // pointers and ring position advance with the stage (this warp runs on kSideRegs registers)
       const uint32_t abytes = parts * (uint32_t)kTile;
-      const size_t u0 = (size_t)kp0 * d.cbs;
       const uint8_t* asrc = cols + (((size_t)tile * d.SG + sg) * d.U + u0) * abytes;  // as K1's saver wrote them
       const uint8_t* bsrc = wt + ((size_t)(sg * k.noct + oct) * d.U + u0) * (size_t)(2 * BN * 128);
       int s = 0;
@@ -662,16 +673,14 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_fwd_cols_kernel(const uint8_t
 //   grad_x   += gcol * mask * bilinear weight      (deform_conv_cuda_kernel.cu:313-362, :923-975) red.global.add.v4 (NHWC)
 //   grad_off += gcol * mask * d(sample)/d(h,w)     (:390-451, :977-1064)                           red.global.add
 //   grad_msk += gcol * sample                      (:1053-1064)
-__global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const float* __restrict__ xh,
-                                                                      const float* __restrict__ offset,
-                                                                      const float* __restrict__ mask,
-                                                                      const uint8_t* __restrict__ gt,
-                                                                      const uint8_t* __restrict__ wt, const TC d,
-                                                                      const K2P k, const int split,
-                                                                      float* __restrict__ gxh, float* __restrict__ goff,
-                                                                      float* __restrict__ gmask) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // offset form keeps the shared address space
+// The body takes its block coordinates so that the fused backward (dcn_bwd_fused_kernel) can run it too; smem is the
+// 1024-byte aligned dynamic shared memory.
+template <int kSide>
+__device__ __forceinline__ void bwd_data_body(uint8_t* smem, int bx, int by, int bz, const float* __restrict__ xh,
+                                              const float* __restrict__ offset, const float* __restrict__ mask,
+                                              const uint8_t* __restrict__ gt, const uint8_t* __restrict__ wt, const TC& d,
+                                              const K2P& k, const int split, float* __restrict__ gxh,
+                                              float* __restrict__ goff, float* __restrict__ gmask) {
   constexpr int kStage = 4 * kTile;  // A hi | A lo | B hi | B lo
   float* gcol = reinterpret_cast<float*>(smem + 2 * kStage);
   int4* taps = reinterpret_cast<int4*>(smem + 2 * kStage + 128 * kGcolPitch * 4);
@@ -680,9 +689,9 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
   uint64_t* empty_bar = bars + 2;    // [2]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int b = blockIdx.x / d.tiles_img, pt = blockIdx.x - b * d.tiles_img, p0 = pt * 128;
-  const int sg = blockIdx.y;
-  const int m0 = blockIdx.z * k.mper, m1 = min(d.MC, m0 + k.mper), nm = m1 - m0;
+  const int b = bx / d.tiles_img, pt = bx - b * d.tiles_img, p0 = pt * 128;
+  const int sg = by;
+  const int m0 = bz * k.mper, m1 = min(d.MC, m0 + k.mper), nm = m1 - m0;
   const int u_begin = 2 * m0, u_end = min(d.U, 2 * m1);
   const int kp0 = u_begin / d.cbs, nkp = (u_end - 1) / d.cbs - kp0 + 1;
   const int dg0 = (sg * d.cps) / d.cpdg;
@@ -704,7 +713,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
   }
   __syncthreads();
   if (warp < kWorkerWarps) reg_alloc<kWorkerRegs>();
-  else reg_dealloc<kSideRegs>();
+  else reg_dealloc<kSide>();
 
   if (warp < kWorkerWarps) {
     const int half = lane >> 4, q = lane & 15;
@@ -888,6 +897,24 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const floa
       }
     }
   }
+}
+
+__device__ __forceinline__ uint8_t* aligned_smem() {
+  extern __shared__ uint8_t smem_raw[];
+  return smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // offset form keeps the shared address space
+}
+
+// grid (N * tiles_img, SG, macro-chunk splits)
+__global__ void __launch_bounds__(kThreads, 1) dcn_bwd_data_tc_kernel(const float* __restrict__ xh,
+                                                                      const float* __restrict__ offset,
+                                                                      const float* __restrict__ mask,
+                                                                      const uint8_t* __restrict__ gt,
+                                                                      const uint8_t* __restrict__ wt, const TC d,
+                                                                      const K2P k, const int split,
+                                                                      float* __restrict__ gxh, float* __restrict__ goff,
+                                                                      float* __restrict__ gmask) {
+  bwd_data_body<kSideRegs>(aligned_smem(), blockIdx.x, blockIdx.y, blockIdx.z, xh, offset, mask, gt, wt, d, k, split, gxh,
+                           goff, gmask);
 }
 
 // ================================================================================================ weight-gradient epilogue
@@ -1083,22 +1110,19 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_tc_kernel(const fl
 // Same grid, tiles and epilogue as K3, but the A operand is streamed back from the column tiles the forward saved
 // (dcn_fwd_tc_kernel's saver warp) instead of being sampled from x again: a pure TMA -> wgmma pipeline.  A 64-pixel stage of
 // a unit is one contiguous 8 KB half of its [128 px][64 ch] tile (the 128-byte swizzle repeats every 8 rows).
-template <int BN>
-__global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const uint8_t* __restrict__ cols,
-                                                                          const uint8_t* __restrict__ gt, const TC d,
-                                                                          const K3P k, const int S, const int split,
-                                                                          float* __restrict__ gw) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+template <int BN, int kSide>
+__device__ __forceinline__ void bwd_weight_cols_body(uint8_t* smem, int bx, int by, int bz, const uint8_t* __restrict__ cols,
+                                                     const uint8_t* __restrict__ gt, const TC& d, const K3P& k, const int S,
+                                                     const int split, float* __restrict__ gw) {
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * k.stage_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + S;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int mb = blockIdx.y;
-  const int sg = blockIdx.x / k.noct, oct = blockIdx.x - sg * k.noct;
+  const int mb = by;
+  const int sg = bx / k.noct, oct = bx - sg * k.noct;
   const int total = d.N * d.stages_img;
-  const int gs0 = blockIdx.z * k.sper, gs1 = min(total, gs0 + k.sper), ns = gs1 - gs0;
+  const int gs0 = bz * k.sper, gs1 = min(total, gs0 + k.sper), ns = gs1 - gs0;
   const int nu = (2 * mb + 1 < d.U) ? 2 : 1;
 
   if (tid == 0) {
@@ -1118,7 +1142,7 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const 
   }
   __syncthreads();
   if (warp < kWorkerWarps) reg_alloc<kWorkerRegs>();
-  else reg_dealloc<kSideRegs>();
+  else reg_dealloc<kSide>();
 
   if (warp < kWorkerWarps) {
     // =============================================================== MMA (as K3), then registers -> this split's partial tile
@@ -1163,6 +1187,46 @@ __global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const 
         bulk_g2s(stage + 2 * kTile, gt + tile * (size_t)(2 * k.BN * 128), gbytes, &full_bar[s]);
       }
     }
+  }
+}
+
+// grid (SG * noct, unit pairs, pixel splits)
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1) dcn_bwd_weight_cols_kernel(const uint8_t* __restrict__ cols,
+                                                                          const uint8_t* __restrict__ gt, const TC d,
+                                                                          const K3P k, const int S, const int split,
+                                                                          float* __restrict__ gw) {
+  bwd_weight_cols_body<BN, kSideRegs>(aligned_smem(), blockIdx.x, blockIdx.y, blockIdx.z, cols, gt, d, k, S, split, gw);
+}
+
+// ================================================================================================ fused backward: K2 + K3c
+// One launch for a backward that wants both gradients from saved columns: the first N * tiles_img * SG * msplit CTAs of the
+// 1-D grid run K2's body, the rest K3c's.  The two read only what the pre-passes wrote and write disjoint outputs, so the
+// K3c CTAs fill the SMs that K2's grid leaves idle and its last wave runs beside K2's CTAs instead of after them.  K2's CTAs
+// come first: they are the long ones.  Dynamic shared memory is the larger of the two bodies' needs.
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1) dcn_bwd_fused_kernel(const float* __restrict__ xh,
+                                                                    const float* __restrict__ offset,
+                                                                    const float* __restrict__ mask,
+                                                                    const uint8_t* __restrict__ gt_px,
+                                                                    const uint8_t* __restrict__ wt, const K2P k2,
+                                                                    float* __restrict__ gxh, float* __restrict__ goff,
+                                                                    float* __restrict__ gmask,
+                                                                    const uint8_t* __restrict__ cols,
+                                                                    const uint8_t* __restrict__ gt_oc, const K3P k3,
+                                                                    const int S3, float* __restrict__ gw, const TC d,
+                                                                    const int split) {
+  const int nx2 = d.N * d.tiles_img, n2 = nx2 * d.SG * k2.msplit;
+  int id = blockIdx.x;
+  if (id < n2) {
+    const int bx = id % nx2, r = id / nx2;
+    bwd_data_body<kSideRegsMax>(aligned_smem(), bx, r % d.SG, r / d.SG, xh, offset, mask, gt_px, wt, d, k2, split, gxh, goff,
+                                gmask);
+  } else {
+    id -= n2;
+    const int nx3 = d.SG * k3.noct, r = id / nx3;
+    bwd_weight_cols_body<BN, kSideRegsMax>(aligned_smem(), id % nx3, r % d.MC, r / d.MC, cols, gt_oc, d, k3, S3, split,
+                                           gw);
   }
 }
 
@@ -1511,6 +1575,12 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
     int rc = d2b_zero_buffers(zp, zb, 4, stream);
     if (rc) return rc;
   }
+  // With saved columns and both gradients wanted, K2 and K3c run as one launch (dcn_bwd_fused_kernel) on a 1-D grid.
+  const long long fused_ctas = (long long)d.N * d.tiles_img * d.SG * k2.msplit + (long long)d.SG * k3.noct * d.MC * k3.nsplit;
+  const bool fused = need_data && need_weight && cols && fused_ctas <= 0x7fffffffLL;
+  const uint8_t* cl = reinterpret_cast<const uint8_t*>(cols);
+  const int S3 = std::min(6, (kMaxSmem - 2048) / k3.stage_bytes);  // K3c's operand ring
+  const int smem3 = S3 * k3.stage_bytes + 1024 + 128;
   if (need_data) {
     uint8_t* gt_px = ws + P.gt_px;
     uint8_t* wt = ws + P.wt;
@@ -1523,11 +1593,20 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
       dcn_wtile_bwd_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(weight, d, wt);
       D2B_CHECK_LAUNCH();
     }
-    const int smem_bytes = 2 * 4 * kTile + 128 * kGcolPitch * 4 + k2.tap_bytes + 1024 + 128;
-    if (int rc = launch_big_smem<dcn_bwd_data_tc_kernel>(dim3(d.N * d.tiles_img, d.SG, k2.msplit), smem_bytes, stream, xh,
-                                                         offset, mask, gt_px, wt, d, k2, P.split, gxh, grad_offset,
-                                                         mask ? grad_mask : nullptr))
-      return rc;
+    const int smem2 = 2 * 4 * kTile + 128 * kGcolPitch * 4 + k2.tap_bytes + 1024 + 128;
+    float* gm = mask ? grad_mask : nullptr;
+    int rc;
+    if (fused) {
+      rc = with_tile_width<64, 128>(k3.BN, [&](auto bn) {
+        return launch_big_smem<dcn_bwd_fused_kernel<decltype(bn)::value>>(
+            dim3((unsigned)fused_ctas), std::max(smem2, smem3), stream, xh, offset, mask, gt_px, wt, k2, gxh, grad_offset, gm,
+            cl, gt_oc, k3, S3, gw_part, d, P.split);
+      });
+    } else {
+      rc = launch_big_smem<dcn_bwd_data_tc_kernel>(dim3(d.N * d.tiles_img, d.SG, k2.msplit), smem2, stream, xh, offset, mask,
+                                                   gt_px, wt, d, k2, P.split, gxh, grad_offset, gm);
+    }
+    if (rc) return rc;
     if (grad_x && !x_nhwc) {
       if (int rc = change_layout(gxh, d, grad_x, false, stream)) return rc;
     }
@@ -1538,26 +1617,25 @@ int d2b_deform_conv_backward_tc(const float* x, const float* offset, const float
       dcn_gout_oc_tiles_kernel<<<d2b_cdiv(total, 256), 256, 0, stream>>>(grad_out, y_saved, ep, d, k3.BN, k3.noct, gt_oc);
       D2B_CHECK_LAUNCH();
     }
-    // output-channel tile fastest, then the unit pair: the CTAs that read one column (or gathered) tile and those that read one
-    // grad_out tile run in the same wave and share them in L2
-    const dim3 grid(d.SG * k3.noct, d.MC, k3.nsplit);
-    int rc;
-    if (cols) {  // the forward kept its sampled columns: stream them back (no second pass over x)
-      const int S = std::min(6, (kMaxSmem - 2048) / k3.stage_bytes);
-      const int smem_bytes = S * k3.stage_bytes + 1024 + 128;
-      const uint8_t* cl = reinterpret_cast<const uint8_t*>(cols);
-      rc = with_tile_width<64, 128>(k3.BN, [&](auto bn) {
-        return launch_big_smem<dcn_bwd_weight_cols_kernel<decltype(bn)::value>>(grid, smem_bytes, stream, cl, gt_oc, d, k3, S,
-                                                                                 P.split, gw_part);
-      });
-    } else {
-      const int smem_bytes = k3.S * k3.stage_bytes + 4096 + 1024 + 128;
-      rc = with_tile_width<64, 128>(k3.BN, [&](auto bn) {
-        return launch_big_smem<dcn_bwd_weight_tc_kernel<decltype(bn)::value>>(grid, smem_bytes, stream, xh, offset, mask, gt_oc,
-                                                                               d, k3, P.split, gw_part);
-      });
+    if (!fused) {  // (the fused launch ran the weight gradient's CTAs already)
+      // output-channel tile fastest, then the unit pair: the CTAs that read one column (or gathered) tile and those that read
+      // one grad_out tile run in the same wave and share them in L2
+      const dim3 grid(d.SG * k3.noct, d.MC, k3.nsplit);
+      int rc;
+      if (cols) {  // the forward kept its sampled columns: stream them back (no second pass over x)
+        rc = with_tile_width<64, 128>(k3.BN, [&](auto bn) {
+          return launch_big_smem<dcn_bwd_weight_cols_kernel<decltype(bn)::value>>(grid, smem3, stream, cl, gt_oc, d, k3, S3,
+                                                                                   P.split, gw_part);
+        });
+      } else {
+        const int smem_bytes = k3.S * k3.stage_bytes + 4096 + 1024 + 128;
+        rc = with_tile_width<64, 128>(k3.BN, [&](auto bn) {
+          return launch_big_smem<dcn_bwd_weight_tc_kernel<decltype(bn)::value>>(grid, smem_bytes, stream, xh, offset, mask,
+                                                                                 gt_oc, d, k3, P.split, gw_part);
+        });
+      }
+      if (rc) return rc;
     }
-    if (rc) return rc;
     if (d.KK <= 9) {  // d.ops is a multiple of 16 (shape gate)
       dcn_gw_reduce_tile_kernel<<<dim3(d.SG * (d.cps / kRedCh), d.ops / kRedOc), 256, 0, stream>>>(gw_part, d, grad_weight);
     } else {
