@@ -24,7 +24,7 @@ class DcnParams(C.Structure):
 
 MAX_LEVELS = 8
 MAX_IMAGES = 64  # D2B_MAX_IMAGES
-ABI_VERSION = 6  # include/d2b200.h D2B_ABI_VERSION
+ABI_VERSION = 7  # include/d2b200.h D2B_ABI_VERSION
 DCN_X_NHWC = 1   # D2B_DCN_X_NHWC
 ROI_ROTATED, ROI_BACKWARD, ROI_NHWC = 1, 2, 4  # D2B_ROI_ROTATED / D2B_ROI_BACKWARD / D2B_ROI_NHWC
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}  # D2B_F32 / D2B_F16 / D2B_BF16
@@ -54,13 +54,14 @@ class DenseLevels(C.Structure):
 LABELS_I8, LABELS_I64 = 0, 1  # D2B_LABELS_*
 SAMPLE_MAX_SAMPLES = 8192  # D2B_SAMPLE_MAX_SAMPLES
 LOSS_STATUS_INVALID_BOX, LOSS_STATUS_INVALID_CLASS, LOSS_STATUS_INVALID_BOX_ORDER = 1, 2, 4  # D2B_LOSS_STATUS_*
-LOSS_TYPES = {"smooth_l1": 0, "giou": 1}  # D2B_LOSS_SMOOTH_L1 / D2B_LOSS_GIOU
+LOSS_TYPES = {"smooth_l1": 0, "giou": 1}  # D2B_LOSS_SMOOTH_L1 / D2B_LOSS_GIOU: the box_reg_loss_type values with a kernel
+LOSS_LINEAR_GIOU = 2  # D2B_LOSS_LINEAR_GIOU: FCOS, dense only
 
 
 class DenseLossLevels(C.Structure):
     _fields_ = [("num_levels", C.c_int), ("logits", C.c_void_p * MAX_LEVELS), ("deltas", C.c_void_p * MAX_LEVELS),
                 ("grad_logits", C.c_void_p * MAX_LEVELS), ("grad_deltas", C.c_void_p * MAX_LEVELS),
-                ("R", C.c_int * MAX_LEVELS)]
+                ("ctr", C.c_void_p * MAX_LEVELS), ("grad_ctr", C.c_void_p * MAX_LEVELS), ("R", C.c_int * MAX_LEVELS)]
 
 
 class SemSegImages(C.Structure):
@@ -103,18 +104,14 @@ def _declare(lib):
         "d2b_keypoint_loss_backward": (i, [vp, i, i, i, i, i64p, u8p, f32p, vp, vp]),
         "d2b_dense_loss_workspace_bytes": (sz, [C.POINTER(DenseLossLevels), i, i, i]),
         "d2b_dense_loss_forward": (i, [C.POINTER(DenseLossLevels), i, i, i, i, f32p, f32p, vp, i, f, f, f, i, f,
-                                       C.POINTER(C.c_float), f32p, f32p, i64p, i64p, vp, vp, sz, vp]),
+                                       C.POINTER(C.c_float), f32p, i64p, vp, vp, sz, vp]),
         "d2b_dense_loss_backward": (i, [C.POINTER(DenseLossLevels), i, i, i, i, f32p, f32p, vp, i, f, f, f, i, f,
-                                        C.POINTER(C.c_float), f32p, f32p, vp]),
-        "d2b_fcos_loss_forward": (i, [C.POINTER(DenseLossLevels), C.POINTER(C.c_void_p), i, i, i, f32p, f32p, i64p, f, f, f32p,
-                                      f32p, f32p, i64p, vp, vp, sz, vp]),
-        "d2b_fcos_loss_backward": (i, [C.POINTER(DenseLossLevels), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), i, i, i,
-                                       f32p, f32p, i64p, f, f, f32p, f32p, f32p, vp]),
+                                        C.POINTER(C.c_float), f32p, vp]),
         "d2b_frcnn_loss_workspace_bytes": (sz, [i]),
-        "d2b_frcnn_loss_forward": (i, [vp, vp, i, i, i, i, i, f32p, f32p, i64p, f, i, f, C.POINTER(C.c_float), f32p, f32p, i64p,
-                                       i64p, i64p, i64p, vp, vp, sz, vp]),
-        "d2b_frcnn_loss_backward": (i, [vp, vp, i, i, i, i, i, f32p, f32p, i64p, f, i, f, C.POINTER(C.c_float), f32p, f32p, vp,
-                                        vp, vp]),
+        "d2b_frcnn_loss_forward": (i, [vp, vp, i, i, i, i, i, f32p, f32p, i64p, f, i, f, C.POINTER(C.c_float), f32p, i64p, vp,
+                                       vp, sz, vp]),
+        "d2b_frcnn_loss_backward": (i, [vp, vp, i, i, i, i, i, f32p, f32p, i64p, f, i, f, C.POINTER(C.c_float), f32p, vp, vp,
+                                        vp]),
         "d2b_box_iou_rotated": (i, [f32p, i64, f32p, i64, f32p, vp]),
         "d2b_match_workspace_bytes": (sz, [i, i, i]),
         "d2b_match_boxes": (i, [f32p, i64p, i, i, f32p, i64, i64p, i, C.POINTER(C.c_double), i, C.POINTER(C.c_int), i, f32p, d,

@@ -8,8 +8,9 @@
 //       Box2BoxTransform[Rotated].get_deltas computed on the fly.  One launch: classification CTAs stream the logits
 //       (16-byte vectors, the row label re-read only when the row changes), regression CTAs own one anchor row per
 //       thread; a second single-CTA launch adds the per-CTA partials in a fixed order.
-//   d2b_fcos_loss_forward / _backward    FCOS.losses + compute_ctrness_targets (meta_arch/fcos.py:193-251): the same kernel
-//       with kFcos -- GIoU of Box2BoxTransformLinear's decode and, on the positive rows, the centerness BCE as a third sum.
+//       With D2B_LOSS_LINEAR_GIOU they are FCOS.losses + compute_ctrness_targets (meta_arch/fcos.py:193-251): the same
+//       kernel with kFcos -- GIoU of Box2BoxTransformLinear's decode and, on the positive rows, the centerness BCE as a
+//       third sum.
 //   d2b_frcnn_loss_forward / _backward   FastRCNNOutputLayers.losses / box_reg_loss (roi_heads/fast_rcnn.py:307-352,
 //       424-463) and _log_classification_stats (:88-115): one warp per proposal row -- max, log-sum-exp, argmax, the class
 //       gather of the deltas, the targets and smooth-L1 -- then the same fixed-order finish.
@@ -220,12 +221,10 @@ __device__ __forceinline__ void block_partial(float s0, float s1, float s2, cons
   }
 }
 
-__global__ void __launch_bounds__(kThreads) finish_kernel(const Partial* __restrict__ part, int nparts,
-                                                          float* __restrict__ sum0, float* __restrict__ sum1,
-                                                          float* __restrict__ sum2,
-                                                          int64_t* __restrict__ c0, int64_t* __restrict__ c1,
-                                                          int64_t* __restrict__ c2, int64_t* __restrict__ c3,
-                                                          int* __restrict__ status) {
+// Adds the partials in a fixed order; writes sums[0, nsums), counts[0, ncounts) and status.
+__global__ void __launch_bounds__(kThreads) finish_kernel(const Partial* __restrict__ part, int nparts, int nsums,
+                                                          int ncounts, float* __restrict__ sums,
+                                                          int64_t* __restrict__ counts, int* __restrict__ status) {
   __shared__ double s_f[3][kThreads];
   __shared__ long long s_c[4][kThreads];
   __shared__ int s_s[kThreads];
@@ -261,13 +260,8 @@ __global__ void __launch_bounds__(kThreads) finish_kernel(const Partial* __restr
     __syncthreads();
   }
   if (tid == 0) {
-    *sum0 = (float)s_f[0][0];
-    *sum1 = (float)s_f[1][0];
-    if (sum2) *sum2 = (float)s_f[2][0];
-    if (c0) *c0 = s_c[0][0];
-    if (c1) *c1 = s_c[1][0];
-    if (c2) *c2 = s_c[2][0];
-    if (c3) *c3 = s_c[3][0];
+    for (int k = 0; k < nsums; ++k) sums[k] = (float)s_f[k][0];
+    for (int k = 0; k < ncounts; ++k) counts[k] = s_c[k][0];
     *status = s_s[0];
   }
 }
@@ -624,14 +618,15 @@ void launch_dense(long long blocks, const DenseLevels& P, const DenseArgs& A, cu
 }
 
 template <bool kBackward>
-int dense_dispatch(long long blocks, int dtype, int D, int label_kind, const DenseLevels& P, const DenseArgs& A,
-                   cudaStream_t st) {
-#define D2B_DENSE_CASE(DT)                                                                              \
-  if (dtype == DT) {                                                                                    \
-    if (D == 4 && label_kind == D2B_LABELS_I8) launch_dense<DT, XyxyBox, LabelsI8, kBackward>(blocks, P, A, st);   \
-    if (D == 4 && label_kind == D2B_LABELS_I64) launch_dense<DT, XyxyBox, LabelsI64, kBackward>(blocks, P, A, st); \
-    if (D == 5 && label_kind == D2B_LABELS_I8) launch_dense<DT, RotBox, LabelsI8, kBackward>(blocks, P, A, st);    \
-    if (D == 5 && label_kind == D2B_LABELS_I64) launch_dense<DT, RotBox, LabelsI64, kBackward>(blocks, P, A, st);  \
+int dense_dispatch(long long blocks, int dtype, int D, int label_kind, int loss_type, const DenseLevels& P,
+                   const DenseArgs& A, cudaStream_t st) {
+#define D2B_DENSE_CASE(DT)                                                                                              \
+  if (dtype == DT) {                                                                                                    \
+    if (loss_type == D2B_LOSS_LINEAR_GIOU) launch_dense<DT, XyxyBox, LabelsI64, kBackward, true>(blocks, P, A, st);     \
+    else if (D == 4 && label_kind == D2B_LABELS_I8) launch_dense<DT, XyxyBox, LabelsI8, kBackward>(blocks, P, A, st);   \
+    else if (D == 4 && label_kind == D2B_LABELS_I64) launch_dense<DT, XyxyBox, LabelsI64, kBackward>(blocks, P, A, st); \
+    else if (D == 5 && label_kind == D2B_LABELS_I8) launch_dense<DT, RotBox, LabelsI8, kBackward>(blocks, P, A, st);    \
+    else if (D == 5 && label_kind == D2B_LABELS_I64) launch_dense<DT, RotBox, LabelsI64, kBackward>(blocks, P, A, st);  \
   }
   D2B_DENSE_CASE(D2B_F32)
   D2B_DENSE_CASE(D2B_F16)
@@ -646,13 +641,21 @@ int dense_setup(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int 
                 const float* gt_boxes, const void* labels, int label_kind, float gamma, float alpha, float beta,
                 int loss_type, float scale_clamp, const float* weights, bool backward, DenseLevels& P, DenseArgs& A,
                 long long& blocks) {
-  if (N < 0 || K <= 0 || (box_dim != 4 && box_dim != 5) || !valid_dtype(dtype) || !weights) return D2B_EINVAL;
+  const bool linear = loss_type == D2B_LOSS_LINEAR_GIOU;  // FCOS: no Box2BoxTransform weights, a centerness per level
+  if (N < 0 || K <= 0 || (box_dim != 4 && box_dim != 5) || !valid_dtype(dtype) || (!weights && !linear))
+    return D2B_EINVAL;
   if (label_kind != D2B_LABELS_I8 && label_kind != D2B_LABELS_I64) return D2B_EINVAL;
   if (label_kind == D2B_LABELS_I8 && K != 1) return D2B_EINVAL;
   if (!(gamma >= 0.f) || !(beta >= 0.f) || alpha != alpha) return D2B_EINVAL;
-  if (!loss_type_ok(loss_type, box_dim)) return D2B_EINVAL;
+  if (linear ? box_dim != 4 || label_kind != D2B_LABELS_I64 : !loss_type_ok(loss_type, box_dim)) return D2B_EINVAL;
   const long long cls_blocks = dense_levels(lv, N, K, dtype, backward, P);
   if (cls_blocks < 0) return D2B_EINVAL;
+  for (int l = 0; l < P.L; ++l) {
+    if (!linear && (lv->ctr[l] || lv->grad_ctr[l])) return D2B_EINVAL;
+    if (linear && (long long)N * P.R[l] > 0 && (!lv->ctr[l] || (backward && !lv->grad_ctr[l]))) return D2B_EINVAL;
+    P.ctr[l] = lv->ctr[l];
+    P.grad_ctr[l] = lv->grad_ctr[l];
+  }
   const int Rtot = P.a0[P.L];
   if ((long long)N * Rtot > 0 && (!anchors || !gt_boxes || !labels)) return D2B_EINVAL;
   blocks = cls_blocks + dense_reg_blocks(N, Rtot);
@@ -668,36 +671,9 @@ int dense_setup(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int 
   A.gamma = gamma;
   A.alpha = alpha;
   A.beta = beta;
-  A.giou = loss_type == D2B_LOSS_GIOU;
+  A.giou = loss_type == D2B_LOSS_GIOU || linear;  // decoded boxes, no get_deltas targets: no width assertion
   A.scale_clamp = scale_clamp;
-  A.w = box_weights(weights, box_dim);
-  return D2B_OK;
-}
-
-// FCOS: the dense rules with xyxy anchors, int64 labels and the GIoU flag, plus the per-level centerness logits.
-int fcos_setup(const d2b_dense_loss_levels* lv, const void* const* ctr, void* const* grad_ctr, int N, int K, int dtype,
-               const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma, float alpha, bool backward,
-               DenseLevels& P, DenseArgs& A, long long& blocks) {
-  const float ones[4] = {1.f, 1.f, 1.f, 1.f};
-  const int rc = dense_setup(lv, N, K, 4, dtype, anchors, gt_boxes, labels, D2B_LABELS_I64, gamma, alpha, 0.f,
-                             D2B_LOSS_GIOU, 0.f, ones, backward, P, A, blocks);
-  if (rc) return rc;
-  if (!ctr || (backward && !grad_ctr)) return D2B_EINVAL;
-  for (int l = 0; l < P.L; ++l) {
-    const bool some = (long long)N * P.R[l] > 0;
-    if (some && (!ctr[l] || (backward && !grad_ctr[l]))) return D2B_EINVAL;
-    P.ctr[l] = ctr[l];
-    P.grad_ctr[l] = backward ? grad_ctr[l] : nullptr;
-  }
-  return D2B_OK;
-}
-
-template <bool kBackward>
-int fcos_dispatch(long long blocks, int dtype, const DenseLevels& P, const DenseArgs& A, cudaStream_t st) {
-  if (dtype == D2B_F32) launch_dense<D2B_F32, XyxyBox, LabelsI64, kBackward, true>(blocks, P, A, st);
-  if (dtype == D2B_F16) launch_dense<D2B_F16, XyxyBox, LabelsI64, kBackward, true>(blocks, P, A, st);
-  if (dtype == D2B_BF16) launch_dense<D2B_BF16, XyxyBox, LabelsI64, kBackward, true>(blocks, P, A, st);
-  D2B_CHECK_LAUNCH();
+  if (!linear) A.w = box_weights(weights, box_dim);
   return D2B_OK;
 }
 
@@ -753,8 +729,7 @@ D2B_API size_t d2b_dense_loss_workspace_bytes(const d2b_dense_loss_levels* lv, i
 D2B_API int d2b_dense_loss_forward(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int dtype,
                                    const float* anchors, const float* gt_boxes, const void* labels, int label_kind,
                                    float gamma, float alpha, float beta, int loss_type, float scale_clamp,
-                                   const float* weights, float* cls_sum,
-                                   float* reg_sum, int64_t* num_pos, int64_t* num_neg, int* status, void* workspace,
+                                   const float* weights, float* sums, int64_t* counts, int* status, void* workspace,
                                    size_t workspace_bytes, void* stream) {
   DenseLevels P;
   DenseArgs A;
@@ -762,17 +737,16 @@ D2B_API int d2b_dense_loss_forward(const d2b_dense_loss_levels* lv, int N, int K
   const int rc = dense_setup(lv, N, K, box_dim, dtype, anchors, gt_boxes, labels, label_kind, gamma, alpha, beta,
                              loss_type, scale_clamp, weights, false, P, A, blocks);
   if (rc) return rc;
-  if (!cls_sum || !reg_sum || !num_pos || !num_neg || !status) return D2B_EINVAL;
+  if (!sums || !counts || !status) return D2B_EINVAL;
   if (blocks > 0 && (!workspace || !aligned16(workspace))) return D2B_EINVAL;
   if (workspace_bytes < (size_t)blocks * sizeof(Partial)) return D2B_EWORKSPACE;
   const cudaStream_t st = (cudaStream_t)stream;
   A.part = (Partial*)workspace;
   if (blocks > 0) {
-    const int e = dense_dispatch<false>(blocks, dtype, box_dim, label_kind, P, A, st);
+    const int e = dense_dispatch<false>(blocks, dtype, box_dim, label_kind, loss_type, P, A, st);
     if (e) return e;
   }
-  finish_kernel<<<1, kThreads, 0, st>>>(A.part, (int)blocks, cls_sum, reg_sum, nullptr, num_pos, num_neg, nullptr, nullptr,
-                                        status);
+  finish_kernel<<<1, kThreads, 0, st>>>(A.part, (int)blocks, 3, 2, sums, counts, status);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }
@@ -780,60 +754,19 @@ D2B_API int d2b_dense_loss_forward(const d2b_dense_loss_levels* lv, int N, int K
 D2B_API int d2b_dense_loss_backward(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int dtype,
                                     const float* anchors, const float* gt_boxes, const void* labels, int label_kind,
                                     float gamma, float alpha, float beta, int loss_type, float scale_clamp,
-                                    const float* weights, const float* grad_cls,
-                                    const float* grad_reg, void* stream) {
+                                    const float* weights, const float* grad_sums, void* stream) {
   DenseLevels P;
   DenseArgs A;
   long long blocks = 0;
   const int rc = dense_setup(lv, N, K, box_dim, dtype, anchors, gt_boxes, labels, label_kind, gamma, alpha, beta,
                              loss_type, scale_clamp, weights, true, P, A, blocks);
   if (rc) return rc;
-  if (!grad_cls || !grad_reg) return D2B_EINVAL;
+  if (!grad_sums) return D2B_EINVAL;
   if (blocks == 0) return D2B_OK;
-  A.grad_cls = grad_cls;
-  A.grad_reg = grad_reg;
-  return dense_dispatch<true>(blocks, dtype, box_dim, label_kind, P, A, (cudaStream_t)stream);
-}
-
-D2B_API int d2b_fcos_loss_forward(const d2b_dense_loss_levels* lv, const void* const* ctr, int N, int K, int dtype,
-                                  const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma,
-                                  float alpha, float* cls_sum, float* reg_sum, float* ctr_sum, int64_t* num_pos,
-                                  int* status, void* workspace, size_t workspace_bytes, void* stream) {
-  DenseLevels P;
-  DenseArgs A;
-  long long blocks = 0;
-  const int rc = fcos_setup(lv, ctr, nullptr, N, K, dtype, anchors, gt_boxes, labels, gamma, alpha, false, P, A, blocks);
-  if (rc) return rc;
-  if (!cls_sum || !reg_sum || !ctr_sum || !num_pos || !status) return D2B_EINVAL;
-  if (blocks > 0 && (!workspace || !aligned16(workspace))) return D2B_EINVAL;
-  if (workspace_bytes < (size_t)blocks * sizeof(Partial)) return D2B_EWORKSPACE;
-  const cudaStream_t st = (cudaStream_t)stream;
-  A.part = (Partial*)workspace;
-  if (blocks > 0) {
-    const int e = fcos_dispatch<false>(blocks, dtype, P, A, st);
-    if (e) return e;
-  }
-  finish_kernel<<<1, kThreads, 0, st>>>(A.part, (int)blocks, cls_sum, reg_sum, ctr_sum, num_pos, nullptr, nullptr, nullptr,
-                                        status);
-  D2B_CHECK_LAUNCH();
-  return D2B_OK;
-}
-
-D2B_API int d2b_fcos_loss_backward(const d2b_dense_loss_levels* lv, const void* const* ctr, void* const* grad_ctr, int N,
-                                   int K, int dtype, const float* anchors, const float* gt_boxes, const int64_t* labels,
-                                   float gamma, float alpha, const float* grad_cls, const float* grad_reg,
-                                   const float* grad_ctr_sum, void* stream) {
-  DenseLevels P;
-  DenseArgs A;
-  long long blocks = 0;
-  const int rc = fcos_setup(lv, ctr, grad_ctr, N, K, dtype, anchors, gt_boxes, labels, gamma, alpha, true, P, A, blocks);
-  if (rc) return rc;
-  if (!grad_cls || !grad_reg || !grad_ctr_sum) return D2B_EINVAL;
-  if (blocks == 0) return D2B_OK;
-  A.grad_cls = grad_cls;
-  A.grad_reg = grad_reg;
-  A.grad_ctr = grad_ctr_sum;
-  return fcos_dispatch<true>(blocks, dtype, P, A, (cudaStream_t)stream);
+  A.grad_cls = grad_sums;
+  A.grad_reg = grad_sums + 1;
+  A.grad_ctr = grad_sums + 2;
+  return dense_dispatch<true>(blocks, dtype, box_dim, label_kind, loss_type, P, A, (cudaStream_t)stream);
 }
 
 D2B_API size_t d2b_frcnn_loss_workspace_bytes(int R) {
@@ -842,15 +775,13 @@ D2B_API size_t d2b_frcnn_loss_workspace_bytes(int R) {
 
 D2B_API int d2b_frcnn_loss_forward(const void* scores, const void* deltas, int R, int K, int kreg, int box_dim, int dtype,
                                    const float* proposals, const float* gt_boxes, const int64_t* gt_classes, float beta,
-                                   int loss_type, float scale_clamp, const float* weights, float* cls_sum, float* reg_sum, int64_t* num_fg,
-                                   int64_t* num_accurate, int64_t* fg_num_accurate, int64_t* num_false_negative,
+                                   int loss_type, float scale_clamp, const float* weights, float* sums, int64_t* counts,
                                    int* status, void* workspace, size_t workspace_bytes, void* stream) {
   FrcnnArgs A;
   const int rc = frcnn_setup(R, K, kreg, box_dim, dtype, scores, deltas, proposals, gt_boxes, gt_classes, beta, loss_type,
                              scale_clamp, weights, A);
   if (rc) return rc;
-  if (!cls_sum || !reg_sum || !num_fg || !num_accurate || !fg_num_accurate || !num_false_negative || !status)
-    return D2B_EINVAL;
+  if (!sums || !counts || !status) return D2B_EINVAL;
   if (R > 0 && (!workspace || !aligned16(workspace))) return D2B_EINVAL;
   if (workspace_bytes < d2b_frcnn_loss_workspace_bytes(R)) return D2B_EWORKSPACE;
   const cudaStream_t st = (cudaStream_t)stream;
@@ -859,8 +790,7 @@ D2B_API int d2b_frcnn_loss_forward(const void* scores, const void* deltas, int R
     const int e = frcnn_dispatch<false>(dtype, box_dim, A, st);
     if (e) return e;
   }
-  finish_kernel<<<1, kThreads, 0, st>>>(A.part, d2b_cdiv(R, kWarps), cls_sum, reg_sum, nullptr, num_fg, num_accurate,
-                                        fg_num_accurate, num_false_negative, status);
+  finish_kernel<<<1, kThreads, 0, st>>>(A.part, d2b_cdiv(R, kWarps), 2, 4, sums, counts, status);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }
@@ -868,16 +798,15 @@ D2B_API int d2b_frcnn_loss_forward(const void* scores, const void* deltas, int R
 D2B_API int d2b_frcnn_loss_backward(const void* scores, const void* deltas, int R, int K, int kreg, int box_dim,
                                     int dtype, const float* proposals, const float* gt_boxes, const int64_t* gt_classes,
                                     float beta, int loss_type, float scale_clamp, const float* weights,
-                                    const float* grad_cls, const float* grad_reg,
-                                    void* grad_scores, void* grad_deltas, void* stream) {
+                                    const float* grad_sums, void* grad_scores, void* grad_deltas, void* stream) {
   FrcnnArgs A;
   const int rc = frcnn_setup(R, K, kreg, box_dim, dtype, scores, deltas, proposals, gt_boxes, gt_classes, beta, loss_type,
                              scale_clamp, weights, A);
   if (rc) return rc;
   if (R == 0) return D2B_OK;
-  if (!grad_cls || !grad_reg || !grad_scores || !grad_deltas) return D2B_EINVAL;
-  A.grad_cls = grad_cls;
-  A.grad_reg = grad_reg;
+  if (!grad_sums || !grad_scores || !grad_deltas) return D2B_EINVAL;
+  A.grad_cls = grad_sums;
+  A.grad_reg = grad_sums + 1;
   A.grad_scores = grad_scores;
   A.grad_deltas = grad_deltas;
   return frcnn_dispatch<true>(dtype, box_dim, A, (cudaStream_t)stream);

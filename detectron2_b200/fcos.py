@@ -5,7 +5,7 @@
     images in one launch (one thread per point, the GT boxes staged in shared memory); the reference builds several
     [G, R, 4] tensors per image.
   * `fcos_losses_fixed` / `fcos_losses` -- FCOS.losses + compute_ctrness_targets (fcos.py:193-251): the focal loss, the
-    GIoU of Box2BoxTransformLinear's decode and the centerness BCE, on the dense loss kernel (`d2b200::fcos_loss`), read in
+    GIoU of Box2BoxTransformLinear's decode and the centerness BCE, on the dense loss kernel (`d2b200::dense_loss`), read in
     place from the per-level predictions, normalised by the EMA of the positive count (initial value 300).
   * `fcos_inference_fixed` / `fcos_inference` -- FCOS.forward_inference (fcos.py:253-301): scores
     sqrt(sigmoid(logits) * sigmoid(centerness)) by torch's elementwise ops, then RetinaNet's batched selection
@@ -25,7 +25,7 @@ from torch.nn import functional as F
 from . import _C
 from ._C import check, ptr, stream_ptr
 from .dense_inference import apply_deltas_linear, dense_detector_inference, dense_detector_inference_fixed
-from .losses import _giou_loss, _raise_status, _sigmoid_focal_loss, _stack, fcos_loss_op
+from .losses import _ema_update, _giou_loss, _raise_status, _sigmoid_focal_loss, _stack, dense_loss_op
 from .matching import _pad
 
 Tensor = torch.Tensor
@@ -113,16 +113,14 @@ def fcos_losses_fixed(anchors, pred_logits: List[Tensor], gt_labels, pred_anchor
     gt_labels [N, R] int64 and gt_boxes [N, R, 4] (fcos_label_anchors_fixed's).  loss_normalizer: caller-held fp64 [1]
     tensor holding the EMA of DenseDetector._ema_update (set it to 300 before the first call); it is updated in place as
     retinanet_losses_fixed's.  Returns (losses {"loss_fcos_cls", "loss_fcos_loc", "loss_fcos_ctr"}, num_pos, status)."""
-    if loss_normalizer.dtype != torch.float64 or loss_normalizer.numel() != 1:
-        raise ValueError("fcos_losses_fixed: loss_normalizer must be a float64 tensor with one element")
     an = anchors if isinstance(anchors, Tensor) else torch.cat(list(anchors), dim=0)
-    cls, reg, ctr, num_pos, status = fcos_loss_op(list(pred_logits), list(pred_anchor_deltas), list(pred_centerness), an,
-                                                  _stack(gt_boxes), _stack(gt_labels), int(num_classes),
-                                                  float(focal_loss_gamma), float(focal_loss_alpha))
-    momentum = 0.9
-    loss_normalizer.copy_(loss_normalizer * momentum + num_pos.clamp(min=1).to(torch.float64) * (1 - momentum))
-    inv = torch.reciprocal(loss_normalizer.reshape(()).to(torch.float32))
-    return {"loss_fcos_cls": cls * inv, "loss_fcos_loc": reg * inv, "loss_fcos_ctr": ctr * inv}, num_pos, status
+    sums, counts, status = dense_loss_op(list(pred_logits), list(pred_anchor_deltas), list(pred_centerness), an,
+                                         _stack(gt_boxes), _stack(gt_labels), int(num_classes), False,
+                                         float(focal_loss_gamma), float(focal_loss_alpha), 0.0, _C.LOSS_LINEAR_GIOU,
+                                         0.0, None)
+    num_pos, _ = counts.unbind(0)
+    cls, reg, ctr = (sums * _ema_update(loss_normalizer, num_pos, "fcos_losses_fixed")).unbind(0)
+    return {"loss_fcos_cls": cls, "loss_fcos_loc": reg, "loss_fcos_ctr": ctr}, num_pos, status
 
 
 def fcos_losses(anchors, pred_logits: List[Tensor], gt_labels: List[Tensor], pred_anchor_deltas: List[Tensor],

@@ -6,8 +6,8 @@
     over the valid anchors plus box regression, normalised by the EMA of the positive count (DenseDetector._ema_update).
   * `fast_rcnn_losses` / `fast_rcnn_losses_fixed` -- FastRCNNOutputLayers.losses / box_reg_loss and
     _log_classification_stats (roi_heads/fast_rcnn.py:88-115, 307-352, 424-463), for the standard, cascade and rotated heads.
-  * `fcos_loss_op` -- FCOS.losses (meta_arch/fcos.py:193-251) on the dense kernel with the linear GIoU and the centerness
-    term; its Python surface is detectron2_b200/fcos.py.
+  * FCOS.losses (meta_arch/fcos.py:193-251) is `dense_loss_op` with `LOSS_LINEAR_GIOU` and the centerness logits: the
+    GIoU of the linear decode plus the centerness term; its Python surface is detectron2_b200/fcos.py.
 
 The reference concatenates the levels, gathers the valid rows behind a boolean mask, builds an int64 one-hot target and
 reads the host about ten times per step (.item() counts, get_deltas' assertion, nonzero).  Here `d2b_dense_loss_*` reads the
@@ -35,7 +35,7 @@ from .dense_inference import apply_deltas as _apply_deltas
 Tensor = torch.Tensor
 
 __all__ = ["rpn_losses", "rpn_losses_fixed", "retinanet_losses", "retinanet_losses_fixed", "fast_rcnn_losses",
-           "fast_rcnn_losses_fixed", "dense_loss_op", "frcnn_loss_op", "fcos_loss_op"]
+           "fast_rcnn_losses_fixed", "dense_loss_op", "frcnn_loss_op"]
 
 _SCALE_CLAMP = 4.135166556742356  # math.log(1000.0 / 16), box_regression.py:14
 
@@ -51,13 +51,16 @@ def _pred_dtype(t: Tensor) -> torch.dtype:
     return t.dtype if t.dtype in _C.DTYPE_CODE else torch.float32
 
 
-def _c_weights(weights: Sequence[float]):
-    return (C.c_float * len(weights))(*[float(w) for w in weights])
+def _c_weights(weights: Optional[Sequence[float]]):
+    """The HOST weights array, or NULL for None (D2B_LOSS_LINEAR_GIOU reads no weights)."""
+    return None if weights is None else (C.c_float * len(weights))(*[float(w) for w in weights])
 
 
-def _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, rpn):
+def _dense_prepare(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, rpn):
     if len(logits) == 0 or len(logits) != len(deltas) or len(logits) > _C.MAX_LEVELS:
         raise ValueError("dense_loss: 1 to %d levels of logits and deltas" % _C.MAX_LEVELS)
+    if len(ctr) not in (0, len(logits)):
+        raise ValueError("dense_loss: no centerness, or one centerness tensor per level")
     dt = _pred_dtype(logits[0])
     xs = [_pred(x, dt) for x in logits]
     ds = [_pred(d, dt) for d in deltas]
@@ -65,37 +68,47 @@ def _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, rpn):
     for x, dl in zip(xs, ds):
         if x.dim() != 3 or x.shape[0] != n or x.shape[2] != num_classes or dl.shape != (n, x.shape[1], d):
             raise ValueError("dense_loss: logits must be [N, R_l, K] and deltas [N, R_l, %d]" % d)
+    cs = []
+    for c, x in zip(ctr, xs):
+        if c.shape not in ((n, x.shape[1]), (n, x.shape[1], 1)):
+            raise ValueError("dense_loss: centerness must be [N, R_l] or [N, R_l, 1]")
+        cs.append(c.reshape(n, x.shape[1]).to(dt).contiguous())
     r = sum(int(x.shape[1]) for x in xs)
     if anchors.shape != (r, d) or gt_boxes.shape != (n, r, d) or labels.shape != (n, r):
         raise ValueError("dense_loss: anchors [R, D], gt_boxes [N, R, D] and labels [N, R] with R = sum of R_l")
     lab = labels.to(torch.int8 if rpn else torch.int64).contiguous()
-    return dt, xs, ds, anchors.float().contiguous(), gt_boxes.float().contiguous(), lab
+    return dt, xs, ds, cs, anchors.float().contiguous(), gt_boxes.float().contiguous(), lab
 
 
-def _dense_levels(xs, ds, gxs=None, gds=None):
+def _dense_levels(xs, ds, cs, gxs=None, gds=None, gcs=None):
     lv = _C.DenseLossLevels()
     lv.num_levels = len(xs)
     for l, (x, d) in enumerate(zip(xs, ds)):
         lv.logits[l], lv.deltas[l], lv.R[l] = x.data_ptr(), d.data_ptr(), int(x.shape[1])
         if gxs is not None:
             lv.grad_logits[l], lv.grad_deltas[l] = gxs[l].data_ptr(), gds[l].data_ptr()
+    for l, c in enumerate(cs):
+        lv.ctr[l] = c.data_ptr()
+        if gcs is not None:
+            lv.grad_ctr[l] = gcs[l].data_ptr()
     return lv
 
 
 @torch.library.custom_op("d2b200::dense_loss", mutates_args=(), device_types="cuda")
-def dense_loss_op(logits: List[Tensor], deltas: List[Tensor], anchors: Tensor, gt_boxes: Tensor, labels: Tensor,
-                  num_classes: int, rpn: bool, gamma: float, alpha: float, beta: float, loss_type: int,
-                  scale_clamp: float, weights: List[float]) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+def dense_loss_op(logits: List[Tensor], deltas: List[Tensor], ctr: List[Tensor], anchors: Tensor, gt_boxes: Tensor,
+                  labels: Tensor, num_classes: int, rpn: bool, gamma: float, alpha: float, beta: float, loss_type: int,
+                  scale_clamp: float, weights: Optional[List[float]]) -> Tuple[Tensor, Tensor, Tensor]:
     """Per level logits [N, R_l, K] and deltas [N, R_l, D] (fp32 / fp16 / bf16), anchors [R, D], matched gt_boxes
-    [N, R, D], labels [N, R] (rpn: int8 {-1, 0, 1} and K = 1; else int64 classes with K = background).
-    Returns (cls_sum, reg_sum, num_pos, num_neg, status) as 0-dim device tensors (fp32, fp32, int64, int64, int32)."""
-    _C.require_cuda(anchors, gt_boxes, labels, *logits, *deltas)
-    dt, xs, ds, an, gt, lab = _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, rpn)
+    [N, R, D], labels [N, R] (rpn: int8 {-1, 0, 1} and K = 1; else int64 classes with K = background).  ctr: empty, or
+    with loss_type LOSS_LINEAR_GIOU (FCOS; weights None) the centerness logits [N, R_l] or [N, R_l, 1] of every level.
+    Returns (sums [3] fp32: classification, regression, centerness; counts [2] int64: num_pos, num_neg; status [] int32)."""
+    _C.require_cuda(anchors, gt_boxes, labels, *logits, *deltas, *ctr)
+    dt, xs, ds, cs, an, gt, lab = _dense_prepare(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, rpn)
     dev = an.device
     n, d = gt.shape[0], an.shape[-1]
-    lv = _dense_levels(xs, ds)
-    cls_sum, reg_sum = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(2))
-    num_pos, num_neg = (torch.empty((), dtype=torch.int64, device=dev) for _ in range(2))
+    lv = _dense_levels(xs, ds, cs)
+    sums = torch.empty((3,), dtype=torch.float32, device=dev)
+    counts = torch.empty((2,), dtype=torch.int64, device=dev)
     status = torch.empty((), dtype=torch.int32, device=dev)
     lib = _C.lib()
     code = _C.DTYPE_CODE[dt]
@@ -104,157 +117,62 @@ def dense_loss_op(logits: List[Tensor], deltas: List[Tensor], anchors: Tensor, g
     with torch.cuda.device(dev):
         check(lib.d2b_dense_loss_forward(C.byref(lv), n, num_classes, d, code, ptr(an), ptr(gt), ptr(lab),
                                          _C.LABELS_I8 if rpn else _C.LABELS_I64, float(gamma), float(alpha), float(beta),
-                                         int(loss_type), float(scale_clamp), _c_weights(weights), ptr(cls_sum),
-                                         ptr(reg_sum), ptr(num_pos), ptr(num_neg), ptr(status), ptr(ws), ws_bytes, stream_ptr(dev)), "dense_loss_forward")
-    return cls_sum, reg_sum, num_pos, num_neg, status
+                                         int(loss_type), float(scale_clamp), _c_weights(weights), ptr(sums), ptr(counts),
+                                         ptr(status), ptr(ws), ws_bytes, stream_ptr(dev)), "dense_loss_forward")
+    return sums, counts, status
 
 
 @dense_loss_op.register_fake
-def _(logits, deltas, anchors, gt_boxes, labels, num_classes, rpn, gamma, alpha, beta, loss_type, scale_clamp, weights):
+def _(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, rpn, gamma, alpha, beta, loss_type, scale_clamp,
+      weights):
     e = anchors.new_empty
-    return (e((), dtype=torch.float32), e((), dtype=torch.float32), e((), dtype=torch.int64), e((), dtype=torch.int64),
-            e((), dtype=torch.int32))
+    return e((3,), dtype=torch.float32), e((2,), dtype=torch.int64), e((), dtype=torch.int32)
 
 
 @torch.library.custom_op("d2b200::dense_loss_backward", mutates_args=(), device_types="cuda")
-def dense_loss_backward_op(logits: List[Tensor], deltas: List[Tensor], anchors: Tensor, gt_boxes: Tensor, labels: Tensor,
-                           num_classes: int, rpn: bool, gamma: float, alpha: float, beta: float, loss_type: int,
-                           scale_clamp: float, weights: List[float], grad_cls: Tensor, grad_reg: Tensor) -> List[Tensor]:
-    """Gradients of every level's logits, then of every level's deltas, in the inputs' dtypes."""
-    dt, xs, ds, an, gt, lab = _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, rpn)
+def dense_loss_backward_op(logits: List[Tensor], deltas: List[Tensor], ctr: List[Tensor], anchors: Tensor,
+                           gt_boxes: Tensor, labels: Tensor, num_classes: int, rpn: bool, gamma: float, alpha: float,
+                           beta: float, loss_type: int, scale_clamp: float, weights: Optional[List[float]],
+                           grad_sums: Tensor) -> List[Tensor]:
+    """Gradients of every level's logits, then deltas, then centerness logits, in the inputs' dtypes and shapes."""
+    dt, xs, ds, cs, an, gt, lab = _dense_prepare(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, rpn)
     dev = an.device
-    gxs = [torch.empty_like(x) for x in xs]
-    gds = [torch.empty_like(x) for x in ds]
-    lv = _dense_levels(xs, ds, gxs, gds)
-    gc = grad_cls.to(torch.float32).reshape(()).contiguous()
-    gr = grad_reg.to(torch.float32).reshape(()).contiguous()
+    gxs, gds, gcs = ([torch.empty_like(t) for t in ts] for ts in (xs, ds, cs))
+    lv = _dense_levels(xs, ds, cs, gxs, gds, gcs)
+    g = grad_sums.to(torch.float32).contiguous()
     with torch.cuda.device(dev):
         check(_C.lib().d2b_dense_loss_backward(C.byref(lv), gt.shape[0], num_classes, an.shape[-1], _C.DTYPE_CODE[dt],
                                                ptr(an), ptr(gt), ptr(lab), _C.LABELS_I8 if rpn else _C.LABELS_I64,
                                                float(gamma), float(alpha), float(beta), int(loss_type),
-                                               float(scale_clamp), _c_weights(weights), ptr(gc),
-                                               ptr(gr), stream_ptr(dev)), "dense_loss_backward")
-    return [g.to(x.dtype) for g, x in zip(gxs + gds, list(logits) + list(deltas))]
-
-
-@dense_loss_backward_op.register_fake
-def _(logits, deltas, anchors, gt_boxes, labels, num_classes, rpn, gamma, alpha, beta, loss_type, scale_clamp, weights,
-      grad_cls, grad_reg):
-    return [torch.empty_like(t) for t in list(logits) + list(deltas)]
-
-
-def _dense_setup(ctx, inputs, output):
-    logits, deltas, anchors, gt_boxes, labels = inputs[:5]
-    ctx.save_for_backward(*logits, *deltas, anchors, gt_boxes, labels)
-    ctx.num_levels = len(logits)
-    ctx.params = inputs[5:]
-
-
-def _dense_bwd(ctx, g_cls, g_reg, *_):
-    saved = ctx.saved_tensors
-    nl = ctx.num_levels
-    logits, deltas = list(saved[:nl]), list(saved[nl:2 * nl])
-    anchors, gt_boxes, labels = saved[2 * nl:]
-    grads = dense_loss_backward_op(logits, deltas, anchors, gt_boxes, labels, *ctx.params, g_cls, g_reg)
-    return (grads[:nl], grads[nl:]) + (None,) * 11
-
-
-dense_loss_op.register_autograd(_dense_bwd, setup_context=_dense_setup)
-
-
-def _fcos_ctr(ctr: List[Tensor], logits: List[Tensor], dt: torch.dtype) -> List[Tensor]:
-    """Centerness logits [N, R_l] (or [N, R_l, 1]) of the logits' dtype, contiguous."""
-    if len(ctr) != len(logits):
-        raise ValueError("fcos_loss: one centerness tensor per level")
-    out = []
-    for c, x in zip(ctr, logits):
-        if c.shape not in ((x.shape[0], x.shape[1]), (x.shape[0], x.shape[1], 1)):
-            raise ValueError("fcos_loss: centerness must be [N, R_l] or [N, R_l, 1]")
-        out.append(c.reshape(x.shape[0], x.shape[1]).to(dt).contiguous())
-    return out
-
-
-def _ptr_array(ts: List[Tensor]):
-    return (C.c_void_p * max(len(ts), 1))(*[t.data_ptr() for t in ts])
-
-
-@torch.library.custom_op("d2b200::fcos_loss", mutates_args=(), device_types="cuda")
-def fcos_loss_op(logits: List[Tensor], deltas: List[Tensor], ctr: List[Tensor], anchors: Tensor, gt_boxes: Tensor,
-                 labels: Tensor, num_classes: int, gamma: float, alpha: float
-                 ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
-    """FCOS.losses on the dense kernel: per level logits [N, R_l, K], deltas [N, R_l, 4] and centerness logits [N, R_l]
-    (fp32 / fp16 / bf16), anchors [R, 4], matched gt_boxes [N, R, 4], labels [N, R] int64 (K = background, -1 ignored).
-    Returns (cls_sum, reg_sum, ctr_sum, num_pos, status) as 0-dim device tensors (fp32 x3, int64, int32)."""
-    _C.require_cuda(anchors, gt_boxes, labels, *logits, *deltas, *ctr)
-    dt, xs, ds, an, gt, lab = _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, False)
-    cs = _fcos_ctr(ctr, xs, dt)
-    dev = an.device
-    n = gt.shape[0]
-    lv = _dense_levels(xs, ds)
-    cls_sum, reg_sum, ctr_sum = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(3))
-    num_pos = torch.empty((), dtype=torch.int64, device=dev)
-    status = torch.empty((), dtype=torch.int32, device=dev)
-    lib = _C.lib()
-    code = _C.DTYPE_CODE[dt]
-    ws_bytes = int(lib.d2b_dense_loss_workspace_bytes(C.byref(lv), n, num_classes, code))
-    ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        check(lib.d2b_fcos_loss_forward(C.byref(lv), _ptr_array(cs), n, num_classes, code, ptr(an), ptr(gt), ptr(lab),
-                                        float(gamma), float(alpha), ptr(cls_sum), ptr(reg_sum), ptr(ctr_sum), ptr(num_pos),
-                                        ptr(status), ptr(ws), ws_bytes, stream_ptr(dev)), "fcos_loss_forward")
-    return cls_sum, reg_sum, ctr_sum, num_pos, status
-
-
-@fcos_loss_op.register_fake
-def _(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, gamma, alpha):
-    e = anchors.new_empty
-    return (e((), dtype=torch.float32), e((), dtype=torch.float32), e((), dtype=torch.float32), e((), dtype=torch.int64),
-            e((), dtype=torch.int32))
-
-
-@torch.library.custom_op("d2b200::fcos_loss_backward", mutates_args=(), device_types="cuda")
-def fcos_loss_backward_op(logits: List[Tensor], deltas: List[Tensor], ctr: List[Tensor], anchors: Tensor, gt_boxes: Tensor,
-                          labels: Tensor, num_classes: int, gamma: float, alpha: float, grad_cls: Tensor,
-                          grad_reg: Tensor, grad_ctr: Tensor) -> List[Tensor]:
-    """Gradients of every level's logits, then deltas, then centerness logits, in the inputs' dtypes and shapes."""
-    dt, xs, ds, an, gt, lab = _dense_prepare(logits, deltas, anchors, gt_boxes, labels, num_classes, False)
-    cs = _fcos_ctr(ctr, xs, dt)
-    dev = an.device
-    gxs = [torch.empty_like(x) for x in xs]
-    gds = [torch.empty_like(x) for x in ds]
-    gcs = [torch.empty_like(x) for x in cs]
-    lv = _dense_levels(xs, ds, gxs, gds)
-    g = [t.to(torch.float32).reshape(()).contiguous() for t in (grad_cls, grad_reg, grad_ctr)]
-    with torch.cuda.device(dev):
-        check(_C.lib().d2b_fcos_loss_backward(C.byref(lv), _ptr_array(cs), _ptr_array(gcs), gt.shape[0], num_classes,
-                                              _C.DTYPE_CODE[dt], ptr(an), ptr(gt), ptr(lab), float(gamma), float(alpha),
-                                              ptr(g[0]), ptr(g[1]), ptr(g[2]), stream_ptr(dev)), "fcos_loss_backward")
+                                               float(scale_clamp), _c_weights(weights), ptr(g), stream_ptr(dev)),
+              "dense_loss_backward")
     ins = list(logits) + list(deltas) + list(ctr)
     return [gr.to(x.dtype).reshape(x.shape) for gr, x in zip(gxs + gds + gcs, ins)]
 
 
-@fcos_loss_backward_op.register_fake
-def _(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, gamma, alpha, grad_cls, grad_reg, grad_ctr):
+@dense_loss_backward_op.register_fake
+def _(logits, deltas, ctr, anchors, gt_boxes, labels, num_classes, rpn, gamma, alpha, beta, loss_type, scale_clamp,
+      weights, grad_sums):
     return [torch.empty_like(t) for t in list(logits) + list(deltas) + list(ctr)]
 
 
-def _fcos_setup(ctx, inputs, output):
+def _dense_setup(ctx, inputs, output):
     logits, deltas, ctr, anchors, gt_boxes, labels = inputs[:6]
     ctx.save_for_backward(*logits, *deltas, *ctr, anchors, gt_boxes, labels)
-    ctx.num_levels = len(logits)
+    ctx.num_levels, ctx.num_ctr = len(logits), len(ctr)
     ctx.params = inputs[6:]
 
 
-def _fcos_bwd(ctx, g_cls, g_reg, g_ctr, *_):
+def _dense_bwd(ctx, g_sums, *_):
     saved = ctx.saved_tensors
-    nl = ctx.num_levels
-    logits, deltas, ctr = list(saved[:nl]), list(saved[nl:2 * nl]), list(saved[2 * nl:3 * nl])
-    anchors, gt_boxes, labels = saved[3 * nl:]
-    grads = fcos_loss_backward_op(logits, deltas, ctr, anchors, gt_boxes, labels, *ctx.params, g_cls, g_reg, g_ctr)
-    return (grads[:nl], grads[nl:2 * nl], grads[2 * nl:]) + (None,) * 6
+    nl, nc = ctx.num_levels, ctx.num_ctr
+    logits, deltas, ctr = list(saved[:nl]), list(saved[nl:2 * nl]), list(saved[2 * nl:2 * nl + nc])
+    anchors, gt_boxes, labels = saved[2 * nl + nc:]
+    grads = dense_loss_backward_op(logits, deltas, ctr, anchors, gt_boxes, labels, *ctx.params, g_sums)
+    return (grads[:nl], grads[nl:2 * nl], grads[2 * nl:]) + (None,) * 11
 
 
-fcos_loss_op.register_autograd(_fcos_bwd, setup_context=_fcos_setup)
+dense_loss_op.register_autograd(_dense_bwd, setup_context=_dense_setup)
 
 
 def _frcnn_prepare(scores, deltas, proposals, gt_boxes, gt_classes):
@@ -285,12 +203,10 @@ def frcnn_loss_op(scores: Tensor, deltas: Tensor, proposals: Tensor, gt_boxes: T
     lib = _C.lib()
     ws_bytes = int(lib.d2b_frcnn_loss_workspace_bytes(r))
     ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
-    c = counts.data_ptr()
     with torch.cuda.device(dev):
         check(lib.d2b_frcnn_loss_forward(ptr(sc), ptr(dl), r, k, kreg, d, _C.DTYPE_CODE[dt], ptr(pr), ptr(gt), ptr(cls),
-                                         float(beta), int(loss_type), float(scale_clamp), _c_weights(weights), ptr(sums), C.c_void_p(sums.data_ptr() + 4),
-                                         C.c_void_p(c), C.c_void_p(c + 8), C.c_void_p(c + 16), C.c_void_p(c + 24),
-                                         ptr(status), ptr(ws), ws_bytes, stream_ptr(dev)), "frcnn_loss_forward")
+                                         float(beta), int(loss_type), float(scale_clamp), _c_weights(weights), ptr(sums),
+                                         ptr(counts), ptr(status), ptr(ws), ws_bytes, stream_ptr(dev)), "frcnn_loss_forward")
     return sums, counts, status
 
 
@@ -312,8 +228,8 @@ def frcnn_loss_backward_op(scores: Tensor, deltas: Tensor, proposals: Tensor, gt
         with torch.cuda.device(dev):
             check(_C.lib().d2b_frcnn_loss_backward(ptr(sc), ptr(dl), sc.shape[0], k, kreg, pr.shape[-1], _C.DTYPE_CODE[dt],
                                                    ptr(pr), ptr(gt), ptr(cls), float(beta), int(loss_type),
-                                                   float(scale_clamp), _c_weights(weights), ptr(g),
-                                                   C.c_void_p(g.data_ptr() + 4), ptr(gs), ptr(gd), stream_ptr(dev)),
+                                                   float(scale_clamp), _c_weights(weights), ptr(g), ptr(gs), ptr(gd),
+                                                   stream_ptr(dev)),
                   "frcnn_loss_backward")
     return gs.to(scores.dtype), gd.to(deltas.dtype)
 
@@ -345,6 +261,18 @@ def _cat_anchors(anchors: Union[Tensor, Sequence[Tensor]]) -> Tensor:
     return anchors if isinstance(anchors, Tensor) else torch.cat(list(anchors), dim=0)
 
 
+def _ema_update(loss_normalizer: Tensor, num_pos: Tensor, what: str) -> Tensor:
+    """DenseDetector._ema_update on the caller-held fp64 [1] `loss_normalizer`, in place: old * 0.9 + max(num_pos, 1) *
+    (1 - 0.9), in fp64 with separately rounded operations, as the Python float recurrence.  Returns the fp32 reciprocal of
+    the new value: the reference divides by the normaliser as a Python float, and torch's CUDA kernel then multiplies by
+    the fp32 reciprocal."""
+    if loss_normalizer.dtype != torch.float64 or loss_normalizer.numel() != 1:
+        raise ValueError("%s: loss_normalizer must be a float64 tensor with one element" % what)
+    momentum = 0.9
+    loss_normalizer.copy_(loss_normalizer * momentum + num_pos.clamp(min=1).to(torch.float64) * (1 - momentum))
+    return torch.reciprocal(loss_normalizer.reshape(()).to(torch.float32))
+
+
 def rpn_losses_fixed(anchors, pred_objectness_logits: List[Tensor], gt_labels, pred_anchor_deltas: List[Tensor],
                      gt_boxes, *, batch_size_per_image: int, smooth_l1_beta: float = 0.0,
                      box2box_weights: Sequence[float] = (1.0, 1.0, 1.0, 1.0), box_reg_loss_type: str = "smooth_l1",
@@ -355,14 +283,14 @@ def rpn_losses_fixed(anchors, pred_objectness_logits: List[Tensor], gt_labels, p
     Returns (losses {"loss_rpn_cls", "loss_rpn_loc"}, num_pos_anchors, num_neg_anchors, status), all device tensors."""
     labels = _stack(gt_labels)
     n = labels.shape[0]
-    cls, reg, num_pos, num_neg, status = dense_loss_op([x.unsqueeze(-1) for x in pred_objectness_logits],
-                                                       list(pred_anchor_deltas), _cat_anchors(anchors), _stack(gt_boxes),
-                                                       labels, 1, True, 0.0, -1.0, float(smooth_l1_beta),
-                                                       _fused_type(box_reg_loss_type), float(scale_clamp),
-                                                       [float(w) for w in box2box_weights])
-    normalizer = batch_size_per_image * n
+    sums, counts, status = dense_loss_op([x.unsqueeze(-1) for x in pred_objectness_logits], list(pred_anchor_deltas), [],
+                                         _cat_anchors(anchors), _stack(gt_boxes), labels, 1, True, 0.0, -1.0,
+                                         float(smooth_l1_beta), _fused_type(box_reg_loss_type), float(scale_clamp),
+                                         [float(w) for w in box2box_weights])
+    cls, reg, _ = (sums / (batch_size_per_image * n)).unbind(0)
+    num_pos, num_neg = counts.unbind(0)
     lw = loss_weight or {}
-    losses = {"loss_rpn_cls": cls / normalizer, "loss_rpn_loc": reg / normalizer}
+    losses = {"loss_rpn_cls": cls, "loss_rpn_loc": reg}
     return {k: v * lw.get(k, 1.0) for k, v in losses.items()}, num_pos, num_neg, status
 
 
@@ -376,18 +304,14 @@ def retinanet_losses_fixed(anchors, pred_logits: List[Tensor], gt_labels, pred_a
     loss_normalizer: caller-held fp64 [1] tensor holding the EMA of DenseDetector._ema_update (set it to 100 before the
     first call); it is updated in place, old * 0.9 + max(num_pos, 1) * (1 - 0.9), in fp64 with separately rounded
     operations, as the Python float recurrence.  Returns (losses {"loss_cls", "loss_box_reg"}, num_pos_anchors, status)."""
-    if loss_normalizer.dtype != torch.float64 or loss_normalizer.numel() != 1:
-        raise ValueError("retinanet_losses_fixed: loss_normalizer must be a float64 tensor with one element")
-    cls, reg, num_pos, _, status = dense_loss_op(list(pred_logits), list(pred_anchor_deltas), _cat_anchors(anchors),
-                                                 _stack(gt_boxes), _stack(gt_labels), int(num_classes), False,
-                                                 float(focal_loss_gamma), float(focal_loss_alpha), float(smooth_l1_beta),
-                                                 _fused_type(box_reg_loss_type), float(scale_clamp),
-                                                 [float(w) for w in box2box_weights])
-    momentum = 0.9
-    loss_normalizer.copy_(loss_normalizer * momentum + num_pos.clamp(min=1).to(torch.float64) * (1 - momentum))
-    # the reference divides by the normaliser as a Python float; torch's CUDA kernel then multiplies by the fp32 reciprocal
-    inv = torch.reciprocal(loss_normalizer.reshape(()).to(torch.float32))
-    return {"loss_cls": cls * inv, "loss_box_reg": reg * inv}, num_pos, status
+    sums, counts, status = dense_loss_op(list(pred_logits), list(pred_anchor_deltas), [], _cat_anchors(anchors),
+                                         _stack(gt_boxes), _stack(gt_labels), int(num_classes), False,
+                                         float(focal_loss_gamma), float(focal_loss_alpha), float(smooth_l1_beta),
+                                         _fused_type(box_reg_loss_type), float(scale_clamp),
+                                         [float(w) for w in box2box_weights])
+    num_pos, _ = counts.unbind(0)
+    cls, reg, _ = (sums * _ema_update(loss_normalizer, num_pos, "retinanet_losses_fixed")).unbind(0)
+    return {"loss_cls": cls, "loss_box_reg": reg}, num_pos, status
 
 
 def fast_rcnn_losses_fixed(scores: Tensor, proposal_deltas: Tensor, proposal_boxes: Tensor, gt_boxes: Tensor,
@@ -402,9 +326,9 @@ def fast_rcnn_losses_fixed(scores: Tensor, proposal_deltas: Tensor, proposal_box
     sums, counts, status = frcnn_loss_op(scores, proposal_deltas, proposal_boxes, gt_boxes, gt_classes,
                                             float(smooth_l1_beta), _fused_type(box_reg_loss_type), float(scale_clamp),
                                             [float(w) for w in box2box_weights])
-    r = scores.shape[0]
     # cross_entropy(mean) of no rows is the reference's scores.sum() * 0: a zero loss (the sum is 0 here)
-    losses = {"loss_cls": sums[0] / max(r, 1), "loss_box_reg": sums[1] / max(r, 1.0)}
+    cls, reg = (sums / max(scores.shape[0], 1)).unbind(0)
+    losses = {"loss_cls": cls, "loss_box_reg": reg}
     lw = loss_weight or {}
     return {k: v * lw.get(k, 1.0) for k, v in losses.items()}, counts, status
 

@@ -31,7 +31,7 @@ extern "C" {
 #define D2B_EWORKSPACE (-2)  /* workspace too small */
 #define D2B_EUNSUPPORTED (-3)
 
-#define D2B_ABI_VERSION 6
+#define D2B_ABI_VERSION 7
 int d2b_abi_version(void);
 /* compile-time facts, replaces detectron2._C.get_cuda_version / has_cuda (csrc/vision.cpp:23-49,86-88) */
 int d2b_cuda_version(void);
@@ -470,8 +470,8 @@ int d2b_panoptic_combine(const d2b_panoptic_images* img, int N, int C, const int
  * get_deltas: every anchor for the dense losses, the foreground proposals for Fast R-CNN); INVALID_CLASS when a Fast R-CNN
  * gt class is outside [0, K] or a dense int64 label outside [-1, K] (int8: outside {-1, 0, 1}); INVALID_BOX_ORDER (GIoU)
  * when a decoded or GT box of a regressed row fails fvcore's x2 >= x1 and y2 >= y1 (NaN included); with GIoU the
- * get_deltas assertion does not apply, as in the reference.  No host synchronisation, static shapes: capturable in a CUDA graph.  All arguments are checked
- * before the first CUDA call.
+ * get_deltas assertion does not apply, as in the reference (nor with LINEAR_GIOU).  No host synchronisation, static
+ * shapes: capturable in a CUDA graph.
  *
  * Dense: lv->logits[l] [N,R_l,K] (16-byte aligned), lv->deltas[l] [N,R_l,box_dim] -- the reference's per-level lists, no cat;
  *   anchors [R,box_dim] shared by the images (R = sum R_l), gt_boxes [N,R,box_dim] matched GT boxes, labels [N,R]:
@@ -479,14 +479,55 @@ int d2b_panoptic_combine(const d2b_panoptic_images* img, int N, int C, const int
  *     D2B_LABELS_I64  int64 {-1, 0..K-1, K = background} (RetinaNet gt_labels): target = one_hot(label)[:K].
  *   Classification: fvcore sigmoid_focal_loss(gamma, alpha; alpha < 0 = no weighting) summed over the rows with label >= 0;
  *   gamma = 0 and alpha < 0 is binary_cross_entropy_with_logits.  Rows with label -1 are not read.  Regression over the
- *   positive rows (I8: label 1, I64: 0 <= label < K).  Outputs (device): cls_sum, reg_sum, num_pos, num_neg (I8: label 0,
- *   I64: label K).  workspace: d2b_dense_loss_workspace_bytes(lv, N, K, dtype) bytes, 16-byte aligned.
- *   Backward: grad_cls / grad_reg (device scalars) = d loss / d cls_sum, d loss / d reg_sum; lv->grad_logits[l] (16-byte
- *   aligned) and lv->grad_deltas[l] are fully written in `dtype` (0 on ignored / non-positive rows).
+ *   positive rows (I8: label 1, I64: 0 <= label < K).
+ *   D2B_LOSS_LINEAR_GIOU (box_dim 4, D2B_LABELS_I64) is FCOS.losses + compute_ctrness_targets (meta_arch/fcos.py:193-251):
+ *   the regression is fvcore giou_loss of the deltas decoded by Box2BoxTransformLinear (relu(deltas) * stride; the relu
+ *   gradient is 0 at <= 0), and the positive rows add the centerness term: binary_cross_entropy_with_logits of
+ *   lv->ctr[l] [N,R_l] (`dtype`, read in place) against sqrt((min(l,r) / max(l,r)) * (min(t,b) / max(t,b))),
+ *   (l,t,r,b) = Box2BoxTransformLinear.get_deltas(anchor, gt box).  weights and scale_clamp are not read (weights may be
+ *   NULL).
+ *   Outputs (device): sums [3] fp32 = classification, regression, centerness (0 unless LINEAR_GIOU); counts [2] int64 =
+ *   num_pos, num_neg (I8: label 0, I64: label K); status [1].  workspace: d2b_dense_loss_workspace_bytes(lv, N, K, dtype)
+ *   bytes, 16-byte aligned.
+ *   Backward: grad_sums [3] (device) = d loss / d sums (the third is read with LINEAR_GIOU only); lv->grad_logits[l]
+ *   (16-byte aligned), lv->grad_deltas[l] and, with LINEAR_GIOU, lv->grad_ctr[l] [N,R_l] are fully written in `dtype` (0 on
+ *   ignored / non-positive rows).
  * Fast R-CNN: scores [R,K+1], deltas [R,kreg*box_dim] (kreg = K class-specific, gathered at the gt class, or 1), proposals
- *   and gt_boxes [R,box_dim] fp32, gt_classes [R] int64.  cls_sum = sum of cross_entropy over all rows; reg_sum over the
- *   foreground rows (0 <= class < K); the counts of _log_classification_stats (argmax: first index on ties, NaN wins).
- *   workspace: d2b_frcnn_loss_workspace_bytes(R) bytes, 16-byte aligned.  Backward: grad_scores / grad_deltas fully written. */
+ *   and gt_boxes [R,box_dim] fp32, gt_classes [R] int64.  Outputs (device): sums [2] fp32 = cross_entropy over all rows,
+ *   regression over the foreground rows (0 <= class < K); counts [4] int64 = num_fg, num_accurate, fg_num_accurate,
+ *   num_false_negative of _log_classification_stats (argmax: first index on ties, NaN wins); status [1].
+ *   workspace: d2b_frcnn_loss_workspace_bytes(R) bytes, 16-byte aligned.  Backward: grad_sums [2] (device) = d loss / d sums;
+ *   grad_scores / grad_deltas fully written.
+ * Workspace queries (host only, no CUDA call): d2b_dense_loss_workspace_bytes returns 0 for N < 0, K < 1 or a dtype that is
+ *   not a D2B_F* code, then for a level table that fails the forward's rule 2 below (without the ctr rules, which need the
+ *   loss type); d2b_frcnn_loss_workspace_bytes returns 0 for R <= 0.
+ * Arguments are checked in this order, and nothing is launched or written before every check has passed:
+ *   dense:  1. D2B_EINVAL: N < 0, K < 1, box_dim neither 4 nor 5, dtype not a D2B_F* code, weights NULL without
+ *              LINEAR_GIOU; label_kind not a D2B_LABELS_* code, or I8 with K != 1; gamma < 0, beta < 0 or either NaN, alpha
+ *              NaN; loss_type not a D2B_LOSS_* type, GIOU with box_dim 5, LINEAR_GIOU with box_dim 5 or I8 labels.
+ *           2. D2B_EINVAL: the level table -- lv NULL, num_levels outside 1..D2B_MAX_LEVELS, R_l < 0, R > INT_MAX; on a
+ *              level with rows (N * R_l > 0) logits[l] or deltas[l] NULL or logits[l] not 16-byte aligned, in the backward
+ *              grad_logits[l] or grad_deltas[l] NULL or grad_logits[l] not 16-byte aligned; with LINEAR_GIOU ctr[l] NULL
+ *              on a level with rows, in the backward grad_ctr[l] too; with another loss type ctr[l] or grad_ctr[l] set.
+ *           3. D2B_EINVAL: when there are rows (N * R > 0), anchors, gt_boxes or labels NULL.
+ *           4. D2B_EINVAL: more than INT_MAX CTAs.
+ *           forward:  5. D2B_EINVAL: sums, counts or status NULL.
+ *                     6. When there are rows, D2B_EINVAL for a NULL or not 16-byte aligned workspace, then D2B_EWORKSPACE
+ *                        when workspace_bytes is below the query's size.
+ *                     7. The loss launch (when there are rows), then the finish, which writes the outputs even
+ *                        without rows.
+ *           backward: 5. D2B_EINVAL: grad_sums NULL.
+ *                     6. No row: D2B_OK, nothing written.
+ *   frcnn:  1. D2B_EINVAL: R < 0, K < 1, kreg neither 1 nor K, box_dim neither 4 nor 5, dtype not a D2B_F* code, weights
+ *              NULL; beta < 0 or NaN, kreg * box_dim > INT_MAX / 2, loss_type neither SMOOTH_L1 nor GIOU, GIOU with
+ *              box_dim 5.
+ *           2. D2B_EINVAL: when R > 0, scores, deltas, proposals, gt_boxes or gt_classes NULL.
+ *           forward:  3. D2B_EINVAL: sums, counts or status NULL.
+ *                     4. When R > 0, D2B_EINVAL for a NULL or not 16-byte aligned workspace, then D2B_EWORKSPACE when
+ *                        workspace_bytes is below d2b_frcnn_loss_workspace_bytes(R).
+ *                     5. The loss launch (when R > 0), then the finish, which writes the outputs even for R = 0.
+ *           backward: 3. R == 0: D2B_OK, nothing written.
+ *                     4. D2B_EINVAL: grad_sums, grad_scores or grad_deltas NULL. */
 #define D2B_LABELS_I8 0
 #define D2B_LABELS_I64 1
 #define D2B_LOSS_STATUS_INVALID_BOX 1
@@ -494,50 +535,34 @@ int d2b_panoptic_combine(const d2b_panoptic_images* img, int N, int C, const int
 #define D2B_LOSS_STATUS_INVALID_BOX_ORDER 4
 #define D2B_LOSS_SMOOTH_L1 0
 #define D2B_LOSS_GIOU 1
+#define D2B_LOSS_LINEAR_GIOU 2 /* dense only */
 typedef struct {
   int num_levels;
   const void* logits[D2B_MAX_LEVELS];
   const void* deltas[D2B_MAX_LEVELS];
   void* grad_logits[D2B_MAX_LEVELS];
   void* grad_deltas[D2B_MAX_LEVELS];
+  const void* ctr[D2B_MAX_LEVELS];   /* LINEAR_GIOU only: centerness logits [N,R_l] */
+  void* grad_ctr[D2B_MAX_LEVELS];
   int R[D2B_MAX_LEVELS];
 } d2b_dense_loss_levels;
 size_t d2b_dense_loss_workspace_bytes(const d2b_dense_loss_levels* lv, int N, int K, int dtype);
 int d2b_dense_loss_forward(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int dtype, const float* anchors,
                            const float* gt_boxes, const void* labels, int label_kind, float gamma, float alpha, float beta,
-                           int loss_type, float scale_clamp, const float* weights, float* cls_sum, float* reg_sum, int64_t* num_pos, int64_t* num_neg,
+                           int loss_type, float scale_clamp, const float* weights, float* sums, int64_t* counts,
                            int* status, void* workspace, size_t workspace_bytes, void* stream);
 int d2b_dense_loss_backward(const d2b_dense_loss_levels* lv, int N, int K, int box_dim, int dtype, const float* anchors,
                             const float* gt_boxes, const void* labels, int label_kind, float gamma, float alpha, float beta,
-                            int loss_type, float scale_clamp, const float* weights, const float* grad_cls, const float* grad_reg, void* stream);
-/* FCOS: FCOS.losses + compute_ctrness_targets (meta_arch/fcos.py:193-251) on the dense kernel, xyxy boxes and D2B_LABELS_I64
- *   labels [N,R] (-1 ignored, 0..K-1 positive, K background; e.g. d2b_fcos_assign's).  cls_sum as the dense loss
- *   (sigmoid_focal_loss with gamma, alpha); reg_sum = fvcore giou_loss of the deltas decoded by Box2BoxTransformLinear
- *   (relu(deltas) * stride; the relu gradient is 0 at <= 0) over the positive rows, INVALID_BOX_ORDER where fvcore asserts;
- *   ctr_sum = binary_cross_entropy_with_logits of ctr[l] [N,R_l] (`dtype`, read in place) over the positive rows against
- *   sqrt((min(l,r) / max(l,r)) * (min(t,b) / max(t,b))), (l,t,r,b) = Box2BoxTransformLinear.get_deltas(anchor, gt box).
- *   num_pos = the positive rows.  ctr / grad_ctr: HOST arrays of lv->num_levels device pointers.  workspace:
- *   d2b_dense_loss_workspace_bytes(lv, N, K, dtype) bytes, 16-byte aligned.  Backward: grad_cls / grad_reg / grad_ctr_sum
- *   (device scalars); lv->grad_logits, lv->grad_deltas and grad_ctr are fully written (0 on non-positive rows for the
- *   deltas and the centerness, sigmoid(x) - t times grad_ctr_sum on the positive ones). */
-int d2b_fcos_loss_forward(const d2b_dense_loss_levels* lv, const void* const* ctr, int N, int K, int dtype,
-                          const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma, float alpha,
-                          float* cls_sum, float* reg_sum, float* ctr_sum, int64_t* num_pos, int* status, void* workspace,
-                          size_t workspace_bytes, void* stream);
-int d2b_fcos_loss_backward(const d2b_dense_loss_levels* lv, const void* const* ctr, void* const* grad_ctr, int N, int K,
-                           int dtype, const float* anchors, const float* gt_boxes, const int64_t* labels, float gamma,
-                           float alpha, const float* grad_cls, const float* grad_reg, const float* grad_ctr_sum,
-                           void* stream);
+                            int loss_type, float scale_clamp, const float* weights, const float* grad_sums, void* stream);
 size_t d2b_frcnn_loss_workspace_bytes(int R);
 int d2b_frcnn_loss_forward(const void* scores, const void* deltas, int R, int K, int kreg, int box_dim, int dtype,
                            const float* proposals, const float* gt_boxes, const int64_t* gt_classes, float beta,
-                           int loss_type, float scale_clamp, const float* weights, float* cls_sum, float* reg_sum, int64_t* num_fg, int64_t* num_accurate,
-                           int64_t* fg_num_accurate, int64_t* num_false_negative, int* status, void* workspace,
-                           size_t workspace_bytes, void* stream);
+                           int loss_type, float scale_clamp, const float* weights, float* sums, int64_t* counts,
+                           int* status, void* workspace, size_t workspace_bytes, void* stream);
 int d2b_frcnn_loss_backward(const void* scores, const void* deltas, int R, int K, int kreg, int box_dim, int dtype,
                             const float* proposals, const float* gt_boxes, const int64_t* gt_classes, float beta,
-                            int loss_type, float scale_clamp, const float* weights, const float* grad_cls, const float* grad_reg, void* grad_scores,
-                            void* grad_deltas, void* stream);
+                            int loss_type, float scale_clamp, const float* weights, const float* grad_sums,
+                            void* grad_scores, void* grad_deltas, void* stream);
 
 /* ---- Rotated-box IoU --------------------------------------------------------------------
  * Replaces torch.ops.detectron2.box_iou_rotated (csrc/vision.cpp:117,

@@ -25,10 +25,12 @@ def test_header_symbols_and_abi_version():
     # one entry point per selection stage, the box type and the decode as D2B_SELECT_* flags
     assert {n for n in declared if re.search(r"_(prepare|select)", n)} == {
         "d2b_rpn_prepare", "d2b_frcnn_prepare", "d2b_dense_prepare", "d2b_rpn_select"}
-    # the FCOS loss sizes its workspace with d2b_dense_loss_workspace_bytes
-    assert {n for n in declared if n.startswith("d2b_fcos_")} == {
-        "d2b_fcos_assign", "d2b_fcos_loss_forward", "d2b_fcos_loss_backward"}
-    assert lib.d2b_abi_version() == _C.ABI_VERSION == 6
+    # the FCOS loss is the dense loss with D2B_LOSS_LINEAR_GIOU
+    assert {n for n in declared if n.startswith("d2b_fcos_")} == {"d2b_fcos_assign"}
+    assert {n for n in declared if re.match(r"d2b_(dense|frcnn)_loss_", n)} == {
+        "d2b_dense_loss_workspace_bytes", "d2b_dense_loss_forward", "d2b_dense_loss_backward",
+        "d2b_frcnn_loss_workspace_bytes", "d2b_frcnn_loss_forward", "d2b_frcnn_loss_backward"}
+    assert lib.d2b_abi_version() == _C.ABI_VERSION == 7
     assert lib.d2b_arch() == b"sm_90a"
     assert _C.get_cuda_version().startswith("CUDA 12")
 

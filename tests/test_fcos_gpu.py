@@ -1,5 +1,6 @@
-"""GPU tests of the FCOS kernels: d2b_fcos_assign, d2b_fcos_loss_* and d2b_dense_prepare (D2B_SELECT_LINEAR) against the
-fixture taken from the real reference methods and against the torch restatement on the same CUDA tensors."""
+"""GPU tests of the FCOS kernels: d2b_fcos_assign, d2b_dense_loss_* (D2B_LOSS_LINEAR_GIOU) and d2b_dense_prepare
+(D2B_SELECT_LINEAR) against the fixture taken from the real reference methods and against the torch restatement on the
+same CUDA tensors."""
 import pytest
 import torch
 

@@ -118,56 +118,177 @@ def test_wrappers_run_the_restatement_on_cpu():
     assert float(losses["loss_cls"]) == 0.0 and float(losses["loss_box_reg"]) == 0.0
 
 
-def test_new_entry_points_validate_arguments_without_a_gpu():
+# The box-branch loss entry points.  Each row is one fault in an otherwise valid call whose pointers are dummy addresses,
+# never dereferenced: (entry points, fault, arguments that differ, expected status or a function of the call's kind giving
+# it, None where the row does not apply).  The kinds are every loss type and label kind an entry point takes; a dense call
+# has K = 1 with int8 labels and K = 80 with int64 ones, and one centerness level table (ctr, grad_ctr) with LINEAR_GIOU.
+# The valid forward calls pass a workspace of 0 bytes, so a call that passes every argument check returns D2B_EWORKSPACE;
+# the valid backward calls have rows, so a row must end before their launch (None where it would not).
+EINVAL, EWORKSPACE = -1, -2
+SL1, GIOU, LIN = 0, 1, 2  # D2B_LOSS_SMOOTH_L1 / _GIOU / _LINEAR_GIOU
+I8, I64 = 0, 1            # D2B_LABELS_I8 / _I64
+DF, DB = "d2b_dense_loss_forward", "d2b_dense_loss_backward"
+FF, FB = "d2b_frcnn_loss_forward", "d2b_frcnn_loss_backward"
+DENSE, FRCNN = (DF, DB), (FF, FB)
+_LOSS_KINDS = {  # (loss type, int8 labels) of every call each entry point takes
+    DF: ((SL1, True), (SL1, False), (GIOU, True), (GIOU, False), (LIN, False)),
+    DB: ((SL1, True), (SL1, False), (GIOU, True), (GIOU, False), (LIN, False)),
+    FF: ((SL1, False), (GIOU, False)),
+    FB: ((SL1, False), (GIOU, False)),
+}
+_P = 0x1000  # a 16-byte aligned dummy address
+_MISALIGNED = 0x1004
+_W = (1.0, 1.0, 1.0, 1.0, 1.0)
+_DENSE_IN = dict(lv=None, N=2, K=80, box_dim=4, dtype=0, anchors=_P, gt_boxes=_P, labels=_P, label_kind=I64, gamma=2.0,
+                 alpha=0.25, beta=0.1, loss_type=SL1, scale_clamp=4.135, weights=_W)
+_FRCNN_IN = dict(scores=_P, deltas=_P, R=10, K=80, kreg=80, box_dim=4, dtype=0, proposals=_P, gt_boxes=_P, gt_classes=_P,
+                 beta=0.0, loss_type=SL1, scale_clamp=4.135, weights=_W)
+_LOSS_PARAMS = {  # every parameter in order, with its value in a valid call (lv: the levels built by _loss_call)
+    DF: dict(_DENSE_IN, sums=_P, counts=_P, status=_P, workspace=_P, workspace_bytes=0),
+    DB: dict(_DENSE_IN, grad_sums=_P),
+    FF: dict(_FRCNN_IN, sums=_P, counts=_P, status=_P, workspace=_P, workspace_bytes=0),
+    FB: dict(_FRCNN_IN, grad_sums=_P, grad_scores=_P, grad_deltas=_P),
+}
+_PASSES = lambda k: None if k.bwd else EWORKSPACE  # noqa: E731  (every check passed: the backward would launch)
+_BWD_ONLY = lambda want: lambda k: want if k.bwd else _PASSES(k)  # noqa: E731  (the forward does not read it)
+_LIN_ONLY = lambda k: _PASSES(k) if k.lt == LIN else EINVAL  # noqa: E731
+_NOT_LIN = lambda k: EINVAL if k.lt == LIN else _PASSES(k)  # noqa: E731
+_NO_ROWS = lambda want: lambda k: want if k.bwd else None  # noqa: E731  (the forward would launch its finish)
+_LOSS_FAULTS = [
+    (DENSE, "N < 0", dict(N=-1), EINVAL),
+    (DENSE, "no class", dict(K=0), EINVAL),
+    (DENSE, "box_dim 3", dict(box_dim=3), EINVAL),
+    (DENSE, "rotated boxes: smooth-L1 only", dict(box_dim=5), lambda k: EINVAL if k.lt != SL1 else _PASSES(k)),
+    (DENSE, "no such dtype", dict(dtype=3), EINVAL),
+    (DENSE, "weights NULL: LINEAR_GIOU reads none", dict(weights=None), _LIN_ONLY),
+    (DENSE, "weights NULL, no rows", dict(weights=None, N=0), _NO_ROWS(None)),
+    (DB, "weights NULL, no rows", dict(weights=None, N=0), lambda k: 0 if k.lt == LIN else EINVAL),
+    (DENSE, "no such label kind", dict(label_kind=2), EINVAL),
+    (DENSE, "int8 labels need K = 1", dict(label_kind=I8, K=80), EINVAL),
+    (DENSE, "gamma < 0", dict(gamma=-1.0), EINVAL),
+    (DENSE, "gamma NaN", dict(gamma=math.nan), EINVAL),
+    (DENSE, "beta < 0", dict(beta=-0.1), EINVAL),
+    (DENSE, "beta NaN", dict(beta=math.nan), EINVAL),
+    (DENSE, "alpha NaN", dict(alpha=math.nan), EINVAL),
+    (DENSE, "no such loss type", dict(loss_type=3), EINVAL),
+    (DENSE, "negative loss type", dict(loss_type=-1), EINVAL),
+    (DENSE, "LINEAR_GIOU on rotated boxes", dict(loss_type=LIN, box_dim=5, ctr=[_P], grad_ctr=[_P]), EINVAL),
+    (DENSE, "LINEAR_GIOU with int8 labels", dict(loss_type=LIN, label_kind=I8, K=1, ctr=[_P], grad_ctr=[_P]), EINVAL),
+    (DENSE, "no level struct", dict(lv=None), EINVAL),
+    (DENSE, "no level", dict(num_levels=0), EINVAL),
+    (DENSE, "9 levels", dict(num_levels=9), EINVAL),
+    (DENSE, "R < 0", dict(R=[-1]), EINVAL),
+    (DENSE, "R > INT_MAX", dict(num_levels=2, R=[2 ** 30] * 2), EINVAL),
+    (DENSE, "logits NULL", dict(logits=[None]), EINVAL),
+    (DENSE, "deltas NULL", dict(deltas=[None]), EINVAL),
+    (DENSE, "logits misaligned", dict(logits=[_MISALIGNED]), EINVAL),
+    (DENSE, "a level without rows needs no pointer", dict(num_levels=2, R=[10, 0], logits=[_P, None], deltas=[_P, None],
+                                                         grad_logits=[_P, None], grad_deltas=[_P, None]), _PASSES),
+    (DENSE, "grad_logits NULL", dict(grad_logits=[None]), _BWD_ONLY(EINVAL)),
+    (DENSE, "grad_deltas NULL", dict(grad_deltas=[None]), _BWD_ONLY(EINVAL)),
+    (DENSE, "grad_logits misaligned", dict(grad_logits=[_MISALIGNED]), _BWD_ONLY(EINVAL)),
+    (DENSE, "ctr NULL", dict(ctr=[None]), lambda k: EINVAL if k.lt == LIN else _PASSES(k)),
+    (DENSE, "ctr set", dict(ctr=[_P]), _LIN_ONLY),
+    (DENSE, "grad_ctr NULL", dict(grad_ctr=[None]), lambda k: _BWD_ONLY(EINVAL)(k) if k.lt == LIN else _PASSES(k)),
+    (DENSE, "grad_ctr set", dict(grad_ctr=[_P]), _LIN_ONLY),
+    (DENSE, "ctr NULL on a level without rows", dict(num_levels=2, R=[10, 0], ctr=[_P, None], grad_ctr=[_P, None]),
+     _LIN_ONLY),
+    (DENSE, "anchors NULL", dict(anchors=None), EINVAL),
+    (DENSE, "gt_boxes NULL", dict(gt_boxes=None), EINVAL),
+    (DENSE, "labels NULL", dict(labels=None), EINVAL),
+    (DENSE, "inputs NULL without rows", dict(N=0, anchors=None, gt_boxes=None, labels=None), _NO_ROWS(0)),
+    (DENSE, "more than INT_MAX CTAs", dict(N=2 ** 30, R=[2 ** 14]), EINVAL),
+    (DF, "sums NULL", dict(sums=None), EINVAL),
+    (DF, "counts NULL", dict(counts=None), EINVAL),
+    (DF, "status NULL", dict(status=None), EINVAL),
+    (DF, "workspace NULL", dict(workspace=None), EINVAL),
+    (DF, "workspace misaligned", dict(workspace=_MISALIGNED), EINVAL),
+    (DF, "valid call: the workspace is too small", dict(), EWORKSPACE),
+    (DB, "grad_sums NULL", dict(grad_sums=None), EINVAL),
+    (DB, "grad_sums NULL without rows", dict(grad_sums=None, N=0), EINVAL),
+    (DB, "no rows: nothing to do", dict(N=0, grad_logits=[None], grad_deltas=[None], grad_ctr=[None]), 0),
+    (FRCNN, "R < 0", dict(R=-1), EINVAL),
+    (FRCNN, "no class", dict(K=0), EINVAL),
+    (FRCNN, "kreg neither 1 nor K", dict(kreg=3), EINVAL),
+    (FRCNN, "class-agnostic deltas", dict(kreg=1), _PASSES),
+    (FRCNN, "box_dim 6", dict(box_dim=6), EINVAL),
+    (FRCNN, "rotated boxes: smooth-L1 only", dict(box_dim=5), lambda k: EINVAL if k.lt != SL1 else _PASSES(k)),
+    (FRCNN, "no such dtype", dict(dtype=9), EINVAL),
+    (FRCNN, "weights NULL", dict(weights=None), EINVAL),
+    (FRCNN, "beta < 0", dict(beta=-0.1), EINVAL),
+    (FRCNN, "beta NaN", dict(beta=math.nan), EINVAL),
+    (FRCNN, "kreg * box_dim > INT_MAX / 2", dict(K=2 ** 30, kreg=2 ** 30), EINVAL),
+    (FRCNN, "LINEAR_GIOU is dense only", dict(loss_type=LIN), EINVAL),
+    (FRCNN, "no such loss type", dict(loss_type=3), EINVAL),
+] + [(FRCNN, name + " NULL", {name: None}, EINVAL)
+     for name in ("scores", "deltas", "proposals", "gt_boxes", "gt_classes")] + [
+    (FRCNN, "inputs NULL without rows", dict(R=0, scores=None, deltas=None, proposals=None, gt_boxes=None, gt_classes=None),
+     _NO_ROWS(0)),
+    (FF, "sums NULL", dict(sums=None), EINVAL),
+    (FF, "counts NULL", dict(counts=None), EINVAL),
+    (FF, "status NULL", dict(status=None), EINVAL),
+    (FF, "workspace NULL", dict(workspace=None), EINVAL),
+    (FF, "workspace misaligned", dict(workspace=_MISALIGNED), EINVAL),
+    (FF, "valid call: the workspace is too small", dict(), EWORKSPACE),
+    (FB, "no rows: D2B_OK before the gradient pointers", dict(R=0, grad_sums=None, grad_scores=None), 0),
+    (FB, "grad_sums NULL", dict(grad_sums=None), EINVAL),
+    (FB, "grad_scores NULL", dict(grad_scores=None), EINVAL),
+    (FB, "grad_deltas NULL", dict(grad_deltas=None), EINVAL),
+]
+
+
+def _loss_call(lib, entry, kind, **over):
+    from detectron2_b200 import _C
+
+    args = dict(_LOSS_PARAMS[entry], loss_type=kind.lt)
+    if "lv" in args:  # levels of 10 anchors each
+        args.update(label_kind=I8 if kind.i8 else I64, K=1 if kind.i8 else 80)
+        lv = _C.DenseLossLevels()
+        lv.num_levels = over.pop("num_levels", 1)
+        for name, _ in lv._fields_[1:]:
+            default = 10 if name == "R" else None if name in ("ctr", "grad_ctr") and kind.lt != LIN else _P
+            for l, v in enumerate(over.pop(name, [default] * _C.MAX_LEVELS)):
+                getattr(lv, name)[l] = v
+        args["lv"] = C.byref(lv)
+    args.update(over)
+    if args["weights"] is not None:
+        args["weights"] = (C.c_float * 5)(*args["weights"])
+    return getattr(lib, entry)(*args.values(), None)
+
+
+def test_loss_entry_points_validate_arguments_without_a_gpu():
+    """Every fault of the four box-branch loss entry points gets its status before anything is launched, for each loss type
+    and label kind the entry point takes.  Without a GPU a launch attempt returns a positive CUDA error, so a status <= 0
+    here also shows that nothing was launched or written (not even the forward's finish).  The workspace queries make no
+    CUDA call."""
+    import types
+
     from detectron2_b200 import _C
 
     lib = _C.lib()
-    EINVAL = -1
-    w = (C.c_float * 5)(1, 1, 1, 1, 1)
+    assert (_C.LOSS_TYPES["smooth_l1"], _C.LOSS_TYPES["giou"], _C.LOSS_LINEAR_GIOU) == (SL1, GIOU, LIN)
+    assert (_C.LABELS_I8, _C.LABELS_I64) == (I8, I64)
+    for entry, kinds in _LOSS_KINDS.items():
+        for lt, i8 in kinds:
+            kind = types.SimpleNamespace(bwd=entry in (DB, FB), lt=lt, i8=i8)
+            for entries, what, args, want in _LOSS_FAULTS:
+                w = want(kind) if callable(want) else want
+                if entry in entries and w is not None:
+                    got = _loss_call(lib, entry, kind, **args)
+                    assert got == w, (entry, what, lt, i8, got)
     lv = _C.DenseLossLevels()
-    lv.num_levels = 1
-    lv.R[0] = 10
-    dummy = C.c_void_p(16)  # never dereferenced: every call below fails its checks first
-    lv.logits[0] = lv.deltas[0] = 16
-    args = dict(N=2, K=80, D=4, dt=0, kind=_C.LABELS_I64, gamma=2.0, alpha=0.25, beta=0.1, lt=0)
-
-    def fwd(lvp=C.byref(lv), **kw):
-        a = dict(args, **kw)
-        return lib.d2b_dense_loss_forward(lvp, a["N"], a["K"], a["D"], a["dt"], dummy, dummy, dummy, a["kind"], a["gamma"],
-                                          a["alpha"], a["beta"], a["lt"], 4.135, w, dummy, dummy, dummy, dummy, dummy, dummy, 0, None)
-
-    assert fwd(lvp=None) == EINVAL
-    assert fwd(D=3) == EINVAL
-    assert fwd(dt=3) == EINVAL
-    assert fwd(kind=_C.LABELS_I8) == EINVAL  # int8 labels need K = 1
-    assert fwd(gamma=-1.0) == EINVAL
-    assert fwd(beta=float("nan")) == EINVAL
-    assert fwd(K=0) == EINVAL
-    assert fwd(lt=2) == EINVAL  # no such loss type
-    assert fwd(lt=1, D=5) == EINVAL  # GIoU is axis-aligned only
-    assert fwd(lt=1) == -2
-    assert fwd() == -2  # workspace too small (checked after the arguments)
-    lv.logits[0] = 8  # logits must be 16-byte aligned
-    assert fwd() == EINVAL
-    lv.logits[0] = 16
-    lv.num_levels = _C.MAX_LEVELS + 1
-    assert fwd() == EINVAL
-    lv.num_levels = 1
-    assert lib.d2b_dense_loss_workspace_bytes(C.byref(lv), 2, 80, 0) > 0
-    assert lib.d2b_dense_loss_backward(C.byref(lv), 2, 80, 4, 0, dummy, dummy, dummy, _C.LABELS_I64, 2.0, 0.25, 0.1, 0,
-                                       4.135, w,
-                                       dummy, dummy, None) == EINVAL  # no gradient buffers
-    assert lib.d2b_frcnn_loss_workspace_bytes(0) == 0
-    frc = lambda R, K, kreg, D, dt, lt=0: lib.d2b_frcnn_loss_forward(dummy, dummy, R, K, kreg, D, dt, dummy, dummy, dummy,
-                                                                     0.0, lt, 4.135, w, *([dummy] * 7), dummy, 0, None)
-    assert frc(-1, 80, 80, 4, 0) == EINVAL
-    assert frc(10, 80, 3, 4, 0) == EINVAL  # kreg must be 1 or K
-    assert frc(10, 80, 80, 6, 0) == EINVAL
-    assert frc(10, 80, 80, 4, 9) == EINVAL
-    assert frc(10, 80, 80, 5, 0, lt=1) == EINVAL
-    assert frc(10, 80, 80, 4, 0) == -2
-    assert lib.d2b_frcnn_loss_backward(dummy, dummy, 10, 80, 80, 4, 0, dummy, dummy, dummy, 0.0, 0, 4.135, w, dummy,
-                                       dummy, None, None, None) == EINVAL
+    lv.num_levels, lv.R[0], lv.logits[0], lv.deltas[0] = 1, 10, _P, _P
+    size = lib.d2b_dense_loss_workspace_bytes(C.byref(lv), 2, 80, 0)
+    assert size > 0 and size % 16 == 0
+    lv.ctr[0] = _P  # the query reads no centerness
+    assert lib.d2b_dense_loss_workspace_bytes(C.byref(lv), 2, 80, 0) == size
+    assert lib.d2b_dense_loss_workspace_bytes(None, 2, 80, 0) == 0
+    for n, k, dt in ((-1, 80, 0), (2, 0, 0), (2, 80, 3)):
+        assert lib.d2b_dense_loss_workspace_bytes(C.byref(lv), n, k, dt) == 0
+    lv.logits[0] = _MISALIGNED
+    assert lib.d2b_dense_loss_workspace_bytes(C.byref(lv), 2, 80, 0) == 0
+    assert lib.d2b_frcnn_loss_workspace_bytes(0) == lib.d2b_frcnn_loss_workspace_bytes(-1) == 0
+    assert lib.d2b_frcnn_loss_workspace_bytes(10) > 0
 
 
 # ---- the fixture taken from the real reference functions (tests/golden/make_golden_losses.py) ------------------------

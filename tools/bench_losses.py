@@ -1,6 +1,7 @@
 """Time the box-branch training losses, forward + backward: the native kernels (d2b_dense_loss_*, d2b_frcnn_loss_*) against
 the reference-shaped torch expressions (the restatement of RPN.losses, RetinaNet.losses and FastRCNNOutputLayers.losses in
-detectron2_b200/losses.py) on the same CUDA tensors, with CUDA events.
+detectron2_b200/losses.py) on the same CUDA tensors, with CUDA events.  FCOS, the dense loss with D2B_LOSS_LINEAR_GIOU, is
+timed by tools/bench_fcos.py.
 
     python tools/bench_losses.py [--iters 30] [--out FILE]
 
