@@ -133,6 +133,10 @@ def _declare(lib):
         "d2b_sem_seg_labels": (i, [vp, i, i, i, i, i, C.POINTER(SemSegImages), vp]),
         "d2b_panoptic_workspace_bytes": (sz, [C.POINTER(PanopticImages), i, i]),
         "d2b_panoptic_combine": (i, [C.POINTER(PanopticImages), i, i, i64p, d, d, d, i64p, i64p, f32p, vp, vp, sz, vp]),
+        "d2b_sem_seg_loss_workspace_bytes": (sz, [i, i, i, i, i, i, i, d]),
+        "d2b_sem_seg_loss_forward": (i, [vp, i, i, i, i, i, i, i64p, i64, i, d, f32p, f32p, u8p, f32p, i64p, vp, vp, sz,
+                                         vp]),
+        "d2b_sem_seg_loss_backward": (i, [vp, i, i, i, i, i, i, i64p, i64, f32p, u8p, f32p, f32p, vp, vp]),
         "d2b_paste_masks": (i, [f32p, f32p, i, i, i, i, f, u8p, vp]),
         "d2b_paste_masks_packed": (i, [f32p, f32p, i, i, i, i, f, vp, vp]),
     }

@@ -25,6 +25,7 @@
 #include <algorithm>
 #include <climits>
 
+#include "bilinear.cuh"
 #include "common.cuh"
 
 namespace {
@@ -41,28 +42,7 @@ constexpr size_t kAlign = 256;
 __host__ __device__ inline size_t align_up(size_t v) { return (v + kAlign - 1) / kAlign * kAlign; }
 __host__ __device__ inline int words_per_row(int W) { return (W + 31) >> 5; }
 
-// ---- semantic labels --------------------------------------------------------------------------------------------------
-// area_pixel_compute_source_index(scale, d, align_corners = false, cubic = false): max(scale * (d + 0.5) - 0.5, 0)
-__device__ __forceinline__ float src_index(float scale, int d) {
-  const float r = __fmaf_rn(scale, __fadd_rn((float)d, 0.5f), -0.5f);
-  return r < 0.f ? 0.f : r;
-}
-
-struct Tap {
-  int i0, i1;      // source index and its neighbour (clamped at the crop's last row / column)
-  float l0, l1;    // weights of i0 and i1
-};
-
-__device__ __forceinline__ Tap make_tap(float scale, int d, int in_size) {
-  const float r = src_index(scale, d);
-  Tap t;
-  t.i0 = (int)r;
-  t.i1 = t.i0 + (t.i0 < in_size - 1 ? 1 : 0);
-  t.l1 = __fsub_rn(r, (float)t.i0);
-  t.l0 = __fsub_rn(1.f, t.l1);
-  return t;
-}
-
+// ---- semantic labels (taps: bilinear.cuh) -----------------------------------------------------------------------------
 // torch.argmax on CUDA: v replaces the running best when it is a NaN and the best is not, or when neither is a NaN and
 // v is larger; ties keep the earlier channel (-0.0 == +0.0 compares equal).
 __device__ __forceinline__ bool beats(float v, float best) {

@@ -454,6 +454,64 @@ int d2b_panoptic_combine(const d2b_panoptic_images* img, int N, int C, const int
                          int64_t* num_segments, int64_t* seg_info, float* seg_score, int* status, void* workspace,
                          size_t workspace_bytes, void* stream);
 
+/* ---- Semantic segmentation loss: bilinear upsampling fused into the pixel cross-entropy ------------------------------
+ * Replaces SemSegFPNHead.losses (modeling/meta_arch/semantic_seg.py:255-267), the "cross_entropy" losses of
+ * DeepLabV3PlusHead / DeepLabV3Head and DeepLabCE (projects/DeepLab/deeplab/loss.py) as Panoptic-DeepLab's semantic head
+ * uses it: F.interpolate(logits.float(), scale_factor=stride, mode="bilinear", align_corners=False) followed by the
+ * per-pixel cross-entropy, without storing the [N,C,H,W] upsampled map or its log_softmax.
+ *   logits [N,C,Hp,Wp] of `dtype` (D2B_F32 / D2B_F16 / D2B_BF16, read in place, each value converted to fp32 first);
+ *   H = Hp * stride, W = Wp * stride, 1 <= stride <= D2B_SEMSEG_MAX_STRIDE.  Every upsampled value is bitwise PyTorch's
+ *   CUDA upsample_bilinear2d with the scale factor's source scale (float)(1.0 / stride) (not h / H); stride 1 is a copy.
+ *   targets [N,H,W] int64: a pixel equal to ignore_value (any int64) is skipped; another value outside [0, C) sets
+ *   D2B_SEMSEG_STATUS_BAD_LABEL in status and is skipped as well (the reference raises; the loss is then unspecified).
+ *   Per valid pixel p: lse(p) = logsumexp_c v_c(p), loss(p) = lse(p) - v_target(p).
+ * reduction D2B_SEMSEG_MEAN (nn.CrossEntropyLoss(reduction="mean", ignore_index)): loss_sum = sum of loss(p) over the valid
+ *   pixels; weights must be NULL.  The caller's loss is loss_sum / count (NaN with no valid pixel, as torch).
+ * reduction D2B_SEMSEG_TOP_K (DeepLabCE with top_k_percent_pixels in [0, 1], no class weight): the per-pixel values
+ *   x(p) = loss(p) (0 on ignored pixels), times weights[p] when weights [N,H,W] fp32 is given; k = (int64)(top_k_percent_pixels
+ *   * N*H*W), as Python's int(); the caller's loss is loss_sum / k.
+ *     top_k_percent_pixels == 1.0: loss_sum = the sum of every x(p), no selection (DeepLabCE's mean over all pixels).
+ *     Otherwise loss_sum = the sum of the k largest x(p): a radix select over an order-preserving uint32 image of the values
+ *     (every NaN above +inf, as torch.topk orders them; -0.0 == +0.0) finds the k-th largest t, loss_sum = sum_{x > t} x +
+ *     (k - #{x > t}) * t.  Pixels tied at t are taken in ascending flat index (the reference's choice among ties is
+ *     unspecified; it changes only the gradient of the tied pixels).  selected [N,H,W] uint8 receives 1 for the k pixels
+ *     taken.  k == 0: loss_sum 0, nothing selected.
+ * Forward outputs (device, no host read): lse [N,H,W] fp32 (0 on skipped pixels), loss_sum [1] fp32, count [1] int64 = the
+ *   valid pixels, status [1] int32; selected as above.  Reductions are per-CTA partials added in a fixed order by a
+ *   finish launch (no float atomics): bitwise reproducible.  workspace: d2b_sem_seg_loss_workspace_bytes(...) bytes,
+ *   256-byte aligned, no initialisation needed; the query makes no CUDA call and returns 0 for arguments that fail rule 1
+ *   below (weights aside), otherwise at least 256.  Launches: 2 (MEAN, TOP_K 1.0) or 8 (TOP_K below 1.0).
+ * Backward: grad_sum [1] fp32 (device) = d loss / d loss_sum.  grad_logits [N,C,Hp,Wp] of `dtype` is written once, every
+ *   element (no zero fill, no atomics): each low-res logit gathers, in a fixed order, over the output pixels p whose two
+ *   row taps and two column taps reach it, tap weight * g(p) * (exp(v_c(p) - lse(p)) - [target(p) = c]), with v_c(p)
+ *   recomputed and g(p) = grad_sum * weights[p] (1 when NULL) on valid pixels whose selected[p] is 1 (all when NULL), 0
+ *   elsewhere.  At the last row / column both taps fall on the same logit and both weights go to it.  Pass the forward's
+ *   weights and selected.  One launch.  No host synchronisation in either direction: capturable in a CUDA graph.
+ * Arguments are checked in this order, and nothing is launched or written before every check has passed:
+ *   forward:  1. D2B_EINVAL: N < 0 or N > 65535, C < 1, Hp < 1, Wp < 1, stride outside 1..D2B_SEMSEG_MAX_STRIDE, dtype
+ *                not a D2B_F* code, N*H*W > INT_MAX - 1024 or C*Hp*Wp > INT_MAX; reduction not a D2B_SEMSEG_* code; MEAN
+ *                with weights; TOP_K with top_k_percent_pixels NaN or outside [0, 1].
+ *             2. D2B_EINVAL: loss_sum, count or status NULL; when N > 0, logits, targets or lse NULL; TOP_K below 1.0 with
+ *                selected NULL.
+ *             3. D2B_EINVAL: workspace NULL or not 256-byte aligned; D2B_EWORKSPACE: workspace_bytes below the query.
+ *             4. The launches; N == 0 runs the finish alone (loss_sum 0, count 0, status 0).
+ *   backward: 1. D2B_EINVAL: the shape and dtype rules of the forward's rule 1.
+ *             2. N == 0: D2B_OK, nothing written.
+ *             3. D2B_EINVAL: logits, targets, lse, grad_sum or grad_logits NULL. */
+#define D2B_SEMSEG_MEAN 0
+#define D2B_SEMSEG_TOP_K 1
+#define D2B_SEMSEG_MAX_STRIDE 32
+#define D2B_SEMSEG_STATUS_BAD_LABEL 1
+size_t d2b_sem_seg_loss_workspace_bytes(int N, int C, int Hp, int Wp, int stride, int dtype, int reduction,
+                                        double top_k_percent_pixels);
+int d2b_sem_seg_loss_forward(const void* logits, int dtype, int N, int C, int Hp, int Wp, int stride,
+                             const int64_t* targets, int64_t ignore_value, int reduction, double top_k_percent_pixels,
+                             const float* weights, float* lse, uint8_t* selected, float* loss_sum, int64_t* count,
+                             int* status, void* workspace, size_t workspace_bytes, void* stream);
+int d2b_sem_seg_loss_backward(const void* logits, int dtype, int N, int C, int Hp, int Wp, int stride,
+                              const int64_t* targets, int64_t ignore_value, const float* weights, const uint8_t* selected,
+                              const float* lse, const float* grad_sum, void* grad_logits, void* stream);
+
 /* ---- Box-branch training losses: RPN / RRPN, RetinaNet, Fast R-CNN ------------------------------------------------
  * Replace RPN.losses (proposal_generator/rpn.py:366-429), RetinaNet.losses (meta_arch/retinanet.py:160-210) and
  * FastRCNNOutputLayers.losses / box_reg_loss / _log_classification_stats (roi_heads/fast_rcnn.py:88-115, 307-352, 424-463)
