@@ -19,6 +19,7 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kPix = 16;       // output bytes per thread
 constexpr int kMaxM = 64;      // largest mask side staged in smem (28 in every shipped config)
+constexpr int kMaxGridY = 65535;  // masks per launch of a (CTAs per mask, N) grid; larger N is launched in slices
 
 __device__ __forceinline__ float sample_coord(float p, float b0, float b1, float M) {
   float g = (p + 0.5f - b0) / (b1 - b0) * 2.f - 1.f;
@@ -319,13 +320,17 @@ D2B_API int d2b_paste_masks_packed(const float* masks, const float* boxes, int N
                                    uint32_t* out, void* stream) {
   if (N == 0 || H == 0 || W == 0) return D2B_OK;
   if (!masks || !boxes || !out || N < 0 || M <= 0 || H < 0 || W < 0 || !(threshold >= 0.f)) return D2B_EINVAL;
-  if (M > kMaxM || N > 65535) return D2B_EUNSUPPORTED;
+  if (M > kMaxM) return D2B_EUNSUPPORTED;
   const int Ww = d2b_cdiv(W, 32);
   const long long words = (long long)H * Ww;
   if ((long long)H * W >= (1LL << 30)) return D2B_EUNSUPPORTED;
   int gx = (int)std::min<long long>(d2b_cdiv(words, kThreads), std::max<long long>(1, d2b_cdiv(16LL * d2b_num_sms(), N)));
-  paste_masks_packed_kernel<<<dim3(gx, N), kThreads, 0, (cudaStream_t)stream>>>(masks, boxes, M, H, W, Ww, threshold, out);
-  D2B_CHECK_LAUNCH();
+  for (int s = 0; s < N; s += kMaxGridY) {  // grid.y holds at most 65535 masks: one launch per slice
+    const int n = std::min(kMaxGridY, N - s);
+    paste_masks_packed_kernel<<<dim3(gx, n), kThreads, 0, (cudaStream_t)stream>>>(
+        masks + (size_t)s * M * M, boxes + 4 * (size_t)s, M, H, W, Ww, threshold, out + (size_t)s * words);
+    D2B_CHECK_LAUNCH();
+  }
   return D2B_OK;
 }
 
@@ -347,9 +352,16 @@ D2B_API int d2b_paste_masks(const float* masks, const float* boxes, int N, int M
     int gx = d2b_cdiv(chunks + 1, kThreads);
     int want = d2b_cdiv(8LL * d2b_num_sms(), N);
     if (gx > want) gx = want < 1 ? 1 : want;
-    dim3 grid(gx, N);
-    if (tab) paste_masks_kernel<true><<<grid, kThreads, tab_bytes, (cudaStream_t)stream>>>(masks, boxes, M, H, W, threshold, out, N, 0);
-    else paste_masks_kernel<false><<<grid, kThreads, 0, (cudaStream_t)stream>>>(masks, boxes, M, H, W, threshold, out, N, 0);
+    for (int s = 0; s < N; s += kMaxGridY) {  // grid.y holds at most 65535 masks: one launch per slice
+      const int n = std::min(kMaxGridY, N - s);
+      const float* mk = masks + (size_t)s * M * M;
+      const float* bx = boxes + 4 * (size_t)s;
+      uint8_t* o = out + (size_t)s * plane;
+      if (tab) paste_masks_kernel<true><<<dim3(gx, n), kThreads, tab_bytes, (cudaStream_t)stream>>>(mk, bx, M, H, W, threshold, o, n, 0);
+      else paste_masks_kernel<false><<<dim3(gx, n), kThreads, 0, (cudaStream_t)stream>>>(mk, bx, M, H, W, threshold, o, n, 0);
+      D2B_CHECK_LAUNCH();
+    }
+    return D2B_OK;
   }
   D2B_CHECK_LAUNCH();
   return D2B_OK;

@@ -687,7 +687,11 @@ int d2b_deform_conv_fused_backward(const float* x, const float* offset_mask, con
 /* ---- paste_masks_in_image ---------------------------------------------------------------
  * Replaces detectron2/layers/mask_ops.py:74-147 (GPU branch: every pixel of the image for every mask).
  * masks [N,M,M] fp32, boxes [N,4] xyxy fp32 -> out [N,H,W] uint8: (v >= threshold) as 0/1 when
- * threshold >= 0, else (uint8)(v*255). */
+ * threshold >= 0, else (uint8)(v*255).  A box whose sample coordinates are not finite (zero or negative extent where a pixel
+ * centre meets x0, NaN or infinite corners) gives v = 0 there.  Any N >= 0.
+ *   1. D2B_OK without a launch when N, H or W is 0.
+ *   2. D2B_EINVAL: masks, boxes or out NULL, N, H or W below 0, M below 1 (the packed form: also threshold below 0 or NaN).
+ *   3. D2B_EUNSUPPORTED: M > 64, or H * W >= 2^30. */
 int d2b_paste_masks(const float* masks, const float* boxes, int N, int M, int H, int W,
                     float threshold, uint8_t* out, void* stream);
 /* The boolean result (threshold >= 0 only) bit-packed: out [N,H,ceil(W/32)] uint32, bit b of word w of row y = pixel
