@@ -53,6 +53,7 @@ class DenseLevels(C.Structure):
 
 LABELS_I8, LABELS_I64 = 0, 1  # D2B_LABELS_*
 SAMPLE_MAX_SAMPLES = 8192  # D2B_SAMPLE_MAX_SAMPLES
+POLYGON_MAX_S = 256  # D2B_POLYGON_MAX_S
 LOSS_STATUS_INVALID_BOX, LOSS_STATUS_INVALID_CLASS, LOSS_STATUS_INVALID_BOX_ORDER = 1, 2, 4  # D2B_LOSS_STATUS_*
 LOSS_TYPES = {"smooth_l1": 0, "giou": 1}  # D2B_LOSS_SMOOTH_L1 / D2B_LOSS_GIOU: the box_reg_loss_type values with a kernel
 LOSS_LINEAR_GIOU = 2  # D2B_LOSS_LINEAR_GIOU: FCOS, dense only
@@ -98,6 +99,9 @@ def _declare(lib):
                                   i64p, vp]),
         "d2b_mask_loss_forward": (i, [f32p, i, i, i, u8p, i, i, i, f32p, i64p, i64p, f32p, u8p, vp]),
         "d2b_mask_loss_backward": (i, [f32p, i, i, i, u8p, i64p, f32p, f32p, vp]),
+        "d2b_polygons_crop_and_resize": (i, [vp, i, vp, i, vp, i, f32p, i64p, i, i, u8p, vp]),
+        "d2b_polygons_to_bitmask": (i, [vp, i, vp, i, vp, i, i, i, u8p, vp]),
+        "d2b_mask_loss_polygons_forward": (i, [f32p, i, i, i, vp, i, vp, i, vp, i, f32p, i64p, i64p, f32p, u8p, vp]),
         "d2b_keypoints_workspace_bytes": (sz, [i, i]),
         "d2b_keypoints_from_heatmaps": (i, [f32p, i, i, i, f32p, f32p, vp, sz, vp]),
         "d2b_keypoint_loss_forward": (i, [vp, i, i, i, i, f32p, f32p, i64p, u8p, f32p, i64p, vp]),

@@ -22,6 +22,7 @@ SOURCES = {
     "abi.cu": [],
     "roi_align.cu": [],
     "paste_masks.cu": ["-fmad=false"],
+    "polygon_masks.cu": ["-fmad=false"],
     "nms.cu": ["-fmad=false"],
     "postproc.cu": ["-fmad=false"],
     "match.cu": ["-fmad=false"],
@@ -47,7 +48,7 @@ def _compile(name, extra, force):
     obj = os.path.join(OBJ, name.replace(".cu", ".o"))
     deps = [src, os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "tc_common.cuh"),
             os.path.join(CSRC, "deform_conv_tc.cuh"), os.path.join(CSRC, "rotated_iou.cuh"), os.path.join(CSRC, "boxes.cuh"),
-            os.path.join(CSRC, "bilinear.cuh"), os.path.join(HERE, "..", "include", "d2b200.h"), __file__]
+            os.path.join(CSRC, "bilinear.cuh"), os.path.join(CSRC, "polygon_raster.cuh"), os.path.join(HERE, "..", "include", "d2b200.h"), __file__]
     if force or _stale(obj, deps):
         cmd = [NVCC] + ARCH + COMMON + extra + ["-c", src, "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)

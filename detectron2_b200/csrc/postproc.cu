@@ -22,6 +22,7 @@
 
 #include "boxes.cuh"
 #include "common.cuh"
+#include "polygon_raster.cuh"
 
 namespace {
 
@@ -523,48 +524,99 @@ __device__ __forceinline__ Tap1 make_tap1(float v, int size) {  // torchvision r
   return t;
 }
 
-__global__ void __launch_bounds__(256) mask_loss_fwd_kernel(const float* __restrict__ logits, int C, int S,
-                                                            const unsigned char* __restrict__ gt, int G, int H, int W,
-                                                            const float* __restrict__ boxes,
-                                                            const long long* __restrict__ mask_index,
+// The target of each bin comes from a policy: BitmaskTarget pools the ground-truth bitmask (the RoIAlign above),
+// PolygonTarget rasterizes the matched instance's polygons into shared memory first (polygon_raster.cuh).  begin() is called
+// by every thread of the CTA; the returned Roi answers one bin.
+struct BitmaskTarget {
+  const unsigned char* __restrict__ gt;
+  int G, H, W;
+  const float* __restrict__ boxes;
+  const long long* __restrict__ mask_index;
+  struct Smem {};
+  struct Roi {
+    const unsigned char* __restrict__ m;
+    int H, W, S, gh, gw;
+    bool have_mask;
+    float sw, sh, bin_w, bin_h, count;
+    __device__ __forceinline__ bool operator()(int bin) const {
+      const int ph = bin / S, pw = bin - ph * S;
+      float v = 0.f;
+      if (have_mask) {
+        for (int iy = 0; iy < gh; ++iy) {
+          const Tap1 ty = make_tap1(sh + (float)ph * bin_h + ((float)iy + .5f) * bin_h / (float)gh, H);
+          for (int ix = 0; ix < gw; ++ix) {
+            const Tap1 tx = make_tap1(sw + (float)pw * bin_w + ((float)ix + .5f) * bin_w / (float)gw, W);
+            const float v1 = m[(size_t)ty.lo * W + tx.lo] ? 1.f : 0.f, v2 = m[(size_t)ty.lo * W + tx.hi] ? 1.f : 0.f;
+            const float v3 = m[(size_t)ty.hi * W + tx.lo] ? 1.f : 0.f, v4 = m[(size_t)ty.hi * W + tx.hi] ? 1.f : 0.f;
+            v += (ty.wl * tx.wl) * v1 + (ty.wl * tx.wh) * v2 + (ty.wh * tx.wl) * v3 + (ty.wh * tx.wh) * v4;
+          }
+        }
+        v /= count;
+      }
+      return v >= 0.5f;
+    }
+  };
+  __device__ __forceinline__ Roi begin(int k, int S, Smem&) const {
+    Roi r;
+    const float* b = boxes + (size_t)k * 4;
+    // aligned = True, spatial_scale = 1: box - 0.5, no minimum size
+    r.sw = b[0] * 1.0f - 0.5f;
+    r.sh = b[1] * 1.0f - 0.5f;
+    const float ew = b[2] * 1.0f - 0.5f, eh = b[3] * 1.0f - 0.5f;
+    const float rw = ew - r.sw, rh = eh - r.sh;
+    r.bin_h = rh / (float)S;
+    r.bin_w = rw / (float)S;
+    r.gh = max((int)ceilf(rh / (float)S), 0);
+    r.gw = max((int)ceilf(rw / (float)S), 0);
+    r.count = (float)max(r.gh * r.gw, 1);
+    const long long mi = mask_index ? mask_index[k] : k;
+    r.have_mask = mi >= 0 && mi < G;
+    r.m = gt + (size_t)(r.have_mask ? mi : 0) * H * W;
+    r.H = H;
+    r.W = W;
+    r.S = S;
+    return r;
+  }
+};
+
+struct PolygonTarget {
+  PolyBatch pb;
+  const float* __restrict__ boxes;
+  const long long* __restrict__ mask_index;
+  using Smem = PolyTileSmem;
+  struct Roi {
+    const PolyTileSmem* sm;
+    int S;
+    __device__ __forceinline__ bool operator()(int bin) const {
+      const int r = bin / S;
+      return poly_mask_bit(*sm, r, bin - r * S);
+    }
+  };
+  __device__ __forceinline__ Roi begin(int k, int S, Smem& sm) const {
+    PolyTransform tf;
+    const bool box_ok = poly_box_transform(boxes + (size_t)k * 4, S, tf);
+    poly_raster_instance(pb, !box_ok ? -1 : mask_index ? mask_index[k] : k, tf, S, S, 0, S, 0, S, sm);
+    return Roi{&sm, S};
+  }
+};
+
+template <class Target>
+__global__ void __launch_bounds__(256) mask_loss_fwd_kernel(const float* __restrict__ logits, int C, int S, Target target,
                                                             const long long* __restrict__ classes,
                                                             float* __restrict__ loss_per_roi,
                                                             unsigned char* __restrict__ targets) {
   __shared__ float s_red[8];
+  __shared__ typename Target::Smem s_target;
   const int k = blockIdx.x, tid = threadIdx.x;
-  const float* b = boxes + (size_t)k * 4;
-  // aligned = True, spatial_scale = 1: box - 0.5, no minimum size
-  const float sw = b[0] * 1.0f - 0.5f, sh = b[1] * 1.0f - 0.5f, ew = b[2] * 1.0f - 0.5f, eh = b[3] * 1.0f - 0.5f;
-  const float rw = ew - sw, rh = eh - sh;
-  const float bin_h = rh / (float)S, bin_w = rw / (float)S;
-  int gh = (int)ceilf(rh / (float)S), gw = (int)ceilf(rw / (float)S);
-  gh = max(gh, 0);
-  gw = max(gw, 0);
-  const float count = (float)max(gh * gw, 1);
-  long long mi = mask_index ? mask_index[k] : k;
-  const bool have_mask = mi >= 0 && mi < G;
-  const unsigned char* __restrict__ m = gt + (size_t)(have_mask ? mi : 0) * H * W;
+  const typename Target::Roi roi = target.begin(k, S, s_target);
   const long long cls = classes ? classes[k] : 0;
   const bool cls_ok = cls >= 0 && cls < C;
   const float* __restrict__ lg = logits + ((size_t)k * C + (cls_ok ? cls : 0)) * S * S;
   float acc_loss = 0.f;
   for (int bin = tid; bin < S * S; bin += 256) {
-    const int ph = bin / S, pw = bin - ph * S;
-    float v = 0.f;
-    if (have_mask) {
-      for (int iy = 0; iy < gh; ++iy) {
-        const Tap1 ty = make_tap1(sh + (float)ph * bin_h + ((float)iy + .5f) * bin_h / (float)gh, H);
-        for (int ix = 0; ix < gw; ++ix) {
-          const Tap1 tx = make_tap1(sw + (float)pw * bin_w + ((float)ix + .5f) * bin_w / (float)gw, W);
-          const float v1 = m[(size_t)ty.lo * W + tx.lo] ? 1.f : 0.f, v2 = m[(size_t)ty.lo * W + tx.hi] ? 1.f : 0.f;
-          const float v3 = m[(size_t)ty.hi * W + tx.lo] ? 1.f : 0.f, v4 = m[(size_t)ty.hi * W + tx.hi] ? 1.f : 0.f;
-          v += (ty.wl * tx.wl) * v1 + (ty.wl * tx.wh) * v2 + (ty.wh * tx.wl) * v3 + (ty.wh * tx.wh) * v4;
-        }
-      }
-      v /= count;
-    }
-    const float t = v >= 0.5f ? 1.f : 0.f;
-    targets[(size_t)k * S * S + bin] = (unsigned char)(v >= 0.5f);
+    const bool tb = roi(bin);
+    const float t = tb ? 1.f : 0.f;
+    targets[(size_t)k * S * S + bin] = (unsigned char)tb;
     if (cls_ok) {
       const float x = lg[bin];
       // binary_cross_entropy_with_logits: (1 - t) x + max(-x, 0) + log(exp(-max) + exp(-x - max)),  max = max(-x, 0)
@@ -611,8 +663,25 @@ D2B_API int d2b_mask_loss_forward(const float* logits, int K, int C, int S, cons
   if (K < 0 || C <= 0 || S <= 0 || G < 0 || H <= 0 || W <= 0) return D2B_EINVAL;
   if (K == 0) return D2B_OK;
   if (!logits || !gt_masks || !boxes || !loss_per_roi || !targets) return D2B_EINVAL;
-  mask_loss_fwd_kernel<<<K, 256, 0, (cudaStream_t)stream>>>(logits, C, S, gt_masks, G, H, W, boxes, (const long long*)mask_index,
-                                                            (const long long*)classes, loss_per_roi, targets);
+  mask_loss_fwd_kernel<<<K, 256, 0, (cudaStream_t)stream>>>(
+      logits, C, S, BitmaskTarget{gt_masks, G, H, W, boxes, (const long long*)mask_index}, (const long long*)classes,
+      loss_per_roi, targets);
+  D2B_CHECK_LAUNCH();
+  return D2B_OK;
+}
+
+D2B_API int d2b_mask_loss_polygons_forward(const float* logits, int K, int C, int S, const double* coords, int V,
+                                           const int* poly_start, int P, const int* inst_start, int G, const float* boxes,
+                                           const int64_t* mask_index, const int64_t* classes, float* loss_per_roi,
+                                           uint8_t* targets, void* stream) {
+  if (K < 0 || C < 1 || S < 1 || S > D2B_POLYGON_MAX_S || V < 0 || P < 0 || G < 0) return D2B_EINVAL;
+  if (K == 0) return D2B_OK;
+  if (!logits || !boxes || !loss_per_roi || !targets || (G > 0 && !inst_start) || (P > 0 && !poly_start) ||
+      (V > 0 && !coords))
+    return D2B_EINVAL;
+  mask_loss_fwd_kernel<<<K, 256, 0, (cudaStream_t)stream>>>(
+      logits, C, S, PolygonTarget{PolyBatch{coords, V, poly_start, P, inst_start, G}, boxes, (const long long*)mask_index},
+      (const long long*)classes, loss_per_roi, targets);
   D2B_CHECK_LAUNCH();
   return D2B_OK;
 }

@@ -348,6 +348,51 @@ int d2b_mask_loss_forward(const float* logits, int K, int C, int S, const uint8_
 int d2b_mask_loss_backward(const float* logits, int K, int C, int S, const uint8_t* targets, const int64_t* classes,
                            const float* grad_scale, float* grad_logits, void* stream);
 
+/* ---- Polygon ground-truth masks (DESIGN.md f-4) ------------------------------------------------------------------------
+ * PolygonMasks.crop_and_resize (detectron2/structures/masks.py:396-420, rasterize_polygons_within_box :39-85) and
+ * polygons_to_bitmask / BitMasks.from_polygon_masks (:22-36, :166-180), bit-exact to pycocotools' rleFrPoly + merge +
+ * decode, for a whole batch without a host round trip.
+ * A batch's polygons (polygon_masks.pack_polygons): coords [V,2] float64 (x, y) vertices; poly_start [P+1] int32, polygon p
+ *   = vertices [poly_start[p], poly_start[p+1]); inst_start [G+1] int32, instance g = polygons [inst_start[g],
+ *   inst_start[g+1]).  An instance's mask is the union of its polygons' masks; an instance without polygons is all zeros.
+ * Contracts for input the reference rejects or leaves undefined: an instance index outside [0, G) gives an all-zero mask;
+ *   an instance range out of order or past P is empty, and so is a polygon range out of order or past V (nothing outside
+ *   the arrays is read); a polygon with a non-finite vertex, or a lattice coordinate 5 x' + 0.5 outside (-2^30, 2^30), adds
+ *   nothing; so does every polygon of a proposal whose box is not finite.
+ *
+ * d2b_polygons_crop_and_resize: boxes [K,4] fp32 proposal boxes; mask_index [K] int64 instance of each proposal (NULL:
+ *   proposal k uses instance k) -> out [K,S,S] uint8 0/1, row-major.  Per proposal, each vertex becomes
+ *   x' = (x - x0) * ratio_w (float64), ratio_w = S / (x1 - x0) in fp32 when x1 - x0 >= 0.1, else S / 0.1 in float64
+ *   (y likewise), and is rasterized on the S x S grid.  One CTA per proposal.
+ *   Checks, in order (nothing is launched before all pass):
+ *     1. D2B_EINVAL: K < 0, S < 1 or S > D2B_POLYGON_MAX_S, V, P or G below 0.
+ *     2. K == 0: D2B_OK.
+ *     3. D2B_EINVAL: boxes or out NULL; inst_start NULL with G > 0, poly_start NULL with P > 0, coords NULL with V > 0.
+ * d2b_polygons_to_bitmask: out [G,H,W] uint8 0/1, every instance rasterized on the full H x W image (no transform).  CTAs
+ *   tile the columns and rows, and each edge visits only the columns it crosses.
+ *   Checks, in order:
+ *     1. D2B_EINVAL: V, P or G below 0, H or W below 1, H * W > INT_MAX, more than INT_MAX tiles.
+ *     2. G == 0: D2B_OK.
+ *     3. D2B_EINVAL: out or inst_start NULL, poly_start NULL with P > 0, coords NULL with V > 0.
+ * d2b_mask_loss_polygons_forward: d2b_mask_loss_forward with the targets of d2b_polygons_crop_and_resize, rasterized inside
+ *   the proposal's CTA: the same loss_per_roi and targets outputs, for all K proposals of a batch in one launch (mask_index
+ *   holds batch-wide instance indices).  The backward is d2b_mask_loss_backward on these targets.
+ *   Checks, in order:
+ *     1. D2B_EINVAL: K < 0, C < 1, S < 1 or S > D2B_POLYGON_MAX_S, V, P or G below 0.
+ *     2. K == 0: D2B_OK.
+ *     3. D2B_EINVAL: logits, boxes, loss_per_roi or targets NULL; inst_start NULL with G > 0, poly_start NULL with P > 0,
+ *        coords NULL with V > 0.
+ * No host synchronisation, no allocation: capturable in a CUDA graph. */
+#define D2B_POLYGON_MAX_S 256
+int d2b_polygons_crop_and_resize(const double* coords, int V, const int* poly_start, int P, const int* inst_start, int G,
+                                 const float* boxes, const int64_t* mask_index, int K, int S, uint8_t* out, void* stream);
+int d2b_polygons_to_bitmask(const double* coords, int V, const int* poly_start, int P, const int* inst_start, int G, int H,
+                            int W, uint8_t* out, void* stream);
+int d2b_mask_loss_polygons_forward(const float* logits, int K, int C, int S, const double* coords, int V,
+                                   const int* poly_start, int P, const int* inst_start, int G, const float* boxes,
+                                   const int64_t* mask_index, const int64_t* classes, float* loss_per_roi,
+                                   uint8_t* targets, void* stream);
+
 /* ---- Keypoint head: heatmap decoding (inference) ----------------------------------------------------------------
  * Replaces the per-detection loop of heatmaps_to_keypoints (detectron2/structures/keypoints.py:164-235), reached from
  * keypoint_rcnn_inference (modeling/roi_heads/keypoint_head.py:99-132).
