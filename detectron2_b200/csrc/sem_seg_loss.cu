@@ -141,17 +141,21 @@ __global__ void __launch_bounds__(kThreads) sem_seg_fwd_kernel(const __grid_cons
         const Tap ty = loss_tap(a.scale, a.stride, oy, a.Hp), tx = loss_tap(a.scale, a.stride, ox, a.Wp);
         const T* __restrict__ src = logits + (size_t)n * C * plane;
         float m = -INFINITY, s = 0.f, vt = 0.f;
+        bool nan = false;
         for (int c = 0; c < C; ++c) {  // online logsumexp: one exp per channel
           const float v = upsampled<DT>(src + c * plane, a.Wp, ty, tx, copy);
           if (c == (int)t) vt = v;
+          nan |= v != v;  // flagged apart from s: the first finite max resets s, whatever came before it
           if (v > m) {
             s = __fadd_rn(m == -INFINITY ? 0.f : __fmul_rn(s, __expf(__fsub_rn(m, v))), 1.f);
             m = v;
-          } else if (v != -INFINITY) {  // a NaN lands here and makes the sum NaN
+          } else if (v != -INFINITY) {
             s = __fadd_rn(s, __expf(__fsub_rn(v, m)));
           }
         }
-        lse = __fadd_rn(m, __logf(s));
+        // log_softmax's max - log(sum exp(v - max)) is NaN when a channel is NaN, or +inf (inf - inf); so is the loss and
+        // the backward's every exp(v - lse) of the pixel
+        lse = nan || m == INFINITY ? __int_as_float(0x7fc00000) : __fadd_rn(m, __logf(s));
         loss = __fsub_rn(lse, vt);
         valid = true;
       }

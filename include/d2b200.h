@@ -509,7 +509,9 @@ int d2b_panoptic_combine(const d2b_panoptic_images* img, int N, int C, const int
  *   CUDA upsample_bilinear2d with the scale factor's source scale (float)(1.0 / stride) (not h / H); stride 1 is a copy.
  *   targets [N,H,W] int64: a pixel equal to ignore_value (any int64) is skipped; another value outside [0, C) sets
  *   D2B_SEMSEG_STATUS_BAD_LABEL in status and is skipped as well (the reference raises; the loss is then unspecified).
- *   Per valid pixel p: lse(p) = logsumexp_c v_c(p), loss(p) = lse(p) - v_target(p).
+ *   Per valid pixel p: lse(p) = logsumexp_c v_c(p), loss(p) = lse(p) - v_target(p).  As in F.log_softmax, lse(p) is NaN
+ *   when some v_c(p) is NaN or +inf, and so are loss(p) and every gradient term of p; a -inf v_c(p) adds nothing to the
+ *   sum (a -inf v_target(p) gives loss(p) = +inf).
  * reduction D2B_SEMSEG_MEAN (nn.CrossEntropyLoss(reduction="mean", ignore_index)): loss_sum = sum of loss(p) over the valid
  *   pixels; weights must be NULL.  The caller's loss is loss_sum / count (NaN with no valid pixel, as torch).
  * reduction D2B_SEMSEG_TOP_K (DeepLabCE with top_k_percent_pixels in [0, 1], no class weight): the per-pixel values
