@@ -262,7 +262,9 @@ __global__ void __launch_bounds__(kThreads) keypoints_finish_kernel(const float*
 
 // ---- keypoint loss ------------------------------------------------------------------------------------------------
 // One coordinate of _keypoints_to_heatmap: floor((c - lo) * (S / (hi - lo))), where torch evaluates S / t as
-// t.reciprocal() * S; c == hi maps to S - 1.  Returns -1 when the cell is outside [0, S).
+// t.reciprocal() * S; c == hi maps to S - 1.  Returns -1 when the cell is outside [0, S).  A NaN f (a NaN coordinate, or
+// 0 * inf at c == lo of a subnormal-width box) is outside too: the reference's floor().long() gives INT64_MIN for it on
+// CUDA, so the keypoint is not valid.
 __device__ __forceinline__ int heatmap_cell(float c, float lo, float hi, int S) {
   if (c == hi) return S - 1;
   const float scale = __fmul_rn(__frcp_rn(__fsub_rn(hi, lo)), (float)S);

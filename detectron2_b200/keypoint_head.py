@@ -185,13 +185,15 @@ def _cat(ts: List[Tensor], width: Tuple[int, ...], like: Tensor) -> Tensor:
 def keypoint_rcnn_loss_fixed(pred_keypoint_logits: Tensor, gt_keypoints: List[Tensor], proposal_boxes: List[Tensor],
                              normalizer: Optional[float] = None) -> Tuple[Tensor, Tensor]:
     """Sync-free form of `keypoint_rcnn_loss` (CUDA tensors): returns (loss, num_valid) as device tensors.  Static shapes:
-    capturable in a CUDA graph."""
+    capturable in a CUDA graph.  Without a valid keypoint the loss and the gradient are 0, also when a logit is NaN or
+    infinite (the reference's pred.sum() * 0 is NaN then)."""
     k = pred_keypoint_logits.shape[1]
     kps = _cat(gt_keypoints, (k, 3), pred_keypoint_logits)
     boxes = _cat(proposal_boxes, (4,), pred_keypoint_logits)
     loss_per_kp, _, _, num_valid = keypoint_loss_op(pred_keypoint_logits, kps, boxes)
     total = loss_per_kp.sum()
-    # without valid keypoints every row's loss and gradient is 0, the value of the reference's pred.sum() * 0
+    # without valid keypoints every row's loss and gradient is 0.  The reference's pred.sum() * 0 is also 0 then, except
+    # when a logit is NaN or infinite, where it is NaN: here the loss stays 0 (no reduction over the logits only to carry it)
     if normalizer is None:
         return total / num_valid.clamp(min=1).to(total.dtype), num_valid
     return total / normalizer, num_valid
@@ -212,7 +214,9 @@ def keypoint_rcnn_loss(pred_keypoint_logits: Tensor, gt_keypoints: List[Tensor],
 
 def keypoints_to_heatmap(keypoints: Tensor, rois: Tensor, heatmap_size: int) -> Tuple[Tensor, Tensor]:
     """Keypoints.to_heatmap (structures/keypoints.py:105-161): keypoints [N, K, 3], rois [N, 4] -> (target [N, K] int64 =
-    y * S + x of the keypoint's cell, 0 where not valid; valid [N, K] int64)."""
+    y * S + x of the keypoint's cell, 0 where not valid; valid [N, K] int64).  A NaN cell (a NaN coordinate, or 0 * inf
+    at x1 of a subnormal-width box) is not valid: the reference's floor().long() gives INT64_MIN for NaN on CUDA (and on
+    x86 CPUs)."""
     if not keypoints.is_cuda:
         return _keypoints_to_heatmap_host(keypoints, rois, heatmap_size)
     _C.require_cuda(rois)

@@ -420,7 +420,8 @@ int d2b_keypoints_from_heatmaps(const float* maps, int R, int K, int S, const fl
  *   (x, y, v) matched ground truth of every proposal; boxes [N,4] fp32 proposal boxes.
  *   target [N,K] int64 = y * S + x of the keypoint's heatmap cell, 0 when not valid; valid [N,K] uint8: the cell is inside
  *   the S x S map and v > 0.  Cell: floor((c - x1) * (S / (x2 - x1))) with S / t evaluated as reciprocal(t) * S, each
- *   operation rounded on its own; c == x2 gives S - 1 (y likewise).
+ *   operation rounded on its own; c == x2 gives S - 1 (y likewise); a NaN cell (a NaN coordinate, or 0 * inf at c == x1
+ *   of a subnormal-width box) is not valid, as PyTorch's CUDA float-to-int64 conversion gives INT64_MIN for NaN.
  *   loss_per_kp [N,K] fp32: logsumexp(row) - row[target] on valid rows, 0 elsewhere; num_valid [1] int64 (zeroed inside).
  *   logits and loss_per_kp may both be NULL: the targets alone (Keypoints.to_heatmap).
  * Backward: grad_scale [N,K] fp32 = d loss / d loss_per_kp; grad_logits [N,K,S,S] of `dtype`, fully written:
